@@ -27,8 +27,6 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 D, C_PER_GPU, S, L, EPS = 1024, 256, 1000, 10, 0.05
-WARP_INST_PER_LAUNCH = 836294520           # config 2, E=4 K=1 geometry: ncu smsp__inst_executed.sum of one launch
-                                           # (profiles/r2_prof_hmc_run.summary.txt; 1076063104 before the packed fp32x2 leapfrog)
 METRIC = 'leapfrog-steps x chains / sec'
 UNIT = 'chain-steps/s'
 REFERENCE_ARM_BUDGET_S = 75.0              # wall-clock bound of `--impl reference` whatever --steps says
@@ -55,7 +53,7 @@ def measured_peak_hbm():
     p = measured_peaks()
     if 'hbm_gbs' in p:
         return float(p['hbm_gbs']), 'measured (MEASURED_PEAKS.json hbm_gbs)'
-    return 6650.0, 'fallback (B200_PROFILING.md 6.65 TB/s)'
+    return 3350.0, 'fallback (H100 SXM data sheet, 3.35 TB/s)'
 
 
 # ----------------------------------------------------------------------------------------------------------
@@ -237,7 +235,7 @@ def cpu_sample_text(host, n_iter, steps_done):
 
 
 def cpu_baseline_quick(budget_s=12.0):
-    """The cpu_baseline leg of the B200 arm: a bounded sample, forked BEFORE this process touches CUDA."""
+    """The cpu_baseline leg of the GPU arm: a bounded sample, forked BEFORE this process touches CUDA."""
     host = host_cpus()
     arm = CpuArm(host['workers'])
     try:
@@ -279,7 +277,7 @@ def run_reference_arm(args, rank, world):
             'impl': 'reference', 'metric': METRIC, 'value': value, 'unit': UNIT, 'n_gpus': args.gpus,
             'steps': args.steps, 'warmup': args.warmup, 'ms_per_step': 1e3 * t_tot / steps_done,
             'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None, 'dtype': 'f32', 'data': 'synthetic',
-            # identical to the B200 arm's `config`; what a reference step is lives in cpu_baseline.sample (independent
+            # identical to the GPU arm's `config`; what a reference step is lives in cpu_baseline.sample (independent
             # chains of config 2 through the reference's per-chain Python loop; the rate is per chain-step, so it
             # extrapolates linearly to the full 256 x 1000 job)
             'config': cfg,
@@ -483,9 +481,9 @@ def other_configs(dev, rank, world):
         integrator=hb.Integrator.SPLITTING, rng='philox', seed=3, chain_offset=rank * C4), reps=1)
     flops = 68.7e6 * C4 * S4 * 10                        # SURVEY 8d: 68.7 MFLOP per chain-step
     tf = flops / (ms * 1e-3) / 1e12
-    peak_tc = float(peaks.get('bf16_tflops_sustained', 2250.0)) / 6.0      # tf32 = bf16/2, 3 UMMAs per product
+    peak_tc = float(peaks.get('bf16_tflops_sustained', 989.0)) / 6.0       # tf32 = bf16/2, 3 MMAs per product; 989: H100 SXM data sheet
     out['config4'] = {'workload': 'BNN 64-128-1 (D=8449) regression, N=1024, M=4 symmetric split HMC, %d chains/GPU, '
-                                  'L=10, eps=5e-4, S=300' % C4, 'kernel': 'mlp_run_kernel (tcgen05 3xTF32)',
+                                  'L=10, eps=5e-4, S=300' % C4, 'kernel': 'mlp_run_kernel (wgmma 3xTF32)',
                       'bound': 'tensor', 'kernel_ms': ms, 'value': C4 * S4 * 10 / (ms * 1e-3), 'unit': UNIT,
                       'algorithmic_tflops': tf, 'roofline_frac': tf / peak_tc, 'roofline_peak_tflops': peak_tc,
                       'accept_rate': float(res.accepted.float().mean())}
@@ -514,7 +512,7 @@ def other_configs(dev, rank, world):
         tgt6, init6, num_samples=S6, num_steps_per_sample=10, step_size=0.1, explicit_binding_const=10,
         sampler=hb.Sampler.RMHMC, integrator=hb.Integrator.EXPLICIT, metric=hb.Metric.HESSIAN, rng='philox', seed=4,
         chain_offset=rank * C6), reps=3)
-    sm_clk = float(peaks.get('sm_max_mhz', 1965.0)) * 1e6
+    sm_clk = float(peaks.get('sm_max_mhz', 1980.0)) * 1e6
     smem_peak = torch.cuda.get_device_properties(dev).multi_processor_count * 128.0 * sm_clk / 1e9     # GB/s
     mv_bytes = C6 * S6 * (6 * 10 + 4) * D6 * D6 * 4.0      # every warp-matvec streams the D x D matrix once (R = 1 chain per warp)
     out['rmhmc_dense_metric_d64'] = {
@@ -528,8 +526,33 @@ def other_configs(dev, rank, world):
     return out
 
 
+DUMP_SAMPLE_ROWS = 4096                    # (chain, iteration) rows of the sample block written by --dump-outputs
+
+
+def dump_outputs(dirname, res):
+    """What the timed call returned in the last timed step for this rank's chains (rank 0's under torchrun), as DIR/<name>.npy (float32 / float64, ~20 MB): the samples
+    at the last iteration, a fixed seeded sample of DUMP_SAMPLE_ROWS rows of the whole (chains, iterations, D) block
+    (their flat row indices in samples_rows_index), the accept / divergence flags, final step sizes and reject counts.
+    The inputs of every step depend only on the command-line arguments, so two builds can be compared output for
+    output."""
+    import numpy as np
+    os.makedirs(dirname, exist_ok=True)
+    samples = res.samples
+    rows = samples.reshape(-1, samples.shape[-1])
+    idx = torch.randperm(rows.shape[0], generator=torch.Generator().manual_seed(0))[:DUMP_SAMPLE_ROWS].sort().values
+    arrays = {'samples_last': samples[:, -1].float(),
+              'samples_rows': rows[idx.to(rows.device)].float(),
+              'samples_rows_index': idx.double(),
+              'accepted': res.accepted.float(),
+              'diverged': res.diverged.float(),
+              'step_size': res.step_size.float(),
+              'num_rejected': res.num_rejected.double()}
+    for name, t in arrays.items():
+        np.save(os.path.join(dirname, name + '.npy'), t.cpu().numpy())
+
+
 # ----------------------------------------------------------------------------------------------------------
-# B200 arm
+# H100 arm
 # ----------------------------------------------------------------------------------------------------------
 def run_b200_arm(args, rank, world, local_rank):
     import torch.distributed as dist
@@ -558,7 +581,7 @@ def run_b200_arm(args, rank, world, local_rank):
 
     q0_host = init_of(rank).pin_memory()
     q0 = q0_host.to(dev)
-    out = torch.empty((C, S, ld), dtype=torch.float32, device=dev)           # 1 GiB: 8x the 126 MB L2
+    out = torch.empty((C, S, ld), dtype=torch.float32, device=dev)           # 1 GiB: 20x the 50 MB L2
     host_out, host_out_pages = pinned_host_block((C, S, ld))
     stats_local = torch.zeros((max(args.steps, args.warmup, 1), C, 2), dtype=torch.float32, device=dev)
     stats = torch.empty((world,) + tuple(stats_local.shape), dtype=torch.float32, device=dev)
@@ -597,8 +620,8 @@ def run_b200_arm(args, rank, world, local_rank):
 
     # ---- warm-up: the W requested steps, then (still untimed) until the GPU has been busy for >= 1.5 s AND the last
     #      16 steps are within 3 % of the fastest seen.  A freshly leased box ran the first ~second of launches up to
-    #      several times slower with the SM clock already reported at maximum (round-1 notes) and a 13-step warm-up (25 ms
-    #      of GPU time) left round 1's SCALE N=1 point 18 % slow; the warm-up is now bounded by GPU-busy time, not by a
+    #      several times slower with the SM clock already reported at maximum, and a warm-up of a few steps (tens of ms of
+    #      GPU time) leaves the first timed steps slow; the warm-up is therefore bounded by GPU-busy time, not by a
     #      step count.  Hard limits: 6 s / 4000 steps.
     for w in range(args.warmup):
         keep_stats(w, step(w))
@@ -639,25 +662,30 @@ def run_b200_arm(args, rank, world, local_rank):
         e_.record()
     # Python's cyclic garbage collector is parked for the timed regions: a generation-2 pass over the heap torch leaves
     # behind takes 20 - 400 ms, lands at an allocation count (deterministically in the SECOND timed step of this script:
-    # measured 19.6, 41.5 and 436 ms against 1.51 ms for every other step) and starves the launch queue.
+    # tens to hundreds of ms against ~1.5 ms for every other step) and starves the launch queue.
     gc.collect()
     gc.disable()
     barrier()
     head_start()
     ev[0].record()
-    res = None
+    res = last_res = None
     for k in range(args.steps):
         ev[1 + 2 * k].record()
         res = step(100 + k)
         ev[2 + 2 * k].record()
         keep_stats(k, res)
+        if k == args.steps - 1:
+            last_res = res
         # drop the result before the next call allocates its (small) output tensors: with two result sets alive the
         # caching allocator has to cudaMalloc a new segment inside the timed region, and cudaMalloc behind a full launch
-        # queue was measured at 7 - 436 ms (always in the second timed step) against 1.51 ms for every other step
+        # queue stalls the launch queue
         res = None
     gather_stats()
     ev[-1].record()
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_res)
+    last_res = None
     t_total_ms = ev[0].elapsed_time(ev[-1])
     step_ms = [ev[1 + 2 * k].elapsed_time(ev[2 + 2 * k]) for k in range(args.steps)]
     t_kernel_ms = sum(step_ms) / args.steps
@@ -815,9 +843,6 @@ def run_b200_arm(args, rank, world, local_rank):
         stream_bytes = Cs * D * 16                       # B_step = 16*D B per leapfrog-step x chain (SURVEY 8d)
         stream_gbs = stream_bytes / (t_stream_ms * 1e-3) / 1e9
         h2d, d2h = C * D * 4, C * S * ld * 4
-        n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
-        sm_mhz = float((clk or {}).get('sm_mhz') or 1965.0)
-        issue_peak = n_sm * 4 * sm_mhz * 1e6 / 1e9
         sorted_ms = sorted(step_ms)
         line = {
             'metric': METRIC, 'value': value, 'unit': UNIT, 'n_gpus': world, 'steps': args.steps,
@@ -825,7 +850,7 @@ def run_b200_arm(args, rank, world, local_rank):
             'vs_baseline': None, 'dtype': 'f32', 'data': 'synthetic',
             'config': workload_config(world),
             'run_notes': {'rng': 'in-kernel Philox4x32-10',
-                          'l2_policy': 'each step streams 1.0 GiB of samples (8x the 126 MB L2); no explicit flush',
+                          'l2_policy': 'each step streams 1.0 GiB of samples (20x the 50 MB L2); no explicit flush',
                           'extra_untimed_warmup_steps': extra_warmup, 'warmup_gpu_busy_ms': busy_ms,
                           'warmup_step_ms_trace': warm_trace,
                           'timed_step_ms': {'min': sorted_ms[0], 'median': sorted_ms[len(sorted_ms) // 2],
@@ -835,21 +860,10 @@ def run_b200_arm(args, rank, world, local_rank):
                                     'bit-exact under the reference step-size schedule (teacher forcing); configs 3/4: see '
                                     'DESIGN.md section 4 for the measured tolerances'},
             'roofline': {'bound': 'hbm', 'kernel': 'hmc_run_kernel<ISO,NONE,E=4,K=1,PHILOX,NUTS=0>', 'achieved': achieved, 'peak': peak,
-                         'unit': 'GB/s', 'frac': achieved / peak,
-                         # dram__bytes_read.sum + dram__bytes_write.sum of one launch, ncu --set full capture
-                         # profiles/r2_prof_hmc_run.summary.txt (1.20 MB read + 989.99 MB written)
-                         'traffic': 991.2e6, 'peak_source': peak_src,
+                         'unit': 'GB/s', 'frac': achieved / peak, 'peak_source': peak_src,
                          'algorithmic_bytes_per_launch': algo_bytes, 'kernel_ms': t_kernel_ms,
                          'note': 'fused trajectory kernel: L=10 steps per 4*D bytes written, fp32-issue bound by design; '
                                  'see roofline_streaming for the HBM-bound form'},
-            # what actually bounds the fused kernel: warp-instruction issue.  Instructions per launch are static for this
-            # geometry (ncu smsp__inst_executed.sum, profiles/r2_prof_hmc_run.summary.txt); time is measured live.
-            'roofline_issue': {'bound': 'issue', 'kernel': 'hmc_run_kernel<ISO,NONE,E=4,K=1>',
-                               'warp_instructions_per_launch': WARP_INST_PER_LAUNCH,
-                               'achieved': WARP_INST_PER_LAUNCH / (t_kernel_ms * 1e-3) / 1e9,
-                               'peak': issue_peak, 'unit': 'G warp-inst/s',
-                               'frac': WARP_INST_PER_LAUNCH / (t_kernel_ms * 1e-3) / 1e9 / issue_peak,
-                               'peak_source': '%d SMs x 4 schedulers x %.0f MHz (sampled under load)' % (n_sm, sm_mhz)},
             'roofline_streaming': {'bound': 'hbm', 'kernel': 'leapfrog_kernel<ISO,NONE> L=1, 32768x1024 state',
                                    'achieved': stream_gbs, 'peak': peak, 'unit': 'GB/s', 'frac': stream_gbs / peak,
                                    'algorithmic_bytes_per_launch': stream_bytes, 'kernel_ms': t_stream_ms,
@@ -914,7 +928,11 @@ def main():
                     help='N > 1: skip the timed all-gather of every step\'s samples (value_with_gather)')
     ap.add_argument('--no-other-configs', action='store_true', help='skip BASELINE configs 3 / 4 / 5')
     ap.add_argument('--no-numa-bind', action='store_true')
+    ap.add_argument('--dump-outputs', metavar='DIR', default=None,
+                    help='after the timed steps, write the last timed step\'s outputs (rank 0\'s chains) to DIR/<name>.npy')
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error('--steps must be at least 1')
     rank = int(os.environ.get('RANK', '0'))
     world = int(os.environ.get('WORLD_SIZE', '1'))
     local_rank = int(os.environ.get('LOCAL_RANK', '0'))

@@ -1,4 +1,4 @@
-"""hamiltorch_b200 -- a B200-native (sm_100a) batched-chain HMC engine behind the hamiltorch surface.
+"""hamiltorch_b200 -- an H100-native (sm_90a) batched-chain HMC engine behind the hamiltorch surface.
 
 Exports the same names as the reference's ``hamiltorch/__init__.py:1-4`` plus the engine's native additions
 (``targets``, ``sample_chains``).  The CUDA library is loaded lazily by the first sampling call and that call

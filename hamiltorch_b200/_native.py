@@ -140,7 +140,7 @@ def load_library():
     if not os.path.exists(LIB_PATH):
         raise NativeError(
             'hamiltorch_b200: %s not found.  Build it with `python -m hamiltorch_b200.build` (needs nvcc, '
-            'cross-compiles sm_100a without a GPU).  There is no CPU fallback.' % LIB_PATH)
+            'cross-compiles sm_90a without a GPU).  There is no CPU fallback.' % LIB_PATH)
     lib = C.CDLL(LIB_PATH)
     for name, (res, args) in _PROTOS.items():
         fn = getattr(lib, name)          # AttributeError here = header/library mismatch
@@ -154,7 +154,7 @@ def load_library():
 
 def require_cuda():
     if not torch.cuda.is_available():
-        raise NativeError('hamiltorch_b200 needs a CUDA device (sm_100a); there is no CPU fallback. '
+        raise NativeError('hamiltorch_b200 needs a CUDA device (sm_90a); there is no CPU fallback. '
                           'The CPU restatement under oracle/ is test infrastructure only.')
 
 

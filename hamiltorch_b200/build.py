@@ -1,8 +1,8 @@
-"""Build libhmcx.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libhmcx.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python -m hamiltorch_b200.build [--force] [--verbose]
 
-The .so is git-ignored (history stays source-only) but travels to the GPU box with the repo snapshot.
+The .so is git-ignored (history stays source-only) but is rebuilt by `__graft_entry__.build()` on every checkout.
 """
 import glob
 import os
@@ -14,8 +14,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB_DIR = os.path.join(HERE, 'lib')
 LIB = os.path.join(LIB_DIR, 'libhmcx.so')
+LIB_FLAGS = LIB + '.flags'          # the nvcc flags (architecture included) the library was built with
 
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
               '--fmad=false',          # parity arithmetic: never contract a*b+c (see hmcx_common.cuh)
               '-Xcompiler', '-fPIC']
 
@@ -40,12 +41,19 @@ def _obj_of(src):
     return os.path.join(LIB_DIR, 'obj', os.path.basename(src)[:-3] + '.o')
 
 
+def _flags():
+    return NVCC_FLAGS + os.environ.get('HMCX_NVCC_EXTRA', '').split()
+
+
 def up_to_date():
-    """The library is newer than every object, and every object is newer than its source and the shared headers
-    (a source edited while a build was running is therefore rebuilt next time; a fresh checkout with only the .so
-    -- the GPU box -- counts as up to date)."""
-    if not os.path.exists(LIB):
+    """The library was built with the current flags (so one built for another architecture is rebuilt), it is newer
+    than every source and header, and every object is newer than its source and the shared headers (a source edited
+    while a build was running is therefore rebuilt next time)."""
+    if not os.path.exists(LIB) or not os.path.exists(LIB_FLAGS):
         return False
+    with open(LIB_FLAGS) as f:
+        if f.read() != ' '.join(_flags()):
+            return False
     t = os.path.getmtime(LIB)
     if not all(os.path.getmtime(f) <= t for f in _deps()):
         return False
@@ -66,7 +74,7 @@ def build(force=False, verbose=False):
     os.makedirs(obj_dir, exist_ok=True)
     nvcc = _nvcc()
     procs, objs = [], []
-    flags = NVCC_FLAGS + os.environ.get('HMCX_NVCC_EXTRA', '').split()
+    flags = _flags()
     stamp = ' '.join(flags)
     common = [f for f in _deps() if not f.endswith('.cu')]
     for src in sources():
@@ -88,8 +96,10 @@ def build(force=False, verbose=False):
         with open(flagfile, 'w') as f:
             f.write(stamp)
     tmp = LIB + '.tmp'
-    subprocess.check_call([nvcc, '-shared', '-o', tmp] + objs + ['-gencode', 'arch=compute_100a,code=sm_100a'])
+    subprocess.check_call([nvcc, '-shared', '-o', tmp] + objs + ['-gencode', 'arch=compute_90a,code=sm_90a'])
     os.replace(tmp, LIB)
+    with open(LIB_FLAGS, 'w') as f:
+        f.write(stamp)
     return LIB
 
 

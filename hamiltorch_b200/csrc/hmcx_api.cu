@@ -121,7 +121,7 @@ int hmcx_hmc_run_sink(const hmcx_target_t* target, const hmcx_mass_t* mass, cons
                                   num_rejected, tuning, workspace, sink, (cudaStream_t)stream);
     if (sink) return HMCX_ERR_UNSUPPORTED;
     if (target->dim > 16 && (target->kind == HMCX_TARGET_GAUSS_FULL || (full_mass && is_elem(target))))
-        // dense target and / or full mass matrix at scale: tcgen05 GEMMs over all chains per leapfrog step (hmcx_tc.cu)
+        // dense target and / or full mass matrix at scale: tensor-core GEMMs over all chains per leapfrog step (hmcx_tc.cu)
         return hmcx::dense_hmc_run(target, mass, rng, nuts, q_init, q_cur, eps, C, ld, L, num_samples, burn,
                                    iter_begin, iter_end, samples_out, accept_out, diverged_out, ham_out,
                                    num_rejected, workspace, (cudaStream_t)stream);

@@ -1,4 +1,4 @@
-// hmcx_common.cuh -- device helpers shared by the sm_100a HMC kernels.
+// hmcx_common.cuh -- device helpers shared by the sm_90a HMC kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -9,11 +9,11 @@
 // L leapfrog steps, MH, bookkeeping, dual averaging -- stays inside one launch: a warp owns R chains (state in registers,
 // lane j holds elements j, j+32, ...), reads each matrix row once from shared memory for its R chains (conflict-free:
 // the matrices are stored transposed, lane <-> column) and accumulates in exact fp32 FMAs.  This replaces, for small D,
-// the step-synchronous tcgen05 path of hmcx_tc.cu (8L+3 GEMM launches of ~9 us per iteration at D = 64: launch-latency
+// the step-synchronous tensor-core path of hmcx_tc.cu (8L+3 GEMM launches of ~9 us per iteration at D = 64: launch-latency
 // bound, tensor pipe 3 %) -- the contraction is 128 x 64 x 64 per tile, far below what feeds a tensor core, so the honest
 // roofline here is shared-memory bandwidth (each warp-matvec streams the D*D*4-byte matrix once: 128 B/clk/SM).
 // Same random streams (Philox keyed by global chain id / iteration, or injected), same bookkeeping and the same
-// element-wise operation order as the tcgen05 path, so both give the same chains up to the summation order of the
+// element-wise operation order as the tensor-core path, so both give the same chains up to the summation order of the
 // contractions.
 #include <cstdlib>
 #include "hmcx_common.cuh"
@@ -485,14 +485,14 @@ __global__ void __launch_bounds__(256, 1) flow_small_kernel(const FlowArgs a) {
 }
 
 static int flow_threads_and_grid(int C, int D, size_t matrix_bytes, int& R, int& threads, int& grid) {
-    int sms = 148;
+    int sms = 132;
     int dev = 0;
     if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     // chains per warp: every warp-matvec streams the whole matrix from shared memory once, so more chains per warp = less
     // shared-memory traffic per chain, fewer chains per warp = more warps (SMs) working on a small batch
     const char* fr = getenv("HMCX_FLOW_R");
     if (fr && (atoi(fr) == 1 || atoi(fr) == 2 || atoi(fr) == 4)) R = atoi(fr);
-    else R = (C <= 4 * sms) ? 1 : (C <= 12 * sms) ? 2 : 4;        // measured: C = 512 -> 1, C >= 4096 -> 4 (profiles/r2_flow_small.txt)
+    else R = (C <= 4 * sms) ? 1 : (C <= 12 * sms) ? 2 : 4;
     const int warps = (C + R - 1) / R;
     int w = (warps + sms - 1) / sms;
     // big batches: when two CTAs' matrices fit one SM, CTAs of 4 warps (finer waves, the same warps per SM); D = 128 with
@@ -537,7 +537,7 @@ static int flow_launch(const FlowArgs& a, cudaStream_t st) {
 }
 
 // The persistent kernel covers D <= 128 with the row stride inside its padded width; HMCX_FLOW_SMALL=0 keeps everything
-// on the tcgen05 path (A/B measurements, tests of that path at small D).
+// on the tensor-core path (A/B measurements, tests of that path at small D).
 bool flow_small_ok(int D, int ld) {
     const char* s = getenv("HMCX_FLOW_SMALL");
     if (s && s[0] == '0') return false;

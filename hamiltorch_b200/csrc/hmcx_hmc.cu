@@ -1,4 +1,4 @@
-// hmcx_hmc.cu -- plain-HMC hot path for element-wise targets (isotropic / diagonal Gaussians) on sm_100a.
+// hmcx_hmc.cu -- plain-HMC hot path for element-wise targets (isotropic / diagonal Gaussians) on sm_90a (H100).
 //
 // Replaces, for a batch of C independent chains, the reference's per-chain Python loop
 //   samplers.py:965-1067  (sample: gibbs -> hamiltonian -> leapfrog -> hamiltonian -> MH -> bookkeeping -> adaptation)
@@ -30,24 +30,7 @@ struct ElemTarget {           // element-wise target + mass description, passed 
     float log_norm;
     uint32_t vpr_magic;       // ceil(2^vpr_shift / (ld/4)): row = (v * magic) >> shift for v < 2^31 (Granlund-Montgomery)
     int vpr_shift;
-    float one, mone;          // +1 / -1 as RUNTIME values (see add2 below): ptxas must not know them
 };
-
-// ---------------------------------------------------------------------------------------------------------
-// Packed fp32x2 arithmetic (sm_100: FMUL2 / FFMA2, two IEEE fp32 lanes per instruction = half the issue slots of the
-// leapfrog chain, each lane rounded exactly like the scalar op).  ptxas contracts `mul.rn.f32x2` + `add.rn.f32x2` into
-// one FFMA2 EVEN with --fmad=false (checked in SASS), which would break the reference's separately-rounded
-// ``q + eps*p``.  The add is therefore issued as fma(t, ONE, a) with ONE = 1.0f a kernel argument the assembler cannot
-// fold: t*1 is exact, so the result is round(a + t) -- bit-identical to the scalar __fadd_rn -- and a product feeding
-// it cannot be contracted.  a - t is fma(t, -1, a).
-// ---------------------------------------------------------------------------------------------------------
-typedef unsigned long long f32x2;
-__device__ __forceinline__ f32x2 pk2(float lo, float hi) { f32x2 r; asm("mov.b64 %0, {%1,%2};" : "=l"(r) : "f"(lo), "f"(hi)); return r; }
-__device__ __forceinline__ void unpk2(f32x2 v, float& lo, float& hi) { asm("mov.b64 {%0,%1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-__device__ __forceinline__ f32x2 mul2(f32x2 a, f32x2 b) { f32x2 r; asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b)); return r; }
-__device__ __forceinline__ f32x2 fma2(f32x2 a, f32x2 b, f32x2 c) {
-    f32x2 r; asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c)); return r;
-}
 
 // per-group constants kept in registers (dead members are eliminated for ISO / MASS_NONE)
 template <int E>
@@ -98,60 +81,10 @@ __device__ __forceinline__ float kterm1(float p, float im) {
 // log p from the reduced sum, targets.py op order: -0.5*sum (+ log_norm)
 __device__ __forceinline__ float log_prob_from_sum(float s, float log_norm) { return add(mul(-0.5f, s), log_norm); }
 
-// The same trajectory on packed pairs (E/2 f32x2 lanes): every product and every sum is rounded exactly as in the scalar
-// form below (see the note at f32x2), so the results are bit-identical; half the FP32 issue slots.
-//   kick  p + c*g with g = -w  ==  p - (c*w)   (c*(-w) == -(c*w) exactly), w = q (ISO) or ivar*(q - mean) (DIAG)
-template <int TK, int MK, int E>
-__device__ __forceinline__ void trajectory_packed(float* q, float* p, const VecConst<E>& c, float eps, float half, int L,
-                                                  float one, float mone) {
-    constexpr int H = E / 2;
-    const f32x2 ONE = pk2(one, one), MONE = pk2(mone, mone), EPS = pk2(eps, eps), HALF = pk2(half, half);
-    f32x2 Q[H], P[H], W[H], MEAN[H], IVAR[H], EI[H];
-#pragma unroll
-    for (int h = 0; h < H; ++h) {
-        Q[h] = pk2(q[2 * h], q[2 * h + 1]);
-        P[h] = pk2(p[2 * h], p[2 * h + 1]);
-        if (TK == HMCX_TARGET_GAUSS_DIAG) {
-            MEAN[h] = pk2(c.mean[2 * h], c.mean[2 * h + 1]);
-            IVAR[h] = pk2(c.ivar[2 * h], c.ivar[2 * h + 1]);
-        }
-        if (MK == HMCX_MASS_DIAG) EI[h] = mul2(EPS, pk2(c.im[2 * h], c.im[2 * h + 1]));       // mul(eps, im), :296
-    }
-    auto grad_w = [&](int h) {                         // W = -g
-        if (TK == HMCX_TARGET_GAUSS_ISO) W[h] = Q[h];
-        else W[h] = mul2(IVAR[h], fma2(MEAN[h], MONE, Q[h]));
-    };
-#pragma unroll
-    for (int h = 0; h < H; ++h) { grad_w(h); P[h] = fma2(mul2(HALF, W[h]), MONE, P[h]); }           // :281
-    auto one_step = [&]() {
-#pragma unroll
-        for (int h = 0; h < H; ++h) {
-            Q[h] = fma2(mul2(MK == HMCX_MASS_DIAG ? EI[h] : EPS, P[h]), ONE, Q[h]);               // :284 / :296
-            grad_w(h);                                                                             // :297
-            P[h] = fma2(mul2(EPS, W[h]), MONE, P[h]);                                              // :298
-        }
-    };
-    int l = 0;
-#pragma unroll 1
-    for (; l + 2 <= L; l += 2) { one_step(); one_step(); }
-    if (l < L) one_step();
-#pragma unroll
-    for (int h = 0; h < H; ++h) {
-        P[h] = fma2(mul2(HALF, W[h]), ONE, P[h]);                                                  // :302  p - half*g
-        unpk2(Q[h], q[2 * h], q[2 * h + 1]);
-        unpk2(P[h], p[2 * h], p[2 * h + 1]);
-    }
-}
-
 // One group of E elements through a whole trajectory (samplers.py:281-302).  Optionally records the L clones.
 template <int TK, int MK, int E, bool TRAJ>
 __device__ __forceinline__ void trajectory(float* q, float* p, const VecConst<E>& c, float eps, float half, int L,
-                                           float* q_traj, float* p_traj, size_t traj_stride, float one = 1.0f,
-                                           float mone = -1.0f) {
-    if (!TRAJ && (E % 2) == 0) {                       // `one` / `mone`: +-1.0f as run-time values (fill_elem_target)
-        trajectory_packed<TK, MK, E>(q, p, c, eps, half, L, one, mone);
-        return;
-    }
+                                           float* q_traj, float* p_traj, size_t traj_stride) {
     float g[E];
 #pragma unroll
     for (int j = 0; j < E; ++j) {
@@ -265,9 +198,8 @@ __device__ __forceinline__ void block_sum3_small(float& a, float& b, float& c, f
 
 // ---------------------------------------------------------------------------------------------------------
 // Thread-block clusters: one chain spread over CS CTAs (SMs) -- finer-grained work units for launches with few chains
-// (BASELINE config 2: 256 chains on 148 SMs), so that every SM holds several independent CTAs whose latencies overlap.
-// MEASURED on B200 (config 2, profiles/README.md r1h): the cluster barrier + DSMEM round trip per iteration costs more
-// than the finer granularity buys -- 2.08 ms (CS=2) and 2.7-3.5 ms (CS=4) against 1.63 ms for one CTA per chain -- so this
+// (BASELINE config 2: 256 chains on 132 SMs), so that every SM holds several independent CTAs whose latencies overlap.
+// At config 2 the cluster barrier + DSMEM round trip per iteration costs more than the finer granularity buys, so this
 // form is opt-in (tuning 41 / 42), kept as the tested starting point for single-chain / few-chain launches where one
 // SM per chain leaves the GPU idle.
 // The chain's only cross-thread traffic, the per-iteration reduction, goes through DISTRIBUTED SHARED MEMORY: every
@@ -475,7 +407,7 @@ hmc_run_kernel(const RunArgs a) {
         // ---- leapfrog (:973) : thread-private ----
 #pragma unroll
         for (int k = 0; k < K; ++k)
-            trajectory<TK, MK, E, false>(q[k], p[k], vc[k], eps, half, a.L, nullptr, nullptr, 0, t.one, t.mone);
+            trajectory<TK, MK, E, false>(q[k], p[k], vc[k], eps, half, a.L, nullptr, nullptr, 0);
         // ---- both Hamiltonians with one fused reduction (:971, :995) ----
         float r0 = kin0, r1 = 0.0f, r2 = 0.0f;
 #pragma unroll
@@ -682,7 +614,7 @@ hmc_run_big_kernel(const RunArgs a, float* __restrict__ work) {
                 p[j] = (MK == HMCX_MASS_DIAG) ? mul(z[j], vc.sd[j]) : z[j];
                 r0 = add(r0, kterm1<MK>(p[j], vc.im[j]));
             }
-            trajectory<TK, MK, 4, false>(q, p, vc, eps, half, a.L, nullptr, nullptr, 0, a.t.one, a.t.mone);
+            trajectory<TK, MK, 4, false>(q, p, vc, eps, half, a.L, nullptr, nullptr, 0);
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 r1 = add(r1, uterm1<TK>(q[j], vc.mean[j], vc.ivar[j]));
@@ -782,7 +714,7 @@ leapfrog_kernel(const ElemTarget t, const float* __restrict__ q_in, const float*
             if (e0 + j >= t.D) { q[j] = 0.0f; p[j] = 0.0f; }
         const float eps = eps_c[c];
         trajectory<TK, MK, 4, TRAJ>(q, p, vc, eps, mul(0.5f, eps), L, TRAJ ? q_traj + 4 * v : nullptr,
-                                    TRAJ ? p_traj + 4 * v : nullptr, traj_stride, t.one, t.mone);
+                                    TRAJ ? p_traj + 4 * v : nullptr, traj_stride);
         st4_stream(q_out + 4 * v, q);
         st4_stream(p_out + 4 * v, p);
     }
@@ -857,14 +789,13 @@ static int fill_elem_target(const hmcx_target_t* target, const hmcx_mass_t* mass
     }
     t.mean = target->mean; t.ivar = target->inv_var; t.log_norm = target->log_norm;
     t.im = mass ? mass->inv_mass : nullptr; t.sd = mass ? mass->mass_factor : nullptr;
-    t.one = 1.0f; t.mone = -1.0f;
     return HMCX_OK;
 }
 
 static inline int cuda_status() { return cudaGetLastError() == cudaSuccess ? HMCX_OK : HMCX_ERR_CUDA; }
 
 static int sm_count() {
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     return sms;
@@ -933,16 +864,16 @@ int elem_gibbs(const hmcx_mass_t* mass, const hmcx_rng_t* rng, int D, int C, int
 }
 
 // Register-resident geometry (one CTA per chain): each thread owns K groups of E contiguous elements.
-//   tuning 0 (auto): one float4 per thread (E=4,K=1) for D <= 2560, two (K=2) above.  Measured on B200: at BASELINE
-//                    config 2 (D=1024) the per-warp fixed cost of an iteration (reduction, loop, RNG for the MH test)
-//                    makes both thinner threads (E=2: 2.25 ms) and fatter threads (K=2: 2.14, K=4: 3.6 ms) slower than
-//                    float4 (1.94 ms); at D >= 3072 (config 5: D=4096) CTAs of 768-1024 threads lose 5-9 % to 512 x 2.
+//   tuning 0 (auto): one float4 per thread (E=4,K=1) for D <= 2560, two (K=2) above.  At BASELINE config 2 (D=1024)
+//                    the per-warp fixed cost of an iteration (reduction, loop, RNG for the MH test) makes both thinner
+//                    threads (E=2) and fatter threads (K=2, K=4) slower than float4; at D >= 3072 (config 5: D=4096)
+//                    CTAs of 768-1024 threads are slower than 512 x 2.
 //   tuning 1: E=4, K=1 forced.
 //   tuning 2 / 4: E=4 with K = 2 / 4 groups per thread;  21: E=2,K=1 (D <= 2048);  22: E=2,K=2.
 static bool pick_geometry(int ld, int tuning, int& E, int& K, int& G) {
     if (ld > 4096) return false;
-    if (tuning == 0) { E = 4; K = ld > 2560 ? 2 : 1; }       // measured (scripts/sweep_nuts.py): D >= 3072 runs 5-9 % faster
-    else if (tuning == 1) { E = 4; K = 1; }                  // with 512 threads x 2 float4 than with 768-1024 x 1
+    if (tuning == 0) { E = 4; K = ld > 2560 ? 2 : 1; }       // D >= 3072: 512 threads x 2 float4 beat 768-1024 x 1
+    else if (tuning == 1) { E = 4; K = 1; }
     else if (tuning == 21) { E = 2; K = 1; }
     else if (tuning == 2 || tuning == 4) { E = 4; K = tuning; }
     else if (tuning == 22) { E = 2; K = 2; }

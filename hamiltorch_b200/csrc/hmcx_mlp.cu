@@ -1,4 +1,4 @@
-// hmcx_mlp.cu -- Bayesian dense-stack (MLP) HMC on sm_100a: the BNN rows of the hot path.
+// hmcx_mlp.cu -- Bayesian dense-stack (MLP) HMC on sm_90a (H100): the BNN rows of the hot path.
 //
 //   define_model_log_prob / define_split_model_log_prob   samplers.py:1093-1258  -> mlp_log_prob(), mlp_grad_split()
 //   leapfrog SPLITTING / SPLITTING_RAND / SPLITTING_KMID  samplers.py:465-603    -> trajectory in mlp_run_kernel
@@ -6,7 +6,7 @@
 //   predict_model                                          samplers.py:1468-1562  -> mlp_predict_kernel
 //   collect_gradients (autograd) is replaced by a hand-written backward pass      -> mlp_grad_split()
 //
-// Design (round 1, fp32 SIMT; the tensor-core batched-over-chains form is the next step, DESIGN.md 3.4):
+// Design of the fp32 SIMT form (the tensor-core first layer is further below, DESIGN.md 3.4):
 // one CTA of 256 threads owns one chain for the whole run.  The chain's flat parameter vector q, its momentum p and
 // the split gradient g live in SHARED MEMORY in the reference's flat layout (util.py:121-136), so every weight is
 // read from smem by the GEMM loops and the leapfrog kick/drift are conflict-free element-wise passes.  A gradient
@@ -17,7 +17,7 @@
 // sgemm order is unknowable); everything element-wise (kicks, drifts, prior, Hamiltonian assembly, MH) keeps the
 // reference's separately-rounded fp32 operation order.
 #include "hmcx_common.cuh"
-#include "hmcx_umma.cuh"
+#include "hmcx_wgmma.cuh"
 #include <cooperative_groups.h>
 
 namespace cg = cooperative_groups;
@@ -37,7 +37,7 @@ struct MlpDev {
     int tile_floats;
     int tile_base;                        // float offset of the tile area in dynamic shared memory (after the state vectors)
     int T;                                // rows per tile (multiple of 4)
-    int tc;                               // 1: the first layer's GEMMs run on tcgen05 (layout below), 0: SIMT tiles
+    int tc;                               // 1: the first layer's GEMMs run on the tensor cores (layout below), 0: SIMT tiles
     int tc_f0, tc_f1, tc_b, tc_part;      // tile-area offsets (floats): two forward X operand buffers, the backward one, partials
     int tc_yraw;                          // cp.async landing buffer of the tile's targets
     const float* xp;                      // packed X operands (hmcx_mlp_pack_x): per tile [fwd hi|lo (128 n0) | bwd hi|lo (128 n0)]
@@ -433,30 +433,31 @@ __device__ __forceinline__ float cluster_sum_scalar(float x, float* slot) {
 
 
 // =========================================================================================================
-// First-layer GEMMs on the 5th-generation tensor cores (tcgen05 / TMEM), for one-hidden-layer stacks
+// First-layer GEMMs on the Hopper tensor cores (wgmma, fp32 accumulators in registers), for one-hidden-layer stacks
 //   n0 -> 128 -> nL   (n0 in {16,32,48,64}, nL <= 4; BASELINE config 4 is 64-128-1)
-// where  H = X W1^T  (forward) and  dW1 = dH^T X  (backward) carry ~all of the flops.  Per 64-row tile of the split:
-//   forward, TRANSPOSED:  H^T[128 units x 64 rows] = W1[128 x n0] . X_tile^T   -- A = W1 (shared memory, K-major,
-//       packed from the flat q at the start of every evaluation), B = X tile (staged from global memory), fp32
-//       accumulators in TENSOR MEMORY; 3xTF32 split operands (hi*hi + hi*lo + lo*hi) keep fp32-level accuracy;
-//   epilogue 1: each thread owns ONE hidden unit (TMEM lane) and 16 rows (columns): bias + activation in registers,
-//       the thin output layer as an in-warp transpose-reduction -> z2 in shared memory -> the usual loss stage;
-//   epilogue 2: dH^T = (W2^T dz2) * act'(H) computed in the same registers; db1 and dW2 are THREAD-LOCAL sums in this
-//       orientation; dH^T is written back to TENSOR MEMORY (tcgen05.st) as tf32 hi / lo;
-//   backward:  dW1[128 x n0] += dH^T[128 x 64 rows] . X_tile  with the A operand read FROM TENSOR MEMORY and
-//       B = X tile re-staged rows-contiguous; the accumulator stays in TMEM across all tiles of the split.
-// The big activations never touch shared memory.  Everything around (prior, schedules, kicks, drifts, Hamiltonians,
-// MH, clusters) is the code of the SIMT path.
+// where  H = X W1^T  (forward) and  dW1 = dH^T X  (backward) carry ~all of the flops.  Per 64-row tile of the split the
+// CTA's four warpgroups split the work 2 x 2: warpgroup wg takes hidden units [64 (wg & 1), +64) and tile rows
+// [32 (wg >> 1), +32):
+//   forward, TRANSPOSED:  H^T[64 units x 32 rows] = W1[64 x n0] . X_rows^T  -- A = W1 as register fragments read from the
+//       chain's q in shared memory, B = the X tile (bulk TMA copy of a pre-packed operand); 3xTF32 split operands
+//       (hi*hi + hi*lo + lo*hi) keep fp32-level accuracy;
+//   epilogue 1: bias + activation on the accumulator fragments (two units x 8 rows per thread), the thin output layer
+//       as shuffle sums over the units -> z2 in shared memory -> the usual loss stage;
+//   epilogue 2: dH^T = (W2^T dz2) * act'(H) in the same registers; db1 and dW2 are thread-local sums;
+//   backward:  dW1[64 units x n0] += dH^T[64 x 32 rows] . X_rows  with dH^T's fragments used AS the A operand
+//       (registers, no shared-memory round trip); the accumulators stay in registers across all tiles of the split and
+//       the two row halves are added once per evaluation.
+// The contraction index of each GEMM is stored in a permuted order in the packed X operands (tc_kpos_fwd / tc_row_bwd)
+// so that every A fragment is a plain float4 of W1 (forward) or a set of accumulator registers (backward).  Everything
+// around (prior, schedules, kicks, drifts, Hamiltonians, MH, clusters) is the code of the SIMT path.
 // =========================================================================================================
 constexpr int TC_TR = 64;                 // data rows per tile (MMA N forward, MMA K backward)
-constexpr int TC_H = 128;                 // hidden units = MMA M = TMEM lanes
+constexpr int TC_H = 128;                 // hidden units
 constexpr int TC_NLMAX = 4;               // outputs handled by the register head
-// TMEM columns: H hh / dH hi | H hl / dH lo | dW1 hh | dW1 hl | W1 hi | W1 lo (the forward A operand, written once per evaluation)
-constexpr int TC_COL_H = 0, TC_COL_LO = 64, TC_COL_W = 128, TC_COL_W1HI = 256, TC_COL_W1LO = 320, TC_COLS = 512;
 
-static_assert(TC_TR / 4 == MLP_THREADS / 32 && TC_TR == 64, "staging / epilogue thread maps assume 16 warps and 64-row tiles");
+static_assert(TC_TR / 4 == MLP_THREADS / 32 && TC_TR == 64, "the thread maps assume 16 warps and 64-row tiles");
 
-struct TcCtx { uint32_t tmem, barH, barW, barF[2], barB, parH, parW, parF[2], parB; int pre_id; };   // pre_id: tile whose operands an earlier evaluation already prefetched (-1: none)
+struct TcCtx { uint32_t barF[2], barB, parF[2], parB; int pre_id; };   // pre_id: tile whose operands an earlier evaluation already prefetched (-1: none)
 
 #ifdef HMCX_TC_PROF
 __device__ long long g_tc_prof[512];
@@ -466,30 +467,15 @@ __device__ int g_tc_prof_n;
 #define TC_MARK(id) do {} while (0)
 #endif
 
-__device__ __forceinline__ void tc_init(TcCtx& tc, uint64_t* bars, uint32_t* slot) {
+__device__ __forceinline__ void tc_init(TcCtx& tc, uint64_t* bars) {
     if (threadIdx.x == 0) {
-        for (int b = 0; b < 5; ++b) mbar_init(smem_u32(&bars[b]), 1);
+        for (int b = 0; b < 3; ++b) mbar_init(smem_u32(&bars[b]), 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (threadIdx.x < 32) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(slot)), "r"(TC_COLS));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    tc.tmem = *slot;
-    tc.barH = smem_u32(&bars[0]);
-    tc.barW = smem_u32(&bars[1]);
-    tc.barF[0] = smem_u32(&bars[2]); tc.barF[1] = smem_u32(&bars[3]); tc.barB = smem_u32(&bars[4]);
-    tc.parH = tc.parW = tc.parF[0] = tc.parF[1] = tc.parB = 0;
+    tc.barF[0] = smem_u32(&bars[0]); tc.barF[1] = smem_u32(&bars[1]); tc.barB = smem_u32(&bars[2]);
+    tc.parF[0] = tc.parF[1] = tc.parB = 0;
     tc.pre_id = -1;
-}
-__device__ __forceinline__ void tc_fini(const TcCtx& tc) {
-    tc_fence_before();
-    __syncthreads();
-    if (threadIdx.x < 32)
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tc.tmem), "r"(TC_COLS));
 }
 
 // round-to-nearest (ties away) tf32 in an fp32 container == cvt.rna.tf32.f32 for finite inputs, as two full-rate
@@ -497,65 +483,30 @@ __device__ __forceinline__ void tc_fini(const TcCtx& tc) {
 __device__ __forceinline__ float tf32_rn(float x) {
     return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
 }
-__device__ __forceinline__ void tc_split4(const float4 v, float4& h, float4& l) {
-    h.x = tf32_rn(v.x); h.y = tf32_rn(v.y); h.z = tf32_rn(v.z); h.w = tf32_rn(v.w);
-    l.x = tf32_rn(v.x - h.x); l.y = tf32_rn(v.y - h.y); l.z = tf32_rn(v.z - h.z); l.w = tf32_rn(v.w - h.w);
-}
-
-// q's W1 (flat, row-major 128 x n0) -> the forward A operand IN TENSOR MEMORY (lane = hidden unit, one 32-bit column per
-// input k), tf32 hi and lo: thread (unit u, column group cq) owns 16 consecutive k of row u.  The four float4 chunks are
-// read in a per-lane rotated order (2-way instead of 8-way bank conflicts on the stride-n0 rows) and rotated back in
-// registers.  Keeping W1 out of shared memory frees 64 KB for the X operand pipeline.
-__device__ __forceinline__ void tc_pack_w1(const MlpDev& m, const float* q, const TcCtx& tc) {
-    const int n0 = m.n[0], warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int lq = warp & 3, cq = warp >> 2, u = 32 * lq + lane;
-    if (16 * cq < n0) {
-        const float* W = q + m.woff[0] + u * n0 + 16 * cq;
-        float4 t[4], a[4], o[4];
+__device__ __forceinline__ void tc_split(const float (&v)[4], uint32_t (&hi)[4], uint32_t (&lo)[4]) {
 #pragma unroll
-        for (int j = 0; j < 4; ++j) t[j] = *reinterpret_cast<const float4*>(W + 4 * ((j + lane) & 3));
-        // t[j] holds chunk (j + lane) & 3, i.e. chunk c sits in t[(c - lane) & 3]: rotate right by lane & 3
-        const bool r1 = lane & 1, r2 = lane & 2;
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-            a[c].x = r1 ? t[(c + 3) & 3].x : t[c].x; a[c].y = r1 ? t[(c + 3) & 3].y : t[c].y;
-            a[c].z = r1 ? t[(c + 3) & 3].z : t[c].z; a[c].w = r1 ? t[(c + 3) & 3].w : t[c].w;
-        }
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-            o[c].x = r2 ? a[(c + 2) & 3].x : a[c].x; o[c].y = r2 ? a[(c + 2) & 3].y : a[c].y;
-            o[c].z = r2 ? a[(c + 2) & 3].z : a[c].z; o[c].w = r2 ? a[(c + 2) & 3].w : a[c].w;
-        }
-        uint32_t hi[16], lo[16];
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-            float4 h, l;
-            tc_split4(o[c], h, l);
-            hi[4 * c] = __float_as_uint(h.x); hi[4 * c + 1] = __float_as_uint(h.y);
-            hi[4 * c + 2] = __float_as_uint(h.z); hi[4 * c + 3] = __float_as_uint(h.w);
-            lo[4 * c] = __float_as_uint(l.x); lo[4 * c + 1] = __float_as_uint(l.y);
-            lo[4 * c + 2] = __float_as_uint(l.z); lo[4 * c + 3] = __float_as_uint(l.w);
-        }
-        const uint32_t tl = tc.tmem + ((uint32_t)(32 * lq) << 16) + 16 * cq;
-        tmem_st16(tl + TC_COL_W1HI, hi);
-        tmem_st16(tl + TC_COL_W1LO, lo);
+    for (int i = 0; i < 4; ++i) {
+        const float h = tf32_rn(v[i]);
+        hi[i] = __float_as_uint(h);
+        lo[i] = __float_as_uint(tf32_rn(v[i] - h));
     }
-    tmem_st_wait();
-    tc_fence_before();                                        // the caller's __syncthreads orders it before the UMMAs
 }
 
 // X never changes during a run, so its tf32 hi / lo split and both operand layouts are built ONCE (hmcx_mlp_pack_x ->
-// mlp_pack_x_kernel) and a tile's operands arrive ready-made by one bulk TMA copy each -- no staging pass, no landing
-// buffer (the first form re-split and re-laid-out every tile twice per evaluation: ~2.4k of its ~9.9k cycles):
-//   forward B operand  [64 rows hi | 64 rows lo (N = 128)] x [n0 (K)], K-major core matrices (8 rows x 16 B); stacking
-//       hi|lo along N lets ONE UMMA produce W1_hi X_hi^T and W1_hi X_lo^T side by side;
-//   backward B operand [n0 hi | n0 lo (N = 2 n0)] x [64 rows (K)], K-major (4 consecutive ROWS of one input column per 16 B).
-// Rows past the end of a ragged last tile are zero in the packed copy.
+// mlp_pack_x_kernel) and a tile's operands arrive ready-made by one bulk TMA copy each:
+//   forward B operand  [64 rows hi | 64 rows lo (N = 128)] x [n0 (K)], K-major core matrices (8 rows x 16 B);
+//   backward B operand [n0 hi | n0 lo (N = 2 n0)] x [64 rows (K)], K-major (4 K positions of one input column per 16 B).
+// K orders: forward position 16 t + 8 e + c + 4 h holds input feature 16 t + 4 c + 2 e + h (wgmma k-step 2 t + e, A
+// fragment column c + 4 h), so thread column c finds the A fragments of k-steps 2t and 2t+1 in ONE float4 of its W1 row;
+// backward position 8 s + c + 4 h holds tile row 8 s + 2 c + h, the row of forward accumulator register 4 s + h of
+// thread column c.  Rows past the end of a ragged last tile are zero in the packed copy.
 __device__ __forceinline__ int tc_pack_off_fwd(int r, int c) { return (c * (2 * TC_TR >> 3) + (r >> 3)) * 32 + (r & 7) * 4; }
 __device__ __forceinline__ int tc_pack_off_bwd(int a, int n, int n0) { return (a * (2 * n0 >> 3) + (n >> 3)) * 32 + (n & 7) * 4; }
+__device__ __forceinline__ int tc_kpos_fwd(int k) { return (k & ~15) + 8 * ((k >> 1) & 1) + ((k >> 2) & 3) + 4 * (k & 1); }
+__device__ __forceinline__ int tc_row_bwd(int p) { return (p & ~7) + 2 * (p & 3) + ((p >> 2) & 1); }
 
 __global__ void __launch_bounds__(256) mlp_pack_x_kernel(const MlpDev m, float* __restrict__ out) {
-    const int n0 = m.n[0], nch = n0 >> 2, tile_id = blockIdx.x;
+    const int n0 = m.n[0], tile_id = blockIdx.x;
     int r0, r_end;
     if (tile_id >= m.flat_base && m.flat_base >= m.tb[m.M]) {        // the all-rows tiling (only packed when it differs)
         r0 = TC_TR * (tile_id - m.flat_base); r_end = m.N;
@@ -567,23 +518,19 @@ __global__ void __launch_bounds__(256) mlp_pack_x_kernel(const MlpDev m, float* 
     const int cnt = min(TC_TR, r_end - r0);
     float* fwd = out + (size_t)tile_id * (2 * 2 * TC_TR * n0);
     float* bwd = fwd + 2 * TC_TR * n0;
-    for (int i = threadIdx.x; i < TC_TR * nch; i += blockDim.x) {
-        const int r = i / nch, c = i - r * nch;
-        const float4 v = r < cnt ? *reinterpret_cast<const float4*>(m.x + (size_t)(r0 + r) * n0 + 4 * c) : make_float4(0.f, 0.f, 0.f, 0.f);
-        float4 h, l;
-        tc_split4(v, h, l);
-        *reinterpret_cast<float4*>(fwd + tc_pack_off_fwd(r, c)) = h;
-        *reinterpret_cast<float4*>(fwd + tc_pack_off_fwd(r, c) + (TC_TR >> 3) * 32) = l;
+    for (int i = threadIdx.x; i < TC_TR * n0; i += blockDim.x) {
+        const int r = i / n0, k = i - r * n0, p = tc_kpos_fwd(k);
+        const float v = r < cnt ? m.x[(size_t)(r0 + r) * n0 + k] : 0.0f, h = tf32_rn(v);
+        const int off = tc_pack_off_fwd(r, p >> 2) + (p & 3);
+        fwd[off] = h;
+        fwd[off + (TC_TR >> 3) * 32] = tf32_rn(v - h);
     }
-    for (int i = threadIdx.x; i < (TC_TR / 4) * n0; i += blockDim.x) {
-        const int a = i / n0, n = i - a * n0;
-        float e[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) e[k] = (4 * a + k) < cnt ? m.x[(size_t)(r0 + 4 * a + k) * n0 + n] : 0.0f;
-        float4 h, l;
-        tc_split4(make_float4(e[0], e[1], e[2], e[3]), h, l);
-        *reinterpret_cast<float4*>(bwd + tc_pack_off_bwd(a, n, n0)) = h;
-        *reinterpret_cast<float4*>(bwd + tc_pack_off_bwd(a, n, n0) + (n0 >> 3) * 32) = l;
+    for (int i = threadIdx.x; i < TC_TR * n0; i += blockDim.x) {
+        const int p = i / n0, n = i - p * n0, r = tc_row_bwd(p);
+        const float v = r < cnt ? m.x[(size_t)(r0 + r) * n0 + n] : 0.0f, h = tf32_rn(v);
+        const int off = tc_pack_off_bwd(p >> 2, n, n0) + (p & 3);
+        bwd[off] = h;
+        bwd[off + (n0 >> 3) * 32] = tf32_rn(v - h);
     }
 }
 
@@ -613,68 +560,40 @@ __device__ __forceinline__ void tc_prefetch_y(const MlpDev& m, float* tile, int 
     }
 }
 
-// H^T = W1 . X^T  (one elected thread; completion -> barH).  A = W1 from TENSOR MEMORY (8 columns per k-step).  Two UMMAs per
-// k-step: W1_hi . [X_hi | X_lo]^T (N = 128, the two products land in columns [0,64) and [64,128)) and W1_lo . X_hi^T
-// (N = 64, accumulated onto [0,64)); the epilogue adds the two column blocks.  The B descriptors differ only in the
-// start-address field (bits 0-13, 16-byte units), so a k-step is an integer add.
-__device__ __forceinline__ void tc_issue_fwd(const MlpDev& m, const TcCtx& tc, const float* xop, uint32_t leader) {
-    const uint32_t idesc2 = make_idesc_tf32(TC_H, 2 * TC_TR), idesc1 = make_idesc_tf32(TC_H, TC_TR);
-    constexpr uint32_t B_LBO = (2 * TC_TR / 8) * 128;
-    uint64_t b = make_kmajor_desc(smem_u32(xop), B_LBO, 128);
-    const int ksteps = m.n[0] >> 3;
-    const uint32_t d = tc.tmem + TC_COL_H;
-    uint32_t a_hi = tc.tmem + TC_COL_W1HI, a_lo = tc.tmem + TC_COL_W1LO;
-    tc_fence_after();
-    for (int k = 0; k < ksteps; ++k) {
-        umma_tf32_ta_p(d, a_hi, b, idesc2, k != 0, leader);
-        umma_tf32_ta_p(d, a_lo, b, idesc1, true, leader);
-        a_hi += 8; a_lo += 8; b += (2 * B_LBO) >> 4;
-    }
-    umma_commit_p(tc.barH, leader);
-}
-
-// dW1 (+)= dH^T . X   (A from tensor memory; completion -> barW): dH_hi . [X_hi | X_lo] (N = 2 n0) and dH_lo . X_hi (N = n0)
-__device__ __forceinline__ void tc_issue_bwd(const MlpDev& m, const TcCtx& tc, const float* xop, bool accumulate, uint32_t leader) {
-    const int n0 = m.n[0];
-    const uint32_t idesc2 = make_idesc_tf32(TC_H, 2 * n0), idesc1 = make_idesc_tf32(TC_H, n0);
-    const uint32_t B_LBO = (uint32_t)(2 * n0 / 8) * 128;
-    uint64_t b = make_kmajor_desc(smem_u32(xop), B_LBO, 128);
-    const uint32_t d = tc.tmem + TC_COL_W;
-    uint32_t a_hi = tc.tmem + TC_COL_H, a_lo = tc.tmem + TC_COL_LO;
-    tc_fence_after();
+// per-thread constants / accumulators of the register epilogues.  Accumulator register i = 4 j + 2 uu + b of a thread
+// holds hidden unit u[uu] and tile row rbase + 8 j + b (hmcx_wgmma.cuh fragment layout, offset by the warpgroup's block)
+struct TcEpi {
+    int u[2], rbase, rh, grp;             // rh: the warpgroup's row half; grp: its 16-unit group (0..7)
+    float b1u[2], w2[2][TC_NLMAX];
+    float db1[2], dw2[2][TC_NLMAX], db2;
+};
+__device__ __forceinline__ void tc_epi_begin(const MlpDev& m, const float* q, TcEpi& e) {
+    const int wg = threadIdx.x >> 7, wl = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+    e.u[0] = 64 * (wg & 1) + 16 * wl + (lane >> 2);
+    e.u[1] = e.u[0] + 8;
+    e.rh = wg >> 1;
+    e.rbase = 32 * e.rh + 2 * (lane & 3);
+    e.grp = 4 * (wg & 1) + wl;
 #pragma unroll
-    for (int k = 0; k < TC_TR / 8; ++k) {
-        umma_tf32_ta_p(d, a_hi, b, idesc2, accumulate || k != 0, leader);
-        umma_tf32_ta_p(d, a_lo, b, idesc1, true, leader);
-        a_hi += 8; a_lo += 8; b += (2 * B_LBO) >> 4;
+    for (int uu = 0; uu < 2; ++uu) {
+        e.b1u[uu] = q[m.boff[0] + e.u[uu]];
+        e.db1[uu] = 0.0f;
+#pragma unroll
+        for (int j = 0; j < TC_NLMAX; ++j) {
+            e.w2[uu][j] = j < m.n[2] ? q[m.woff[1] + j * TC_H + e.u[uu]] : 0.0f;
+            e.dw2[uu][j] = 0.0f;
+        }
     }
-    umma_commit_p(tc.barW, leader);
-}
-
-// v[i] = this lane's value for row i; returns the sum over the warp's 32 lanes for row (lane >> 1)
-__device__ __forceinline__ float warp_transpose_sum16(float (&v)[16]) {
-    const int lane = threadIdx.x & 31;
-#define HMCX_TS_STEP(HALF, OFF)                                                          \
-    {                                                                                    \
-        const bool upper = (lane & OFF) != 0;                                            \
-        _Pragma("unroll") for (int i = 0; i < HALF; ++i) {                               \
-            const float send = upper ? v[i] : v[i + HALF];                               \
-            const float keep = upper ? v[i + HALF] : v[i];                               \
-            v[i] = keep + __shfl_xor_sync(0xffffffffu, send, OFF);                       \
-        }                                                                                \
-    }
-    HMCX_TS_STEP(8, 16) HMCX_TS_STEP(4, 8) HMCX_TS_STEP(2, 4) HMCX_TS_STEP(1, 2)
-#undef HMCX_TS_STEP
-    return v[0] + __shfl_xor_sync(0xffffffffu, v[0], 1);
+    e.db2 = 0.0f;
 }
 
 // bias + activation / activation derivative over a thread's 16 values, the activation kind resolved once
 template <int A>
-__device__ __forceinline__ void tc_act16_t(const uint32_t (&v)[16], float b, float (&act)[16]) {
+__device__ __forceinline__ void tc_act16_t(const float (&v)[16], const float (&b)[2], float (&act)[16]) {
 #pragma unroll
-    for (int i = 0; i < 16; ++i) act[i] = act_fwd(__uint_as_float(v[i]) + b, A);
+    for (int i = 0; i < 16; ++i) act[i] = act_fwd(v[i] + b[(i >> 1) & 1], A);
 }
-__device__ __forceinline__ void tc_act16(const uint32_t (&v)[16], float b, float (&act)[16], int a) {
+__device__ __forceinline__ void tc_act16(const float (&v)[16], const float (&b)[2], float (&act)[16], int a) {
     if (a == HMCX_ACT_RELU) tc_act16_t<HMCX_ACT_RELU>(v, b, act);
     else if (a == HMCX_ACT_TANH) tc_act16_t<HMCX_ACT_TANH>(v, b, act);
     else if (a == HMCX_ACT_SIGMOID) tc_act16_t<HMCX_ACT_SIGMOID>(v, b, act);
@@ -692,56 +611,97 @@ __device__ __forceinline__ void tc_dact16(const float (&act)[16], float (&d)[16]
     else tc_dact16_t<HMCX_ACT_NONE>(act, d);
 }
 
-// per-thread constants / accumulators of the register epilogues: thread <-> hidden unit u, 16 rows of the tile
-struct TcEpi {
-    int u, cq, lq;
-    float b1u, w2[TC_NLMAX];
-    float db1, dw2[TC_NLMAX], db2;
-};
-__device__ __forceinline__ void tc_epi_begin(const MlpDev& m, const float* q, TcEpi& e) {
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    e.lq = warp & 3; e.cq = warp >> 2; e.u = 32 * e.lq + lane;
-    e.b1u = q[m.boff[0] + e.u];
+// H^T block of this warpgroup = W1 . X^T: per 16 input features one float4 of each of the thread's two W1 rows gives the
+// A fragments of two k-steps; three wgmmas per k-step (W1_hi X_hi, W1_hi X_lo, W1_lo X_hi).  wgmma reads its register A
+// operands asynchronously, so each group is waited for before the next 16 features overwrite those registers.
+__device__ __forceinline__ void tc_mma_fwd(const MlpDev& m, const float* q, const TcEpi& e, uint32_t xop, float (&h)[16]) {
+    constexpr uint32_t B_LBO = (2 * TC_TR / 8) * 128;
+    const int n0 = m.n[0], c = threadIdx.x & 3;
+    const float* w0 = q + m.woff[0] + e.u[0] * n0 + 4 * c;
+    const float* w1 = q + m.woff[0] + e.u[1] * n0 + 4 * c;
+    xop += 512u * (uint32_t)e.rh;                         // this warpgroup's 32 rows = 4 of the operand's 8-row groups
 #pragma unroll
-    for (int j = 0; j < TC_NLMAX; ++j) {
-        e.w2[j] = j < m.n[2] ? q[m.woff[1] + j * TC_H + e.u] : 0.0f;
-        e.dw2[j] = 0.0f;
+    for (int i = 0; i < 16; ++i) h[i] = 0.0f;
+    for (int t = 0; t < (n0 >> 4); ++t) {
+        const float4 x0 = *reinterpret_cast<const float4*>(w0 + 16 * t), x1 = *reinterpret_cast<const float4*>(w1 + 16 * t);
+        uint32_t ah0[4], al0[4], ah1[4], al1[4];
+        tc_split({x0.x, x1.x, x0.y, x1.y}, ah0, al0);
+        tc_split({x0.z, x1.z, x0.w, x1.w}, ah1, al1);
+        const uint32_t b0 = xop + (uint32_t)(2 * t) * 2u * B_LBO, b1 = b0 + 2u * B_LBO;
+        wgmma_fence();
+        wgmma_tf32_rs<32>(h, ah0, make_kmajor_desc(b0, B_LBO, 128));
+        wgmma_tf32_rs<32>(h, ah0, make_kmajor_desc(b0 + 1024u, B_LBO, 128));
+        wgmma_tf32_rs<32>(h, al0, make_kmajor_desc(b0, B_LBO, 128));
+        wgmma_tf32_rs<32>(h, ah1, make_kmajor_desc(b1, B_LBO, 128));
+        wgmma_tf32_rs<32>(h, ah1, make_kmajor_desc(b1 + 1024u, B_LBO, 128));
+        wgmma_tf32_rs<32>(h, al1, make_kmajor_desc(b1, B_LBO, 128));
+        wgmma_commit();
+        wgmma_wait<0>();
     }
-    e.db1 = 0.0f; e.db2 = 0.0f;
+}
+
+// dW1 block (+)= dH^T . X over this warpgroup's 32 rows: the A fragment of k-step j is accumulator registers
+// 4j, 4j+2, 4j+1, 4j+3 (tc_row_bwd); N = n0
+template <int N0>
+__device__ __forceinline__ void tc_mma_bwd_n(float (&dw)[32], const uint32_t (&hi)[16], const uint32_t (&lo)[16], uint32_t xb,
+                                             int rh) {
+    constexpr uint32_t B_LBO = (uint32_t)(2 * N0 / 8) * 128, LO = (uint32_t)(N0 / 8) * 128;
+    float (&d)[N0 / 2] = *reinterpret_cast<float (*)[N0 / 2]>(&dw[0]);
+    uint32_t ah[4][4], al[4][4];                 // every A fragment is written before the fence that precedes the wgmmas
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        ah[j][0] = hi[4 * j]; ah[j][1] = hi[4 * j + 2]; ah[j][2] = hi[4 * j + 1]; ah[j][3] = hi[4 * j + 3];
+        al[j][0] = lo[4 * j]; al[j][1] = lo[4 * j + 2]; al[j][2] = lo[4 * j + 1]; al[j][3] = lo[4 * j + 3];
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        const uint32_t b = xb + (uint32_t)(4 * rh + j) * 2u * B_LBO;
+        wgmma_tf32_rs<N0>(d, ah[j], make_kmajor_desc(b, B_LBO, 128));
+        wgmma_tf32_rs<N0>(d, ah[j], make_kmajor_desc(b + LO, B_LBO, 128));
+        wgmma_tf32_rs<N0>(d, al[j], make_kmajor_desc(b, B_LBO, 128));
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+}
+__device__ __forceinline__ void tc_mma_bwd(int n0, float (&dw)[32], const uint32_t (&hi)[16], const uint32_t (&lo)[16],
+                                           uint32_t xb, int rh) {
+    if (n0 == 16) tc_mma_bwd_n<16>(dw, hi, lo, xb, rh);
+    else if (n0 == 32) tc_mma_bwd_n<32>(dw, hi, lo, xb, rh);
+    else if (n0 == 48) tc_mma_bwd_n<48>(dw, hi, lo, xb, rh);
+    else tc_mma_bwd_n<64>(dw, hi, lo, xb, rh);
 }
 
 // forward of one (prefetched) tile up to the network outputs: out[r * nL + j] (the loss stage's layout); the hidden
-// activations of this thread's (unit, 16 rows) block stay in `act`.  Ends with every thread past a __syncthreads.
+// activations of this thread's (2 units, 8 rows) block stay in `act`.  Ends with every thread past a __syncthreads.
 __device__ __forceinline__ void tc_forward_tile(const MlpDev& m, const float* q, float* tile, TcCtx& tc, const TcEpi& e,
                                                 float (&act)[16], int buf) {
     const int nL = m.n[2], lane = threadIdx.x & 31;
     if (threadIdx.x >= 32 && threadIdx.x < 64) asm volatile("cp.async.wait_group 0;" ::: "memory");    // the targets
-    if (threadIdx.x < 32) {                                       // warp 0 issues, warp-uniformly (hmcx_umma.cuh): ~65 instead of
-        mbar_wait(tc.barF[buf], tc.parF[buf]);                    // ~115 cycles per MMA.  This tile's forward operand has landed
-        TC_MARK(3);
-        tc_issue_fwd(m, tc, tile + (buf ? m.tc_f1 : m.tc_f0), elect_one());
-    }
+    mbar_wait(tc.barF[buf], tc.parF[buf]);                        // this tile's forward operand has landed
     tc.parF[buf] ^= 1;
-    TC_MARK(4);
-    mbar_wait(tc.barH, tc.parH);
-    tc.parH ^= 1;
-    tc_fence_after();
+    TC_MARK(3);
+    float h[16];
+    tc_mma_fwd(m, q, e, smem_u32(tile + (buf ? m.tc_f1 : m.tc_f0)), h);
     TC_MARK(5);
-    uint32_t v[16], w[16];
-    tmem_ld16(tc.tmem + ((uint32_t)(32 * e.lq) << 16) + TC_COL_H + 16 * e.cq, v);
-    tmem_ld16(tc.tmem + ((uint32_t)(32 * e.lq) << 16) + TC_COL_LO + 16 * e.cq, w);       // the W1_hi X_lo block
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) + __uint_as_float(w[i]));
-    tc_act16(v, e.b1u, act, m.act[0]);
+    tc_act16(h, e.b1u, act, m.act[0]);
     float* part = tile + m.tc_part;
 #pragma unroll
     for (int j = 0; j < TC_NLMAX; ++j) {
         if (j < nL) {
-            float t[16];
+            float t[8];                                           // rows rbase + 8 (k >> 1) + (k & 1), summed over 2 units
 #pragma unroll
-            for (int i = 0; i < 16; ++i) t[i] = e.w2[j] * act[i];
-            const float sum = warp_transpose_sum16(t);
-            if ((lane & 1) == 0) part[(e.lq * TC_TR + 16 * e.cq + (lane >> 1)) * TC_NLMAX + j] = sum;
+            for (int k = 0; k < 8; ++k) t[k] = e.w2[0][j] * act[4 * (k >> 1) + (k & 1)] + e.w2[1][j] * act[4 * (k >> 1) + 2 + (k & 1)];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {                         // ... and over the 8 lanes of the same column
+                t[k] += __shfl_xor_sync(0xffffffffu, t[k], 4);
+                t[k] += __shfl_xor_sync(0xffffffffu, t[k], 8);
+                t[k] += __shfl_xor_sync(0xffffffffu, t[k], 16);
+            }
+            if (lane < 4) {
+#pragma unroll
+                for (int k = 0; k < 8; ++k) part[(e.grp * TC_TR + e.rbase + 8 * (k >> 1) + (k & 1)) * TC_NLMAX + j] = t[k];
+            }
         }
     }
     __syncthreads();
@@ -749,8 +709,8 @@ __device__ __forceinline__ void tc_forward_tile(const MlpDev& m, const float* q,
     float* out = tile + m.aoff[2];
     for (int i = threadIdx.x; i < TC_TR * nL; i += MLP_THREADS) {
         const int r = i / nL, j = i - r * nL;
-        const float s = ((part[(0 * TC_TR + r) * TC_NLMAX + j] + part[(1 * TC_TR + r) * TC_NLMAX + j]) +
-                         part[(2 * TC_TR + r) * TC_NLMAX + j]) + part[(3 * TC_TR + r) * TC_NLMAX + j];
+        float s = part[r * TC_NLMAX + j];
+        for (int g = 1; g < 8; ++g) s += part[(g * TC_TR + r) * TC_NLMAX + j];
         out[i] = s + q[m.boff[1] + j];
     }
     __syncthreads();
@@ -760,13 +720,16 @@ __device__ __forceinline__ void tc_forward_tile(const MlpDev& m, const float* q,
 // g += d ll_split / dq over this rank's 64-row tiles of [r_begin, r_end)
 __device__ __forceinline__ void tc_backprop_rows(const MlpDev& m, const float* q, float* g, float* tile, TcCtx& tc,
                                                  int r_begin, int r_end, int tile0, ClusterCtx cc, int next_s = -2) {
-    const int nL = m.n[2], n0 = m.n[0];
+    const int nL = m.n[2], n0 = m.n[0], lane = threadIdx.x & 31;
     TcEpi e;
     tc_epi_begin(m, q, e);
     float* out = tile + m.aoff[2];
     float* dz = tile + m.dzoff[0];
     const float* ytile = tile + m.tc_yraw;
     const int stride = TC_TR * cc.size;
+    float dw[32];                                                 // this warpgroup's dW1 block (first n0 / 2 registers)
+#pragma unroll
+    for (int i = 0; i < 32; ++i) dw[i] = 0.0f;
     int done = 0;
     int r0 = r_begin + TC_TR * cc.rank;                           // this rank's tiles: rank, rank + size, ...
     int id = tile0 + cc.rank;                                     // ... and their packed operands
@@ -792,46 +755,35 @@ __device__ __forceinline__ void tc_backprop_rows(const MlpDev& m, const float* q
         uint32_t hi[16], lo[16];
 #pragma unroll
         for (int i = 0; i < 16; ++i) {
-            const int r = 16 * e.cq + i;
+            const int r = e.rbase + 8 * (i >> 2) + (i & 1), uu = (i >> 1) & 1;
             float da = 0.0f;
 #pragma unroll
             for (int j = 0; j < TC_NLMAX; ++j) {
                 if (j < nL) {
                     const float d = dz[r * nL + j];
-                    da = fmaf(d, e.w2[j], da);
-                    e.dw2[j] = fmaf(d, act[i], e.dw2[j]);
+                    da = fmaf(d, e.w2[uu][j], da);
+                    e.dw2[uu][j] = fmaf(d, act[i], e.dw2[uu][j]);
                 }
             }
             const float dh = da * dact[i];
-            e.db1 += dh;
+            e.db1[uu] += dh;
             const float h = tf32_rn(dh);
             hi[i] = __float_as_uint(h);
             lo[i] = __float_as_uint(tf32_rn(dh - h));
         }
-        const uint32_t tl = tc.tmem + ((uint32_t)(32 * e.lq) << 16) + 16 * e.cq;
-        tmem_st16(tl + TC_COL_H, hi);
-        tmem_st16(tl + TC_COL_LO, lo);
-        tmem_st_wait();
-        tc_fence_before();
-        TC_MARK(9);
-        __syncthreads();
         TC_MARK(10);
-        if (threadIdx.x < 32) {
-            mbar_wait(tc.barB, tc.parB);                          // the backward operand has landed (long ago)
-            tc_issue_bwd(m, tc, tile + m.tc_b, done != 0, elect_one());
-        }
+        mbar_wait(tc.barB, tc.parB);                              // the backward operand has landed (long ago)
         tc.parB ^= 1;
+        tc_mma_bwd(n0, dw, hi, lo, smem_u32(tile + m.tc_b), e.rh);
         ++done;
         TC_MARK(11);
-        mbar_wait(tc.barW, tc.parW);                              // the backward operand buffer and the dH columns are free again
-        tc.parW ^= 1;
+        __syncthreads();                                          // every warpgroup is done with the backward operand
         if (has_next) tc_prefetch_bwd(m, tile, tc, id + cc.size);
         TC_MARK(12);
     }
     if (done == 0) return;                                        // (uniform over the CTA)
     // The first tile of the NEXT evaluation (the schedule knows its split): its operands do not depend on q, so they are
-    // requested now and land while this evaluation finishes (dW1 read-out, reductions, cluster sum, kick, drift) -- an
-    // evaluation used to start with ~2.3k cycles of exposed TMA latency.
+    // requested now and land while this evaluation finishes (dW1 read-out, reductions, cluster sum, kick, drift).
     int nid = -1;
     if (next_s > -2) {
         const int nb = next_s < 0 ? 0 : m.sb[next_s], ne = next_s < 0 ? m.N : m.sb[next_s + 1];
@@ -842,23 +794,23 @@ __device__ __forceinline__ void tc_backprop_rows(const MlpDev& m, const float* q
             tc_prefetch_y(m, tile, nr0, min(TC_TR, ne - nr0));    // the last loss stage is over
         }
     }
-    tc_fence_after();
-    // ---- dW1: TMEM -> padded staging -> g, conflict-free both ways
+    // ---- dW1: the two row halves' blocks -> padded staging (first half stores, second half adds) -> g
     float* stg = tile + m.tc_f1;                 // forward buffer 1 | backward buffer (adjacent, both idle now)
     const int pitch = n0 + 4;
-    if (16 * e.cq < n0) {
-        uint32_t v[16], w[16];
-        tmem_ld16(tc.tmem + ((uint32_t)(32 * e.lq) << 16) + TC_COL_W + 16 * e.cq, v);
-        tmem_ld16(tc.tmem + ((uint32_t)(32 * e.lq) << 16) + TC_COL_W + n0 + 16 * e.cq, w);   // the dH_hi X_lo block
+    for (int half = 0; half < 2; ++half) {
+        if (e.rh == half) {
 #pragma unroll
-        for (int i = 0; i < 16; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) + __uint_as_float(w[i]));
-#pragma unroll
-        for (int i = 0; i < 16; i += 4)
-            *reinterpret_cast<float4*>(stg + e.u * pitch + 16 * e.cq + i) =
-                make_float4(__uint_as_float(v[i]), __uint_as_float(v[i + 1]), __uint_as_float(v[i + 2]), __uint_as_float(v[i + 3]));
+            for (int i = 0; i < 32; i += 2) {
+                if (i < n0 / 2) {
+                    float2* s2 = reinterpret_cast<float2*>(stg + e.u[(i >> 1) & 1] * pitch + 8 * (i >> 2) + 2 * (lane & 3));
+                    float2 v = make_float2(dw[i], dw[i + 1]);
+                    if (half) { const float2 o = *s2; v.x = o.x + v.x; v.y = o.y + v.y; }
+                    *s2 = v;
+                }
+            }
+        }
+        __syncthreads();
     }
-    tc_fence_before();
-    __syncthreads();
     float* gW = g + m.woff[0];
     for (int i4 = threadIdx.x; i4 < TC_H * n0 / 4; i4 += MLP_THREADS) {
         const int u = (4 * i4) / n0, k = 4 * i4 - u * n0;
@@ -867,20 +819,29 @@ __device__ __forceinline__ void tc_backprop_rows(const MlpDev& m, const float* q
         a.x += d.x; a.y += d.y; a.z += d.z; a.w += d.w;
         *reinterpret_cast<float4*>(gW + 4 * i4) = a;
     }
-    // ---- db1, dW2: four per-unit partials (one per 16-row column group) summed in a fixed order; db2
+    // ---- db1, dW2: summed over the 4 lanes that share a unit, then two per-unit partials (one per row half) in a fixed
+    // order; db2
     float* red = tile + m.tc_part;
-    red[(e.cq * TC_H + e.u) * (1 + TC_NLMAX)] = e.db1;
 #pragma unroll
-    for (int j = 0; j < TC_NLMAX; ++j) red[(e.cq * TC_H + e.u) * (1 + TC_NLMAX) + 1 + j] = e.dw2[j];
+    for (int uu = 0; uu < 2; ++uu) {
+        float v = e.db1[uu];
+        v += __shfl_xor_sync(0xffffffffu, v, 1);
+        v += __shfl_xor_sync(0xffffffffu, v, 2);
+        if ((lane & 3) == 0) red[(e.rh * TC_H + e.u[uu]) * (1 + TC_NLMAX)] = v;
+#pragma unroll
+        for (int j = 0; j < TC_NLMAX; ++j) {
+            float w = e.dw2[uu][j];
+            w += __shfl_xor_sync(0xffffffffu, w, 1);
+            w += __shfl_xor_sync(0xffffffffu, w, 2);
+            if ((lane & 3) == 0) red[(e.rh * TC_H + e.u[uu]) * (1 + TC_NLMAX) + 1 + j] = w;
+        }
+    }
     fence_async_smem();                                           // the staging reads above precede the TMA write below
     __syncthreads();
     if (nid >= 0) { tc_prefetch_bwd(m, tile, tc, nid); tc.pre_id = nid; }
     if (threadIdx.x < TC_H) {
         const int u = threadIdx.x;
-        auto tot = [&](int f) {
-            return ((red[(0 * TC_H + u) * (1 + TC_NLMAX) + f] + red[(1 * TC_H + u) * (1 + TC_NLMAX) + f]) +
-                    red[(2 * TC_H + u) * (1 + TC_NLMAX) + f]) + red[(3 * TC_H + u) * (1 + TC_NLMAX) + f];
-        };
+        auto tot = [&](int f) { return red[u * (1 + TC_NLMAX) + f] + red[(TC_H + u) * (1 + TC_NLMAX) + f]; };
         g[m.boff[0] + u] += tot(0);
         for (int j = 0; j < nL; ++j) g[m.woff[1] + j * TC_H + u] += tot(1 + j);
     }
@@ -947,7 +908,7 @@ __device__ __forceinline__ void mlp_grad_split(const MlpDev& m, const float* q, 
     TC_MARK(1);
     if (cc.rank == 0) mlp_prior_grad(m, q, g);                 // the prior part enters the rank-ordered sum once
     else for (int i = threadIdx.x; i < m.Dp; i += MLP_THREADS) g[i] = 0.0f;
-    if (m.tc) { tc_pack_w1(m, q, tc); fence_async_smem(); }    // (generic accesses of the operand buffers precede the TMA writes)
+    if (m.tc) fence_async_smem();                              // (generic accesses of the operand buffers precede the TMA writes)
     __syncthreads();
     TC_MARK(2);
     if (m.has_data) {
@@ -993,7 +954,6 @@ __device__ __forceinline__ float mlp_log_prob(const MlpDev& m, const float* q, f
     if (!m.has_data) return prior_term;
     TcEpi te;
     if (m.tc) {
-        tc_pack_w1(m, q, tc);
         tc_epi_begin(m, q, te);
         fence_async_smem();
         __syncthreads();
@@ -1077,8 +1037,7 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
     __shared__ float s_bcast[4];
     __shared__ float s_xchg;
     __shared__ int s_perm[HMCX_MLP_MAX_SPLITS];
-    __shared__ __align__(8) uint64_t s_bars[5];
-    __shared__ uint32_t s_tmem;
+    __shared__ __align__(8) uint64_t s_bars[3];
 
     const MlpDev& m = a.m;
     ClusterCtx cc = {0, 1};
@@ -1092,7 +1051,7 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
     const size_t row = (size_t)c * a.ld;
     const uint64_t chain_id = a.chain_offset + (uint64_t)c;
     TcCtx tc = {};
-    if (m.tc) tc_init(tc, s_bars, &s_tmem);
+    if (m.tc) tc_init(tc, s_bars);
 
     for (int i = tid; i < m.Dp; i += MLP_THREADS) { q[i] = i < D ? a.q_cur[row + i] : 0.0f; p[i] = 0.0f; g[i] = 0.0f; }
     __syncthreads();
@@ -1445,7 +1404,6 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
         if (a.nuts) { a.h_bar[c] = h_bar; a.eps_bar[c] = eps_bar; }
         if (a.num_rejected) a.num_rejected[c] += rejected;
     }
-    if (m.tc) tc_fini(tc);
 }
 
 // gradient / log-prob of C parameter vectors (collect_gradients mirror, also the unit-test hook of the backward pass)
@@ -1454,14 +1412,13 @@ mlp_grad_kernel(const MlpDev m, const float* __restrict__ qin, int ld, int split
                 float* __restrict__ lpout) {
     extern __shared__ __align__(128) float sm[];
     __shared__ float sred[64];
-    __shared__ __align__(8) uint64_t s_bars[5];
-    __shared__ uint32_t s_tmem;
+    __shared__ __align__(8) uint64_t s_bars[3];
     float* q = sm;
     float* g = q + m.Dp;
     float* tile = sm + m.tile_base;
     const size_t row = (size_t)blockIdx.x * ld;
     TcCtx tc = {};
-    if (m.tc) tc_init(tc, s_bars, &s_tmem);
+    if (m.tc) tc_init(tc, s_bars);
     for (int i = threadIdx.x; i < m.Dp; i += MLP_THREADS) { q[i] = i < m.D ? qin[row + i] : 0.0f; g[i] = 0.0f; }
     __syncthreads();
     if (gout) {
@@ -1473,7 +1430,6 @@ mlp_grad_kernel(const MlpDev m, const float* __restrict__ qin, int ld, int split
         const float lp = mlp_log_prob<1>(m, q, tile, sred, split, nullptr, ClusterCtx{0, 1}, nullptr, tc);
         if (threadIdx.x == 0) lpout[blockIdx.x] = lp;
     }
-    if (m.tc) tc_fini(tc);
 }
 
 // predict_model: one CTA per posterior sample
@@ -1482,8 +1438,7 @@ mlp_predict_kernel(const MlpDev m, const float* __restrict__ samples, int ld, fl
                    float* __restrict__ lpout) {
     extern __shared__ __align__(128) float sm[];
     __shared__ float sred[64];
-    __shared__ __align__(8) uint64_t s_bars[5];
-    __shared__ uint32_t s_tmem;
+    __shared__ __align__(8) uint64_t s_bars[3];
     float* q = sm;
     float* tile = sm + m.tile_base;
     const size_t row = (size_t)blockIdx.x * ld;
@@ -1491,10 +1446,9 @@ mlp_predict_kernel(const MlpDev m, const float* __restrict__ samples, int ld, fl
     __syncthreads();
     float* my_pred = pred + (size_t)blockIdx.x * m.N * m.n[m.L];
     TcCtx tc = {};
-    if (m.tc) tc_init(tc, s_bars, &s_tmem);
+    if (m.tc) tc_init(tc, s_bars);
     const float lp = mlp_log_prob<1>(m, q, tile, sred, -1, my_pred, ClusterCtx{0, 1}, nullptr, tc);
     if (threadIdx.x == 0 && lpout) lpout[blockIdx.x] = lp;
-    if (m.tc) tc_fini(tc);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -1517,7 +1471,7 @@ static bool mlp_tc_shape(const MlpDev& m) {
     return m.L == 2 && m.n[1] == TC_H && m.n[0] >= 16 && m.n[0] <= 64 && (m.n[0] & 15) == 0 && m.n[2] <= TC_NLMAX && m.has_data;
 }
 
-// tensor-core layout of the tile area (one-hidden-layer stacks n0 -> 128 -> nL, see the tcgen05 section above)
+// tensor-core layout of the tile area (one-hidden-layer stacks n0 -> 128 -> nL, see the tensor-core section above)
 static bool mlp_layout_tc(MlpDev& m, int state_vectors) {
     if (!mlp_tc_shape(m) || !m.xp) return false;
     const int n0 = m.n[0];
@@ -1672,7 +1626,7 @@ int mlp_split_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hm
     if (a.m.has_data && a.m.D <= MLP_THREADS * 36) {
         int min_tiles = 1 << 30;
         for (int s = 0; s < a.m.M; ++s) min_tiles = min(min_tiles, (a.m.sb[s + 1] - a.m.sb[s] + a.m.T - 1) / a.m.T);
-        int dev = 0, sms = 148;
+        int dev = 0, sms = 132;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         const int pinned = target->mlp->cluster_size;

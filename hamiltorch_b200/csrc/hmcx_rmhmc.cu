@@ -1,4 +1,4 @@
-// hmcx_rmhmc.cu -- Riemannian-manifold HMC (sampler=RMHMC) on sm_100a.
+// hmcx_rmhmc.cu -- Riemannian-manifold HMC (sampler=RMHMC) on sm_90a (H100).
 //
 //   fisher + softabs          samplers.py:69-127      -> eval_metric()  (closed-form Hessian, Jacobi eigensolver)
 //   cholesky_inverse          samplers.py:130-149     -> via the eigen-decomposition (G~^-1 p = Q diag(1/lam~) Q^T p)

@@ -1,21 +1,18 @@
-// hmcx_tc.cu -- 5th-generation tensor-core (tcgen05 / TMEM) building block for the dense contractions of the path:
+// hmcx_tc.cu -- Hopper tensor-core (wgmma) building block for the dense contractions of the path:
 //     D[M x N] = A[M x K] . B[N x K]^T        (A, B, D row-major fp32; fp32-accurate via 3xTF32 split operands)
 // This is the GEMM behind full-covariance Gaussian targets / full mass matrices at large D
 // (grad log p = -(q - mu) P for ALL chains at once is exactly this contraction with M = chains, N = K = D,
 // samplers.py:294, :812 and targets.GaussianFull) -- SURVEY.md section 8f item 2.
 //
-// Blackwell mechanics (one CTA per 128 x 128 output tile, 128 threads):
-//   * operands are staged by the CTA's threads from global memory into shared memory in the canonical UMMA
-//     K-major / no-swizzle layout (8-row x 16-byte core matrices), each fp32 split into tf32 hi + tf32 lo;
-//   * ONE elected thread issues tcgen05.mma.cta_group::1.kind::tf32 (M=128, N=128, K=8 per instruction), three per
-//     k-step: hi*hi + hi*lo + lo*hi, accumulating in fp32 in TENSOR MEMORY (128 lanes x 128 columns);
-//   * completion is tracked with tcgen05.commit -> mbarrier; the epilogue reads the accumulator back with
-//     tcgen05.ld (32x32b.x32: warp w owns TMEM lanes 32w..32w+31) and stores rows to global memory.
-// Descriptor encodings follow the CUTLASS sm100 definitions (cute/arch/mma_sm100_desc.hpp: SmemDescriptor,
-// InstrDescriptor) -- re-derived here, no CUTLASS code is used.
+// sm_90a mechanics (one CTA per 128 x BN output tile):
+//   * operands sit in shared memory in the canonical K-major / no-swizzle layout (8-row x 16-byte core matrices), each
+//     fp32 split into tf32 hi + tf32 lo;
+//   * one warpgroup issues wgmma.mma_async m64nBNk8 tf32 for the two 64-row halves of the tile, three per k-step:
+//     hi*hi + hi*lo + lo*hi, accumulating in fp32 REGISTERS (hmcx_wgmma.cuh);
+//   * the epilogues need one thread per chain row, so the accumulator tile is handed over through shared memory.
 #include <cstdlib>
 #include "hmcx_common.cuh"
-#include "hmcx_umma.cuh"
+#include "hmcx_wgmma.cuh"
 
 namespace hmcx {
 
@@ -27,21 +24,9 @@ int flow_small_rmhmc_run(const hmcx_target_t*, const hmcx_rmhmc_t*, const hmcx_c
                          float*, const float*, int, int, int, int, int, int, int, float*, uint8_t*, uint8_t*, float*, int32_t*,
                          float, float, cudaStream_t);
 
-// 32 lanes x 32 columns of the accumulator: thread (lane) <-> TMEM lane, register i <-> column i; waits for the data
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-        "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-          "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-          "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-          "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
 constexpr int TC_M = 128, TC_N = 128, TC_KC = 32;        // CTA tile and K chunk (fp32 elements)
-constexpr int TC_THREADS = 128;
+constexpr int TC_THREADS = 128;                           // one warpgroup: the MMAs and the epilogue rows
+constexpr int DENSE_THREADS = TC_THREADS + 32;            // + one warp whose lane 0 is the TMA producer
 
 // Stage a [128 rows x KC] fp32 slab (row stride `ld`) into the canonical layout, split into tf32 hi and lo copies.
 // Core matrix (rg = row/8, kc = k/4) lives at ((kc * 16 + rg) * 128) bytes: SBO = 128 B, LBO = 16*128 = 2048 B.
@@ -62,6 +47,22 @@ __device__ __forceinline__ void stage_operand(const float* __restrict__ g, int l
     }
 }
 
+// The three 3xTF32 products of one k-step for both 64-row halves of a 128-row A block: acc[h] += A[64h..] . B^T.
+// sa / sb: shared addresses of the hi blocks at this k-step, lo blocks `a_lo` / `b_lo` bytes further.
+template <int BN>
+__device__ __forceinline__ void mma_kstep_3xtf32(float (&acc)[2][BN / 2], uint32_t sa, uint32_t a_lo, uint32_t sb,
+                                                 uint32_t b_lo) {
+    constexpr uint32_t A_LBO = (TC_M / 8) * 128, B_LBO = (BN / 8) * 128;
+    const uint64_t bh = make_kmajor_desc(sb, B_LBO, 128), bl = make_kmajor_desc(sb + b_lo, B_LBO, 128);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const uint64_t ah = make_kmajor_desc(sa + h * 1024u, A_LBO, 128), al = make_kmajor_desc(sa + a_lo + h * 1024u, A_LBO, 128);
+        wgmma_tf32_ss<BN>(acc[h], ah, bh);
+        wgmma_tf32_ss<BN>(acc[h], ah, bl);
+        wgmma_tf32_ss<BN>(acc[h], al, bh);
+    }
+}
+
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_nt_tf32x3_kernel(const float* __restrict__ A, const float* __restrict__ B, float* __restrict__ D, int M, int N,
                       int K) {
@@ -70,81 +71,48 @@ gemm_nt_tf32x3_kernel(const float* __restrict__ A, const float* __restrict__ B, 
     float* a_lo = a_hi + TC_M * TC_KC;
     float* b_hi = a_lo + TC_M * TC_KC;
     float* b_lo = b_hi + TC_N * TC_KC;
-    __shared__ __align__(8) uint64_t s_mbar;
-    __shared__ uint32_t s_tmem;
 
     const int tile_n = blockIdx.x, tile_m = blockIdx.y;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t mbar = smem_u32(&s_mbar);
-
-    if (threadIdx.x == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(mbar));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 0) {                                                           // TMEM: 128 fp32 accumulator columns
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(&s_tmem)), "r"(128));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem = s_tmem;
-
     const float* Ag = A + (size_t)tile_m * TC_M * K;
     const float* Bg = B + (size_t)tile_n * TC_N * K;
-    const uint32_t idesc = make_idesc_tf32(TC_M, TC_N);
-    uint32_t parity = 0;
+    float acc[2][TC_N / 2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < TC_N / 2; ++i) acc[h][i] = 0.0f;
     for (int k0 = 0; k0 < K; k0 += TC_KC) {
         stage_operand(Ag + k0, K, a_hi, a_lo);
         stage_operand(Bg + k0, K, b_hi, b_lo);
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");           // generic-proxy writes -> async proxy (UMMA)
+        fence_async_smem();                                                    // generic-proxy writes -> wgmma operands
         __syncthreads();
-        if (warp == 0) {                                                       // warp-uniform issue (hmcx_umma.cuh)
-            const uint32_t leader = elect_one();
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+        wgmma_fence();
 #pragma unroll
-            for (int s = 0; s < TC_KC / 8; ++s) {                              // UMMA K = 8 tf32 = two core matrices
-                const uint32_t koff = (uint32_t)s * 2u * 2048u;
-                const uint64_t ah = make_kmajor_desc(smem_u32(a_hi) + koff, 2048, 128);
-                const uint64_t al = make_kmajor_desc(smem_u32(a_lo) + koff, 2048, 128);
-                const uint64_t bh = make_kmajor_desc(smem_u32(b_hi) + koff, 2048, 128);
-                const uint64_t bl = make_kmajor_desc(smem_u32(b_lo) + koff, 2048, 128);
-                umma_tf32_p(tmem, ah, bh, idesc, (k0 | s) != 0, leader);
-                umma_tf32_p(tmem, ah, bl, idesc, true, leader);
-                umma_tf32_p(tmem, al, bh, idesc, true, leader);
-            }
-            umma_commit_p(mbar, leader);
+        for (int s = 0; s < TC_KC / 8; ++s) {                                  // wgmma K = 8 tf32 = two core matrices
+            const uint32_t koff = (uint32_t)s * 2u * 2048u;
+            mma_kstep_3xtf32<TC_N>(acc, smem_u32(a_hi) + koff, (uint32_t)(TC_M * TC_KC * 4), smem_u32(b_hi) + koff,
+                                   (uint32_t)(TC_N * TC_KC * 4));
         }
-        mbar_wait(mbar, parity);                                               // MMAs done: smem may be overwritten
-        parity ^= 1;
+        wgmma_commit();
+        wgmma_wait<0>();                                                       // MMAs done: smem may be overwritten
         __syncthreads();
     }
-    // ---- epilogue: TMEM -> registers -> global ----
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int row = tile_m * TC_M + warp * 32 + lane;
-    float* drow = D + (size_t)row * N + (size_t)tile_n * TC_N;
-#pragma unroll 1
-    for (int c0 = 0; c0 < TC_N; c0 += 32) {
-        uint32_t v[32];
-        const uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0;
-        tmem_ld32(taddr, v);
-        if (row < M) {
+    // ---- epilogue: straight from the accumulator fragments (hmcx_wgmma.cuh) to global memory ----
 #pragma unroll
-            for (int j = 0; j < 32; j += 4)
-                *reinterpret_cast<float4*>(drow + c0 + j) =
-                    make_float4(__uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]),
-                                __uint_as_float(v[j + 3]));
+    for (int h = 0; h < 2; ++h) {
+#pragma unroll
+        for (int i = 0; i < TC_N / 2; i += 2) {
+            const int row = tile_m * TC_M + 64 * h + 16 * warp + (lane >> 2) + 8 * ((i >> 1) & 1);
+            const int col = tile_n * TC_N + 8 * (i >> 2) + 2 * (lane & 3);
+            if (row < M) *reinterpret_cast<float2*>(D + (size_t)row * N + col) = make_float2(acc[h][i], acc[h][i + 1]);
         }
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem), "r"(128));
 }
 
 
 // =========================================================================================================
 // Dense-target plain HMC / HMC_NUTS: full-covariance Gaussian at large D, all chains per step on the tensor cores
-//   grad log p (samplers.py:297 via autograd of targets.GaussianFull) for ALL chains = -(Q - mu) P : one tcgen05 GEMM
+//   grad log p (samplers.py:297 via autograd of targets.GaussianFull) for ALL chains = -(Q - mu) P : one tensor-core GEMM
 //   per leapfrog step with the kick (:281/:298/:302) and the drift (:284/:296) fused into its epilogue.
 // Step-synchronous: a trajectory is L+1 launches of dense_step_kernel (each needs every column of the new Q, a
 // grid-wide dependency), bracketed by dense_gibbs_kernel and dense_mh_kernel; launched back-to-back on one stream
@@ -165,7 +133,7 @@ struct DenseArgs {
 enum { DENSE_FIRST = 0, DENSE_MIDDLE = 1, DENSE_LAST = 2, DENSE_EVAL = 3 };
 
 // ---- packed operand layout ---------------------------------------------------------------------------------------
-// Operands are kept in global memory ALREADY in the canonical UMMA layout and ALREADY split into tf32 hi / lo, one
+// Operands are kept in global memory ALREADY in the canonical wgmma layout and ALREADY split into tf32 hi / lo, one
 // contiguous block per (row tile, 32-wide K chunk, hi|lo): a block of R rows is R*32 floats, element (r, k) at
 //     ((k/4) * (R/8) + r/8) * 32 + (r%8) * 4 + (k%4)            [8-row x 16-byte core matrices, K-major, no swizzle]
 // so that the GEMM main loop is nothing but 1-D bulk TMA copies (cp.async.bulk -> UBLKCP) into the stage buffers.
@@ -207,7 +175,7 @@ __host__ __device__ constexpr int dense_stage_floats(int BN) { return 2 * TC_M *
 
 // Programmatic dependent launch: the step-synchronous dense paths are chains of short GEMM launches on one stream.  Each
 // kernel lets its successor start launching at once (griddepcontrol.launch_dependents) and itself waits for its
-// predecessor's completion + memory flush (griddepcontrol.wait) only after its prologue (mbarrier init, TMEM allocation),
+// predecessor's completion + memory flush (griddepcontrol.wait) only after its prologue (mbarrier init),
 // so launch latency and prologue overlap the previous kernel's main loop and epilogue.  All global reads and writes of a
 // kernel come after its wait.  HMCX_PDL=0 in the environment falls back to plain stream order.
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
@@ -227,141 +195,110 @@ static void launch_pdl(void (*kernel)(KArgs...), dim3 grid, int threads, size_t 
     cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
     cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
-// the 2 x 2 cluster form (multicast operands): grid.x and grid.y even
-template <typename... KArgs, typename... Args>
-static void launch_pdl_cluster(void (*kernel)(KArgs...), dim3 grid, int threads, size_t smem, cudaStream_t st, Args... args) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid; cfg.blockDim = dim3(threads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 2; attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
-}
-static bool dense_cluster_ok(dim3 grid, int BN) {
-    // opt-in (HMCX_DENSE_CLUSTER=1): measured on B200, the multicast form does NOT beat one CTA per tile -- these GEMMs are
-    // bound by SHARED-MEMORY bandwidth (3xTF32: every MMA re-reads 8 KB of operands per 64 cycles = 128 B/clk, the SM's
-    // limit, plus the TMA writes), not by L2 -> SM traffic; see DESIGN.md 3.7
-    static const bool on = [] { const char* e = getenv("HMCX_DENSE_CLUSTER"); return e && e[0] == '1'; }();
-    return on && BN >= 64 && (grid.x % 2) == 0 && (grid.y % 2) == 0;
-}
 
-// Prologue shared by the dense kernels: mbarrier ring + accumulator columns in tensor memory (warp 0 allocates).
-template <int BN, int ST, bool CL = false>
-__device__ __forceinline__ uint32_t dense_prologue(uint64_t* s_full, uint64_t* s_empty, uint64_t* s_done, uint32_t* s_tmem) {
+// Prologue shared by the dense kernels: the mbarrier ring.
+template <int ST>
+__device__ __forceinline__ void dense_prologue(uint64_t* s_full, uint64_t* s_empty) {
     if (threadIdx.x == 0) {
-        // CL (2 x 2 cluster, multicast operands): a stage is written by this CTA, its row peer and its column peer, so it is
-        // free only when the MMA warps of all three have released it
-        for (int s = 0; s < ST; ++s) { mbar_init(smem_u32(&s_full[s]), 1); mbar_init(smem_u32(&s_empty[s]), CL ? 3 : 1); }
-        mbar_init(smem_u32(s_done), 1);
+        for (int s = 0; s < ST; ++s) { mbar_init(smem_u32(&s_full[s]), 1); mbar_init(smem_u32(&s_empty[s]), 1); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if ((threadIdx.x >> 5) == 0) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" :: "r"(smem_u32(s_tmem)), "r"(BN < 32 ? 32 : BN));
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    if (CL) cluster_sync_all();                                // every CTA's barriers exist before a peer signals them
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    return *s_tmem;
 }
 
-// The warp-specialised main loop shared by the dense kernels: thread 0 = TMA producer (1-D bulk copies of the packed
-// hi|lo operand blocks into an ST-stage ring), thread 32 = MMA issuer (three tf32 UMMAs per 8-wide k-step: hi*hi +
-// hi*lo + lo*hi, fp32 accumulators in tensor memory), tcgen05.commit releasing stages / signalling `s_done`.
-// CL = true: launched as 2 x 2 thread-block clusters over (column tile, row tile).  The two CTAs of a cluster ROW share the
-// A block (same chains), the two of a cluster COLUMN share the B block (same columns of the matrix): every CTA fetches ONE
-// half (hi or lo) of its A block and of its B block and MULTICASTS it to both sharers, so each operand byte leaves L2 once
-// per cluster instead of once per CTA -- half the L2 -> SM traffic that bounded these kernels (512 MB per launch at
-// D = 2048 x 1024 chains = 8.4 TB/s).
-template <int BN, int ST, bool CL = false>
-__device__ __forceinline__ void dense_mainloop(float* smem, uint64_t* s_full, uint64_t* s_empty, uint64_t* s_done_p,
-                                               uint32_t tmem, const float* __restrict__ QpIn,
-                                               const float* __restrict__ Ppack, int tile_m, int tile_n, int kchunks) {
+// The warp-specialised main loop shared by the dense kernels: thread TC_THREADS (lane 0 of the last warp) = TMA producer
+// (1-D bulk copies of the packed hi|lo operand blocks into an ST-stage ring), threads [0, TC_THREADS) = the MMA warpgroup
+// (three tf32 wgmmas per 8-wide k-step and 64-row half: hi*hi + hi*lo + lo*hi, fp32 accumulators in registers).  One
+// wgmma group stays in flight: a stage is released when the group that read it has completed.  On return the ring is
+// idle and `acc` holds the 128 x BN tile in the fragment layout of hmcx_wgmma.cuh (MMA threads only).
+template <int BN, int ST>
+__device__ __forceinline__ void dense_mainloop(float* smem, uint64_t* s_full, uint64_t* s_empty, float (&acc)[2][BN / 2],
+                                               const float* __restrict__ QpIn, const float* __restrict__ Ppack,
+                                               int tile_m, int tile_n, int kchunks) {
     constexpr int A_BLK = TC_M * TC_KC, B_BLK = BN * TC_KC;
     constexpr uint32_t STAGE_BYTES = (uint32_t)dense_stage_floats(BN) * 4u;
-    uint64_t& s_done = *s_done_p;
-    const uint32_t cx = CL ? cluster_ctaid_x() : 0, cy = CL ? cluster_ctaid_y() : 0;       // cluster rank = cx + 2 cy
-    const uint16_t mask_row = (uint16_t)(0x3u << (2 * cy)), mask_col = (uint16_t)((1u << cx) | (1u << (cx + 2)));
-    if (threadIdx.x == 0) {
+    if (threadIdx.x == TC_THREADS) {
         // ===== TMA producer: bulk copies per stage (A hi, A lo, B hi, B lo are adjacent pairs in global memory) =====
         for (int i = 0; i < kchunks; ++i) {
             const int s = i % ST;
             mbar_wait(smem_u32(&s_empty[s]), ((i / ST) & 1) ^ 1);
             const uint32_t full = smem_u32(&s_full[s]);
-            mbar_expect_tx(full, STAGE_BYTES);                  // (a peer's multicast may complete bytes before this: fine)
+            mbar_expect_tx(full, STAGE_BYTES);
             float* st = smem + (size_t)s * dense_stage_floats(BN);
-            if (CL) {
-                // my half of the A block (cx = 0: hi, 1: lo) to both CTAs of my row; my half of the B block (cy) to my column
-                bulk_g2s_multicast(smem_u32(st + cx * A_BLK), QpIn + pack_block_base(tile_m, i, (int)cx, kchunks, TC_M),
-                                   A_BLK * 4, full, mask_row);
-                bulk_g2s_multicast(smem_u32(st + 2 * A_BLK + cy * B_BLK), Ppack + pack_block_base(tile_n, i, (int)cy, kchunks, BN),
-                                   B_BLK * 4, full, mask_col);
-            } else {
-                bulk_g2s(smem_u32(st), QpIn + pack_block_base(tile_m, i, 0, kchunks, TC_M), 2 * A_BLK * 4, full);
-                bulk_g2s(smem_u32(st + 2 * A_BLK), Ppack + pack_block_base(tile_n, i, 0, kchunks, BN), 2 * B_BLK * 4, full);
-            }
+            bulk_g2s(smem_u32(st), QpIn + pack_block_base(tile_m, i, 0, kchunks, TC_M), 2 * A_BLK * 4, full);
+            bulk_g2s(smem_u32(st + 2 * A_BLK), Ppack + pack_block_base(tile_n, i, 0, kchunks, BN), 2 * B_BLK * 4, full);
         }
-    } else if ((threadIdx.x >> 5) == 1) {
-        // ===== MMA issuer: the WHOLE warp runs the loop (warp-uniform: descriptors in uniform registers), the elected lane's
-        // instructions take effect (hmcx_umma.cuh, "warp-uniform issue": 65 instead of ~115 cycles per MMA) =====
-        const uint32_t leader = elect_one();
-        const uint32_t idesc = make_idesc_tf32(TC_M, BN);
-        constexpr uint32_t A_LBO = (TC_M / 8) * 128, B_LBO = (BN / 8) * 128;
+    } else if (threadIdx.x < TC_THREADS) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int j = 0; j < BN / 2; ++j) acc[h][j] = 0.0f;
         for (int i = 0; i < kchunks; ++i) {
             const int s = i % ST;
             mbar_wait(smem_u32(&s_full[s]), (i / ST) & 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
             const uint32_t sa = smem_u32(smem + (size_t)s * dense_stage_floats(BN));
             const uint32_t sb = sa + 2 * A_BLK * 4;
+            wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < TC_KC / 8; ++k) {
-                const uint64_t ah = make_kmajor_desc(sa + k * 2 * A_LBO, A_LBO, 128);
-                const uint64_t al = make_kmajor_desc(sa + A_BLK * 4 + k * 2 * A_LBO, A_LBO, 128);
-                const uint64_t bh = make_kmajor_desc(sb + k * 2 * B_LBO, B_LBO, 128);
-                const uint64_t bl = make_kmajor_desc(sb + B_BLK * 4 + k * 2 * B_LBO, B_LBO, 128);
-                umma_tf32_p(tmem, ah, bh, idesc, (i | k) != 0, leader);
-                umma_tf32_p(tmem, ah, bl, idesc, true, leader);
-                umma_tf32_p(tmem, al, bh, idesc, true, leader);
-            }
-            // frees the stage when these MMAs have read it -- in every CTA that writes into it
-            if (CL) umma_commit_multicast_p(smem_u32(&s_empty[s]), (uint16_t)(mask_row | mask_col), leader);
-            else umma_commit_p(smem_u32(&s_empty[s]), leader);
+            for (int k = 0; k < TC_KC / 8; ++k)
+                mma_kstep_3xtf32<BN>(acc, sa + k * 2 * (TC_M / 8) * 128, A_BLK * 4, sb + k * 2 * (BN / 8) * 128, B_BLK * 4);
+            wgmma_commit();
+            wgmma_wait<1>();                                   // the previous chunk's group has read its stage
+            if (i > 0 && threadIdx.x == 0) mbar_arrive(smem_u32(&s_empty[(i - 1) % ST]));
         }
-        umma_commit_p(smem_u32(&s_done), leader);
+        wgmma_wait<0>();
     }
     __syncwarp();
-    mbar_wait(smem_u32(&s_done), 0);
-    if (CL) cluster_sync_all();          // no CTA leaves while a peer's release may still arrive on its barriers
+    __syncthreads();
 }
 
-// One leapfrog step for all chains:  acc = (Q - mu) P  on tcgen05, then kick / drift in the epilogue.
-//   grid (Dp/BN, Cp/128), 128 threads: thread 0 = TMA producer, thread 32 = MMA issuer, all 4 warps = epilogue.
-template <int BN, bool CL = false>
-__global__ void __launch_bounds__(TC_THREADS, 1)
+// The accumulator tile -> shared memory (row pitch BN + 4 floats), so that the epilogue can give each thread one row.
+template <int BN>
+__device__ __forceinline__ void dense_stage_acc(const float (&acc)[2][BN / 2], float* stg) {
+    if (threadIdx.x < TC_THREADS) {
+        const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int i = 0; i < BN / 2; i += 2) {
+                const int r = 64 * h + 16 * warp + (lane >> 2) + 8 * ((i >> 1) & 1), c = 8 * (i >> 2) + 2 * (lane & 3);
+                *reinterpret_cast<float2*>(stg + r * (BN + 4) + c) = make_float2(acc[h][i], acc[h][i + 1]);
+            }
+    }
+    __syncthreads();
+}
+__device__ __forceinline__ void stage_ld32(const float* src, uint32_t (&v)[32]) {
+#pragma unroll
+    for (int j = 0; j < 32; j += 4) {
+        const float4 t = *reinterpret_cast<const float4*>(src + j);
+        v[j] = __float_as_uint(t.x); v[j + 1] = __float_as_uint(t.y); v[j + 2] = __float_as_uint(t.z); v[j + 3] = __float_as_uint(t.w);
+    }
+}
+
+// One leapfrog step for all chains:  acc = (Q - mu) P  on the tensor cores, then kick / drift in the epilogue.
+//   grid (Dp/BN, Cp/128), 160 threads: warps 0-3 = MMA warpgroup + epilogue (one chain row each), thread 128 = TMA producer.
+template <int BN>
+__global__ void __launch_bounds__(DENSE_THREADS, 1)
 dense_step_kernel(const DenseArgs a, const float* __restrict__ Qin, const float* __restrict__ QpIn,
                   const float* __restrict__ Ppack, float* __restrict__ Qout, float* __restrict__ QpOut,
                   float* __restrict__ P, const float* __restrict__ eps, int mode, float* __restrict__ upart) {
     constexpr int ST = dense_stages(BN);
     extern __shared__ __align__(1024) float smem[];
-    __shared__ __align__(8) uint64_t s_full[ST], s_empty[ST], s_done;
-    __shared__ uint32_t s_tmem;
+    __shared__ __align__(8) uint64_t s_full[ST], s_empty[ST];
     pdl_launch_dependents();
     const int tile_n = blockIdx.x, tile_m = blockIdx.y;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int Dp = a.Dp, kchunks = Dp / TC_KC;
 
-    const uint32_t tmem = dense_prologue<BN, ST, CL>(s_full, s_empty, &s_done, &s_tmem);
+    dense_prologue<ST>(s_full, s_empty);
 
-    pdl_wait();               // everything above (barriers, TMEM) overlapped the previous launch's tail; its writes are visible now
-    dense_mainloop<BN, ST, CL>(smem, s_full, s_empty, &s_done, tmem, QpIn, Ppack, tile_m, tile_n, kchunks);
+    pdl_wait();               // the barrier set-up overlapped the previous launch's tail; its writes are visible now
+    float acc[2][BN / 2];
+    dense_mainloop<BN, ST>(smem, s_full, s_empty, acc, QpIn, Ppack, tile_m, tile_n, kchunks);
+    dense_stage_acc<BN>(acc, smem);
     // ===== epilogue: acc = ((Q-mu) P)[row, cols]; g = -acc; kick, optional drift (+ packed copy for the next GEMM) =====
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int row = tile_m * TC_M + warp * 32 + lane;
-    const bool live = row < a.C;
+    const int row = tile_m * TC_M + threadIdx.x;
+    const bool live = threadIdx.x < TC_THREADS && row < a.C;
+    const float* srow = smem + (size_t)threadIdx.x * (BN + 4);
     const float e = live ? eps[row] : 0.0f, half = mul(0.5f, e);
     const float ck = (mode == DENSE_FIRST) ? half : e;
     const bool drift = (mode == DENSE_FIRST || mode == DENSE_MIDDLE);
@@ -369,10 +306,9 @@ dense_step_kernel(const DenseArgs a, const float* __restrict__ Qin, const float*
     const size_t base = (size_t)row * Dp + (size_t)tile_n * BN;
 #pragma unroll 1
     for (int c0 = 0; c0 < BN; c0 += 32) {
-        uint32_t v[32];
-        const uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0;
-        tmem_ld32(taddr, v);
         if (live) {
+            uint32_t v[32];
+            stage_ld32(srow + c0, v);
             const int colbase = tile_n * BN + c0;                           // a 32-aligned column block = one K chunk
             float* qp_hi = QpOut + pack_block_base(tile_m, colbase / TC_KC, 0, kchunks, TC_M);
             float* qp_lo = QpOut + pack_block_base(tile_m, colbase / TC_KC, 1, kchunks, TC_M);
@@ -407,9 +343,6 @@ dense_step_kernel(const DenseArgs a, const float* __restrict__ Qin, const float*
         }
     }
     if (live && upart) upart[(size_t)row * a.NT + tile_n] = udot;
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem), "r"(BN < 32 ? 32 : BN));
 }
 
 
@@ -440,26 +373,26 @@ struct LinEpi {
     float sign;            // s = +1 / -1
 };
 
-template <int BN, bool CL = false>
-__global__ void __launch_bounds__(TC_THREADS, 1)
+template <int BN>
+__global__ void __launch_bounds__(DENSE_THREADS, 1)
 dense_lin_kernel(int C, int Dp, int NT, const float* __restrict__ Apack, const float* __restrict__ Bpack, const LinEpi ep) {
     constexpr int ST = dense_stages(BN);
     extern __shared__ __align__(1024) float smem[];
-    __shared__ __align__(8) uint64_t s_full[ST], s_empty[ST], s_done;
-    __shared__ uint32_t s_tmem;
+    __shared__ __align__(8) uint64_t s_full[ST], s_empty[ST];
     pdl_launch_dependents();
     const int tile_n = blockIdx.x, tile_m = blockIdx.y;
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int kchunks = Dp / TC_KC;
 
-    const uint32_t tmem = dense_prologue<BN, ST, CL>(s_full, s_empty, &s_done, &s_tmem);
+    dense_prologue<ST>(s_full, s_empty);
 
     pdl_wait();
-    dense_mainloop<BN, ST, CL>(smem, s_full, s_empty, &s_done, tmem, Apack, Bpack, tile_m, tile_n, kchunks);
+    float acc[2][BN / 2];
+    dense_mainloop<BN, ST>(smem, s_full, s_empty, acc, Apack, Bpack, tile_m, tile_n, kchunks);
+    dense_stage_acc<BN>(acc, smem);
 
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const int row = tile_m * TC_M + warp * 32 + lane;
-    const bool live = row < C;
+    const int row = tile_m * TC_M + threadIdx.x;
+    const bool live = threadIdx.x < TC_THREADS && row < C;
+    const float* srow = smem + (size_t)threadIdx.x * (BN + 4);
     const float e = (live && ep.eps) ? ep.eps[row] : 0.0f, half = mul(0.5f, e);
     const float k1 = (ep.k1 == LIN_K_HALF) ? half : e, k2 = (ep.k2 == LIN_K_HALF) ? half : e;
     const bool neg = ep.sign < 0.0f;
@@ -467,10 +400,9 @@ dense_lin_kernel(int C, int Dp, int NT, const float* __restrict__ Apack, const f
     const size_t base = (size_t)row * Dp + (size_t)tile_n * BN;
 #pragma unroll 1
     for (int c0 = 0; c0 < BN; c0 += 32) {
-        uint32_t v[32];
-        const uint32_t taddr = tmem + ((uint32_t)(warp * 32) << 16) + (uint32_t)c0;
-        tmem_ld32(taddr, v);
         if (live) {
+            uint32_t v[32];
+            stage_ld32(srow + c0, v);
             const int colbase = tile_n * BN + c0;                           // a 32-aligned column block = one K chunk
             float* xp_hi = ep.Xpack ? ep.Xpack + pack_block_base(tile_m, colbase / TC_KC, 0, kchunks, TC_M) : nullptr;
             float* xp_lo = ep.Xpack ? ep.Xpack + pack_block_base(tile_m, colbase / TC_KC, 1, kchunks, TC_M) : nullptr;
@@ -505,20 +437,14 @@ dense_lin_kernel(int C, int Dp, int NT, const float* __restrict__ Apack, const f
         }
     }
     if (live && ep.part) ep.part[(size_t)row * NT + tile_n] = dot;
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 0) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" :: "r"(tmem), "r"(BN < 32 ? 32 : BN));
 }
 
 static bool lin_launch(int BN, dim3 grid, cudaStream_t st, int C, int Dp, int NT, const float* Apack, const float* Bpack,
                        const LinEpi& ep) {
     const size_t sm = (size_t)dense_stages(BN) * dense_stage_floats(BN) * sizeof(float);
-    const bool cl = dense_cluster_ok(grid, BN);
-    if (BN == 128 && cl) launch_pdl_cluster(dense_lin_kernel<128, true>, grid, TC_THREADS, sm, st, C, Dp, NT, Apack, Bpack, ep);
-    else if (BN == 64 && cl) launch_pdl_cluster(dense_lin_kernel<64, true>, grid, TC_THREADS, sm, st, C, Dp, NT, Apack, Bpack, ep);
-    else if (BN == 128) launch_pdl(dense_lin_kernel<128>, grid, TC_THREADS, sm, st, C, Dp, NT, Apack, Bpack, ep);
-    else if (BN == 64) launch_pdl(dense_lin_kernel<64>, grid, TC_THREADS, sm, st, C, Dp, NT, Apack, Bpack, ep);
-    else launch_pdl(dense_lin_kernel<32>, grid, TC_THREADS, sm, st, C, Dp, NT, Apack, Bpack, ep);
+    if (BN == 128) launch_pdl(dense_lin_kernel<128>, grid, DENSE_THREADS, sm, st, C, Dp, NT, Apack, Bpack, ep);
+    else if (BN == 64) launch_pdl(dense_lin_kernel<64>, grid, DENSE_THREADS, sm, st, C, Dp, NT, Apack, Bpack, ep);
+    else launch_pdl(dense_lin_kernel<32>, grid, DENSE_THREADS, sm, st, C, Dp, NT, Apack, Bpack, ep);
     return true;
 }
 static bool lin_configure() {
@@ -529,10 +455,6 @@ static bool lin_configure() {
                                     (int)((size_t)dense_stages(64) * dense_stage_floats(64) * 4)) == cudaSuccess;
     ok = ok && cudaFuncSetAttribute(dense_lin_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                     (int)((size_t)dense_stages(32) * dense_stage_floats(32) * 4)) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(dense_lin_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)((size_t)dense_stages(128) * dense_stage_floats(128) * 4)) == cudaSuccess;
-    ok = ok && cudaFuncSetAttribute(dense_lin_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int)((size_t)dense_stages(64) * dense_stage_floats(64) * 4)) == cudaSuccess;
     if (!ok) cudaGetLastError();
     return ok;
 }
@@ -781,7 +703,7 @@ dense_kick_elem_kernel(const DenseArgs a, const float* __restrict__ Q, float* __
 }
 
 // sample() loop with a full (2-D) inv_mass at D > 16 (samplers.py:199, :294, :812): every drift, the momentum
-// refresh and both kinetic energies are (chains x D) . (D x D) GEMMs on tcgen05 (dense_lin_kernel); a GaussianFull
+// refresh and both kinetic energies are (chains x D) . (D x D) GEMMs on the tensor cores (dense_lin_kernel); a GaussianFull
 // target adds the gradient GEMM, GaussianIso / GaussianDiag kick element-wise.  2L+4 (L+3) GEMMs per iteration.
 // K / N padding to multiples of 32 (one K chunk); column-tile width = the widest of 128/64/32 that divides Dp and still
 // gives the GPU ~100 CTAs (each CTA re-streams its 128 chain rows)
@@ -969,19 +891,10 @@ int dense_hmc_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hm
 
     const dim3 ggrid(a.NT, mt);
     auto step = [&](const float* qin, const float* qpin, float* qout, float* qpout, int mode) -> bool {
-        const bool cl = dense_cluster_ok(ggrid, a.BN);
-        if (a.BN == 128) {
-            const size_t sm = (size_t)dense_stages(128) * dense_stage_floats(128) * sizeof(float);
-            if (cl) launch_pdl_cluster(dense_step_kernel<128, true>, ggrid, TC_THREADS, sm, st, a, qin, qpin, ppack, qout, qpout, P, eps, mode, upart);
-            else launch_pdl(dense_step_kernel<128>, ggrid, TC_THREADS, sm, st, a, qin, qpin, ppack, qout, qpout, P, eps, mode, upart);
-        } else if (a.BN == 64) {
-            const size_t sm = (size_t)dense_stages(64) * dense_stage_floats(64) * sizeof(float);
-            if (cl) launch_pdl_cluster(dense_step_kernel<64, true>, ggrid, TC_THREADS, sm, st, a, qin, qpin, ppack, qout, qpout, P, eps, mode, upart);
-            else launch_pdl(dense_step_kernel<64>, ggrid, TC_THREADS, sm, st, a, qin, qpin, ppack, qout, qpout, P, eps, mode, upart);
-        } else {
-            const size_t sm = (size_t)dense_stages(32) * dense_stage_floats(32) * sizeof(float);
-            launch_pdl(dense_step_kernel<32>, ggrid, TC_THREADS, sm, st, a, qin, qpin, ppack, qout, qpout, P, eps, mode, upart);
-        }
+        const size_t sm = (size_t)dense_stages(a.BN) * dense_stage_floats(a.BN) * sizeof(float);
+        if (a.BN == 128) launch_pdl(dense_step_kernel<128>, ggrid, DENSE_THREADS, sm, st, a, qin, qpin, ppack, qout, qpout, P, eps, mode, upart);
+        else if (a.BN == 64) launch_pdl(dense_step_kernel<64>, ggrid, DENSE_THREADS, sm, st, a, qin, qpin, ppack, qout, qpout, P, eps, mode, upart);
+        else launch_pdl(dense_step_kernel<32>, ggrid, DENSE_THREADS, sm, st, a, qin, qpin, ppack, qout, qpout, P, eps, mode, upart);
         return true;
     };
     {
@@ -992,10 +905,6 @@ int dense_hmc_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hm
                                         (int)((size_t)dense_stages(64) * dense_stage_floats(64) * 4)) == cudaSuccess;
         ok = ok && cudaFuncSetAttribute(dense_step_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                         (int)((size_t)dense_stages(32) * dense_stage_floats(32) * 4)) == cudaSuccess;
-        ok = ok && cudaFuncSetAttribute(dense_step_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        (int)((size_t)dense_stages(128) * dense_stage_floats(128) * 4)) == cudaSuccess;
-        ok = ok && cudaFuncSetAttribute(dense_step_kernel<64, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        (int)((size_t)dense_stages(64) * dense_stage_floats(64) * 4)) == cudaSuccess;
         if (!ok) { cudaGetLastError(); return HMCX_ERR_CUDA; }
     }
     dense_pad_matrix_kernel<<<296, 256, 0, st>>>(target->prec, D, prec, a.Dp);
@@ -1034,7 +943,7 @@ int dense_hmc_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hm
 // sampler=RMHMC on Gaussian targets without jitter: the metric G = -Hessian (HESSIAN) or its softabs map is the SAME
 // matrix at every point, so dH/dtheta = -grad log p(theta) and dH/dp = G^-1 p (samplers.py:389-462 through autograd of
 // :677-736), and every flow of the explicit integrator (A-B-C-B-A on the augmented state, :427-458) and of the
-// implicit one (:363-386; its fixed points converge in two sweeps) is a (chains x D).(D x D) GEMM on tcgen05 with the
+// implicit one (:363-386; its fixed points converge in two sweeps) is a (chains x D).(D x D) GEMM on the tensor cores with the
 // metric solve G^-1 p as one of them.  The host supplies G^-1, chol(G) (gibbs :183-184) and log det G, all computed
 // with the reference's torch ops.
 // ---------------------------------------------------------------------------------------------------------
@@ -1217,9 +1126,8 @@ int dense_rmhmc_run(const hmcx_target_t* target, const hmcx_rmhmc_t* cfg, const 
 }
 
 
-// NOTE (measured on B200): tf32 operands in MN-major form do NOT work with the no-swizzle canonical layout -- they need
-// the dedicated SWIZZLE_128B_BASE32B layout.  Every operand of this file is therefore kept K-major; an operand that an
-// epilogue produces "row per thread" is written transposed into its packed K-major block.
+// wgmma takes tf32 operands from shared memory in K-major form only: an operand that an epilogue produces "row per
+// thread" is written transposed into its packed K-major block.
 
 int gemm_nt_tf32x3(const float* A, const float* B, float* D, int M, int N, int K, cudaStream_t st) {
     if (!A || !B || !D || M < 1 || N < 1 || K < 1) return HMCX_ERR_INVALID_ARG;

@@ -1,4 +1,4 @@
-"""Host-side driver of the sm_100a kernels: turns descriptors + torch tensors into C-ABI calls (include/hmcx.h).
+"""Host-side driver of the sm_90a kernels: turns descriptors + torch tensors into C-ABI calls (include/hmcx.h).
 
 Everything here is plumbing -- device buffers, padding to the (C, ld) layout, the step-size adaptation table,
 the random-stream modes.  The arithmetic of the hot path lives in csrc/*.cu.
@@ -97,7 +97,7 @@ class NativeTarget:
             m.num_rows = xd.shape[0]
         m.num_splits = self.num_splits
         m.cluster_size = int(getattr(first, 'cluster_size', 0))      # 0 = auto; 1/2/4 pins CTAs per chain
-        m.tensor_cores = int(getattr(first, 'tensor_cores', 0))      # 0 = auto (tcgen05 when the shape fits); 1 = off
+        m.tensor_cores = int(getattr(first, 'tensor_cores', 0))      # 0 = auto (tensor cores when the shape fits); 1 = off
         for i, b in enumerate(begin):
             m.split_begin[i] = b
         self.mlp_struct = m
@@ -106,7 +106,7 @@ class NativeTarget:
         s.mlp = C.pointer(m)
         self.struct = s
         if x is not None and m.tensor_cores == 0 and self.device.type == 'cuda':
-            # tensor-core form: x as ready-made tcgen05 operands (tf32 hi | lo, both GEMM layouts), built once per target
+            # tensor-core form: x as ready-made tensor-core operands (tf32 hi | lo, both GEMM layouts), built once per target
             lib = N.load_library()
             nbytes = int(lib.hmcx_mlp_packed_x_bytes(C.byref(s)))
             if nbytes:
@@ -157,7 +157,7 @@ class NativeMass:
         elif isinstance(inv_mass, list):
             # block list (samplers.py:188-197, :287-292, :803-809, :944-947) == the block-diagonal 2-D inv_mass: every
             # block inverted and Cholesky-factorised on its own with the reference's torch ops, then laid out as ONE
-            # (D, D) operand pair for the full-mass kernels (thread-per-chain for D <= 16, tcgen05 dense_lin above)
+            # (D, D) operand pair for the full-mass kernels (thread-per-chain for D <= 16, tensor-core dense_lin above)
             blocks = [b.detach().to(torch.float32) for b in inv_mass]
             if any(b.dim() != 2 or b.shape[0] != b.shape[1] for b in blocks) or sum(b.shape[0] for b in blocks) != dim:
                 raise RuntimeError('block-list inv_mass: square blocks whose sizes add up to %d' % dim)
@@ -453,7 +453,6 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
             # windowed delivery: the run is cut into `host_windows` windows of iterations; each window's sample slots
             # leave for the pinned block through the COPY ENGINE on a second stream while the next window computes
             # (hmcx_copy_rows_async).  Costs a device staging block of the samples' size; delivers at the DMA rate
-            # (57 GB/s on B200/PCIe 5) where SM-issued stores to host memory reach ~52.5.
             host_out, out = out, None
         else:
             host_samples = True                    # caller-provided pinned sample block: the kernel streams into it
@@ -863,7 +862,7 @@ def rmhmc_hamiltonian(target, q, p, jitter=None, softabs_const=None, softabs=Fal
 
 
 def gemm_nt(A, B):
-    """D = A @ B.T on tcgen05 tensor cores with 3xTF32 split operands (fp32-accurate).  A (M,K), B (N,K) fp32 CUDA;
+    """D = A @ B.T on the tensor cores (wgmma) with 3xTF32 split operands (fp32-accurate).  A (M,K), B (N,K) fp32 CUDA;
     M, N multiples of 128, K a multiple of 32."""
     N.require_cuda()
     lib = N.load_library()

@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference's sampler surface (hamiltorch/samplers.py) on top of the sm_100a kernels.
+"""Host-side mirror of the reference's sampler surface (hamiltorch/samplers.py) on top of the sm_90a kernels.
 
 Same names, argument order, defaults and error behaviour as the reference for the hot path:
 ``sample`` (samplers.py:850), ``leapfrog`` (:205), ``hamiltonian`` (:738), ``gibbs`` (:152), ``acceptance``
@@ -333,7 +333,7 @@ def sample_chains(log_prob_func, params_init, num_samples=10, num_steps_per_samp
     straight into pinned host memory: ``.samples`` is then a CPU tensor (synchronise the stream before reading).
     ``out=<pinned host block>, host_windows=W`` (W >= 2) delivers into the caller's block through the copy engine instead:
     the run is cut into W windows of iterations and each window's sample slots go to the host on a second stream while the
-    next window computes (costs a device staging block; 57 instead of ~52.5 GB/s over PCIe 5 on B200).
+    next window computes (costs a device staging block).
     """
     if params_init.dim() != 2:
         raise RuntimeError('sample_chains: params_init must be (num_chains, D)')

@@ -1,7 +1,7 @@
 """Native target descriptors.
 
 The reference takes an opaque Python ``log_prob_func`` (samplers.py:857-858) and differentiates it with
-autograd (samplers.py:65).  An opaque callable cannot enter a CUDA kernel, so the B200 engine recognises a
+autograd (samplers.py:65).  An opaque callable cannot enter a CUDA kernel, so the engine recognises a
 small family of *descriptors*.  Every descriptor is
 
 * a valid reference ``log_prob_func`` (``__call__`` takes a 1-D tensor, returns a scalar, is written with plain
@@ -28,7 +28,7 @@ _LOG_2PI = math.log(2.0 * math.pi)
 
 
 class Target:
-    """Base class: a log-density the sm_100a kernels know how to differentiate."""
+    """Base class: a log-density the sm_90a kernels know how to differentiate."""
 
     kind = -1
     dim = 0
@@ -237,7 +237,7 @@ def mlp_spec(model):
                 raise NotImplementedError('an activation must follow a Linear layer')
             acts[-1] = _ACT_OF_MODULE[type(m).__name__]
         else:
-            raise NotImplementedError('unsupported layer for the B200 dense-stack kernel: %s' % type(m).__name__)
+            raise NotImplementedError('unsupported layer for the dense-stack kernel: %s' % type(m).__name__)
     if not linears:
         raise NotImplementedError('no Linear layer found')
     if acts[-1] != ACT_NONE:

@@ -1,5 +1,5 @@
 /*
- * hmcx.h -- C ABI of libhmcx.so, the B200 (sm_100a) batched-chain Hamiltonian Monte Carlo engine.
+ * hmcx.h -- C ABI of libhmcx.so, the H100 (sm_90a) batched-chain Hamiltonian Monte Carlo engine.
  *
  * Drop-in boundary for the hot path of AdamCobb/hamiltorch (reference, pure Python): the reference has no
  * FFI of its own, its boundary is the Python function surface (SURVEY.md section 8b).  Each entry point below
@@ -92,11 +92,11 @@ typedef struct hmcx_mlp {
     int32_t split_begin[HMCX_MLP_MAX_SPLITS + 1];
     int32_t cluster_size;                          /* CTAs (SMs) cooperating on one chain: 0 = automatic, 1 / 2 / 4 =
                                                       pinned (bit-reproducibility across chain counts)          */
-    int32_t tensor_cores;                          /* HMCX_MLP_TC_AUTO: first-layer GEMMs on tcgen05 (3xTF32, fp32-level
+    int32_t tensor_cores;                          /* HMCX_MLP_TC_AUTO: first-layer GEMMs on the tensor cores (3xTF32, fp32-level
                                                       accuracy) when the stack is n0 -> 128 -> nL with n0 in
                                                       {16,32,48,64}, nL <= 4; HMCX_MLP_TC_OFF: fp32 SIMT tiles  */
     const float* x_packed;                         /* device buffer of hmcx_mlp_packed_x_bytes() filled by hmcx_mlp_pack_x():
-                                                      x as ready-made tcgen05 operands (tf32 hi | lo, both GEMM layouts),
+                                                      x as ready-made tensor-core operands (tf32 hi | lo, both GEMM layouts),
                                                       one bulk TMA copy per tile.  NULL: fp32 SIMT tiles               */
 } hmcx_mlp_t;
 
@@ -322,7 +322,7 @@ int hmcx_split_leapfrog(const hmcx_target_t* target, const hmcx_mass_t* mass, co
 
 /*
  * Packed X operands of the BNN tensor-core path (hmcx_mlp_t.x_packed).  The data matrix of define_model_log_prob
- * (samplers.py:1093-1201) never changes during a run, so its tf32 hi / lo split and the two tcgen05 operand layouts
+ * (samplers.py:1093-1201) never changes during a run, so its tf32 hi / lo split and the two tensor-core operand layouts
  * (forward: rows x inputs, backward: inputs x rows) are built once per target:
  *   hmcx_mlp_packed_x_bytes   size of the buffer (0: this stack has no tensor-core form -- leave x_packed NULL)
  *   hmcx_mlp_pack_x           fills it from target->mlp->x on `stream` (x_packed itself is not read)
@@ -331,8 +331,8 @@ size_t hmcx_mlp_packed_x_bytes(const hmcx_target_t* target);
 int hmcx_mlp_pack_x(const hmcx_target_t* target, float* packed_out, void* stream);
 
 /*
- * hmcx_gemm_nt_tf32x3: D[M,N] = A[M,K] . B[N,K]^T on the 5th-generation tensor cores (tcgen05.mma kind::tf32 with
- * 3xTF32 split operands => fp32-accurate, fp32 accumulation in tensor memory).  Row-major fp32 device arrays;
+ * hmcx_gemm_nt_tf32x3: D[M,N] = A[M,K] . B[N,K]^T on the Hopper tensor cores (wgmma.mma_async tf32 with 3xTF32 split
+ * operands => fp32-accurate, fp32 accumulation in registers).  Row-major fp32 device arrays;
  * M, N multiples of 128, K a multiple of 32.  The dense contraction behind full-covariance targets / full mass
  * matrices at large D (grad log p of ALL chains = -(Q - mu) P: M = chains, N = K = D; samplers.py:294, :812).
  */
@@ -357,7 +357,7 @@ size_t hmcx_rmhmc_dense_workspace_bytes(int32_t C, int32_t D);
 
 /*
  * hmcx_rmhmc_dense_run == the sample() loop for sampler=RMHMC (as hmcx_rmhmc_run) for targets GAUSS_ISO / GAUSS_DIAG /
- * GAUSS_FULL of ANY dimension with cfg->jitter < 0 (None): every flow is a tcgen05 GEMM over all chains (3xTF32,
+ * GAUSS_FULL of ANY dimension with cfg->jitter < 0 (None): every flow is a tensor-core GEMM over all chains (3xTF32,
  * operands packed for 1-D bulk TMA), 8 per explicit leapfrog step.  workspace: hmcx_rmhmc_dense_workspace_bytes().
  * D <= 128 (and ld <= D rounded up to 32): the whole run is ONE persistent launch instead (hmcx_flow.cu: the matrices in
  * shared memory, a warp owns 1-4 chains, exact fp32 FMAs; the workspace is then unused; environment HMCX_FLOW_SMALL=0

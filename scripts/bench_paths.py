@@ -1,6 +1,6 @@
 """Secondary measurements (not the driver's bench line): BASELINE configs 3, 4, 5 on one GPU, device-timed with CUDA
 events, next to the oracle port (the reference's algorithm) on one host core for a bounded sample.
-    python scripts/bench_paths.py [base] [dense] [sat] > profiles/<round>_paths.jsonl
+    python scripts/bench_paths.py [base] [dense] [sat] > paths.jsonl
 """
 import json
 import os

@@ -1,5 +1,5 @@
 """Run ONE of BASELINE configs 3 / 4 / 5 (the same inputs as bench.py's other_configs) `reps` times and print the device
-time per launch -- the command ncu wraps for the per-config captures under profiles/.
+time per launch -- the command a profiler wraps for per-config captures.
     python scripts/run_cfg.py 3 [reps] [chains]"""
 import os
 import sys

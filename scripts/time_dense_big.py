@@ -16,4 +16,4 @@ for C, D in ((4096, 2048), (8192, 1024)):
     init = torch.randn(C, D, generator=g).cuda()
     S, L = 10, 10
     ms = timed(lambda: engine.hmc_run(tgt, init, S, L, 0.1, seed=5))
-    print(json.dumps(dict(cluster=os.environ.get('HMCX_DENSE_CLUSTER', '0'), C=C, D=D, us_per_step_launch=1e3 * ms / (S * (L + 1)), tflops=2.0*C*D*D*(L+1)*S/(ms*1e-3)/1e12)))
+    print(json.dumps(dict(C=C, D=D, us_per_step_launch=1e3 * ms / (S * (L + 1)), tflops=2.0*C*D*D*(L+1)*S/(ms*1e-3)/1e12)))

@@ -66,9 +66,9 @@ def main():
                 S_ = S
             ms, r, mv = run(kind, C, D, S_, L)
             cs = C * S_ * L / (ms * 1e-3)
-            # shared-memory roofline of the flow kernel: every warp-matvec streams D*D*4 bytes; 128 B/clk/SM * 148 SMs
+            # shared-memory roofline of the flow kernel: every warp-matvec streams D*D*4 bytes; 128 B/clk/SM * #SMs
             print('%-18s C=%5d D=%3d S=%3d L=%d  %-9s R=%-4s %9.3f ms  %.3g chain-steps/s  accept %.2f  matvecs/iter %d'
-                  % (kind, C, D, S_, L, 'flow' if env[0] == '1' else 'tcgen05', env[1] or 'auto', ms, cs,
+                  % (kind, C, D, S_, L, 'flow' if env[0] == '1' else 'gemm', env[1] or 'auto', ms, cs,
                      float(r.accepted.float().mean()), mv), flush=True)
 
 

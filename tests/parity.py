@@ -20,7 +20,7 @@ H_TOL_REL = 2e-6
 # ---------------------------------------------------------------------------------------------------------------------
 # Tolerances of the NON-bit-exact comparisons (RMHMC: closed form + Jacobi vs autograd through eigh; coupled / dense /
 # Bayesian-NN contractions: summation order) are set from MEASUREMENT, not from a guess: tests/golden/measured_errors.json
-# holds, per compared quantity (tag), the error max |a - d| / (1 + |d|) observed on B200 (regenerate: run the GPU tests with
+# holds, per compared quantity (tag), the error max |a - d| / (1 + |d|) observed on the H100 (regenerate: run the GPU tests with
 # HMCX_PARITY_REPORT=<file>.jsonl, then scripts/collect_parity.py).  A comparison passes when its error is within
 # TOL_FACTOR x that measurement (floor TOL_FLOOR, so that a re-ordered reduction does not flip a test), and never above the
 # test's ceiling -- the old blanket bound (2e-3 RMHMC, 2e-4 contractions).  A tag without a measurement uses the ceiling.
@@ -62,7 +62,7 @@ def assert_close(tag, actual, desired, ceiling):
         with open(rep, 'a') as f:
             f.write(json.dumps({'tag': tag, 'error': m}) + '\n')
     tol = tol_for(tag, ceiling)
-    assert m <= tol, '%s: error %.3g > tolerance %.3g (measured on B200: %s, ceiling %.3g)' % (
+    assert m <= tol, '%s: error %.3g > tolerance %.3g (measured: %s, ceiling %.3g)' % (
         tag, m, tol, MEASURED.get(tag), ceiling)
 
 # dual averaging (samplers.py:629-674): fp32 exp/log (CUDA libm vs Sleef, <= 2 ulp) and the summation-order noise of

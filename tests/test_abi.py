@@ -1,4 +1,4 @@
-"""CPU: the C-ABI library builds for sm_100a, loads, and exports every symbol include/hmcx.h declares.
+"""CPU: the C-ABI library builds for sm_90a, loads, and exports every symbol include/hmcx.h declares.
 No compute call needs a GPU here: argument validation returns before any CUDA work."""
 import ctypes as C
 import os
@@ -26,14 +26,14 @@ def test_header_symbols_exported(built_library):
     assert lib.hmcx_abi_version() == _native.ABI_VERSION
 
 
-def test_library_is_sm100a(built_library):
+def test_library_is_sm90a(built_library):
     import shutil
     import subprocess
     cuobjdump = shutil.which('cuobjdump') or '/usr/local/cuda/bin/cuobjdump'
     if not os.path.exists(cuobjdump):
         pytest.skip('cuobjdump not available')
     out = subprocess.run([cuobjdump, '-lelf', built_library], capture_output=True, text=True).stdout
-    assert 'sm_100a' in out, out
+    assert 'sm_90a' in out, out
 
 
 def test_invalid_arguments_are_rejected_without_cuda(built_library):

@@ -1,5 +1,5 @@
 """CPU: the reference arm of bench.py (the reference's algorithm on the host cores) prints ONE JSON line with the
-contract's keys, and the B200 arm refuses to run without a GPU instead of falling back to anything."""
+contract's keys, and the GPU arm refuses to run without a GPU instead of falling back to anything."""
 import json
 import os
 import subprocess
@@ -22,7 +22,7 @@ def test_reference_arm_json_contract():
     assert d['config']['workload'].startswith('BASELINE config 2')
     sys.path.insert(0, ROOT)
     import bench
-    assert d['config'] == bench.workload_config(1)            # key for key what the B200 arm reports
+    assert d['config'] == bench.workload_config(1)            # key for key what the GPU arm reports
     assert d['cpu_baseline']['kind'] == 'port' and d['cpu_baseline']['cores'] >= 1
     assert 'physical_cores' in d['cpu_baseline'] and 'iterations' in d['cpu_baseline']['sample']
     assert d['steps_completed'] == 1 and d['cut_short'] is False

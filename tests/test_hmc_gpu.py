@@ -71,7 +71,7 @@ def test_golden_chain_parity(name):
 
 def _is_small_dense(case):
     """16 < D <= 128 with a dense precision or a 2-D / block-list inv_mass: runs on the persistent small-D kernel
-    (hmcx_flow.cu) by default and on the step-synchronous tcgen05 path when HMCX_FLOW_SMALL=0."""
+    (hmcx_flow.cu) by default and on the step-synchronous tensor-core path when HMCX_FLOW_SMALL=0."""
     import hamiltorch_b200.targets as T
     tgt, im = case['target'], case['kw'].get('inv_mass')
     full_mass = isinstance(im, list) or (torch.is_tensor(im) and im.dim() == 2)
@@ -80,7 +80,7 @@ def _is_small_dense(case):
 
 @pytest.mark.parametrize('name', sorted(n for n, c in cases.plain_cases().items() if _is_small_dense(c)))
 def test_golden_chain_parity_tcgen05_path(name, monkeypatch):
-    """The golden chains of the small dense cases ALSO through the tcgen05 GEMM path (the default at D > 128)."""
+    """The golden chains of the small dense cases ALSO through the tensor-core GEMM path (the default at D > 128)."""
     monkeypatch.setenv('HMCX_FLOW_SMALL', '0')
     test_golden_chain_parity(name)
 

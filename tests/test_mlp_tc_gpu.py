@@ -1,5 +1,5 @@
-"""GPU tests of the tensor-core (tcgen05 / TMEM) first-layer path of the Bayesian-NN kernels: one-hidden-layer stacks
-n0 -> 128 -> nL run H^T = W1 X^T and dW1 = dH^T X as 3xTF32 UMMAs (hmcx_mlp.cu, "First-layer GEMMs on the 5th-generation
+"""GPU tests of the tensor-core (wgmma) first-layer path of the Bayesian-NN kernels: one-hidden-layer stacks
+n0 -> 128 -> nL run H^T = W1 X^T and dW1 = dH^T X as 3xTF32 wgmmas (hmcx_mlp.cu, "First-layer GEMMs on the Hopper
 tensor cores").  Checked against autograd through the reference's closure (targets.MLPTarget.__call__ restates
 samplers.py:1141-1188 with the same torch ops), against the fp32 SIMT kernels of the same library
 (hmcx_mlp_t.tensor_cores = HMCX_MLP_TC_OFF), and chain-by-chain against the oracle."""
@@ -61,6 +61,22 @@ def test_tc_gradient_and_log_prob_match_autograd_and_simt(n_in, n_out, act, task
     gs, lps = engine.grad_log_prob(descs_simt, q, split=-1)
     assert (g - gs).abs().max().item() <= TC_GRAD_RTOL * gs.abs().max().item()
     assert torch.allclose(lp, lps, rtol=2e-5, atol=1e-4)
+
+
+def test_tc_gradient_and_log_prob_are_deterministic():
+    """Two identical calls on the config-4 shape (64-128-1, four 256-row splits, i.e. four 64-row tiles per split) return
+    the same bits: the tensor-core gradient has a fixed summation order, so any difference is a race.  One CTA per chain,
+    so the 264 chains are 264 independent repetitions within one call."""
+    model, descs = _problem(21, 1024, 64, 1, 'ReLU', 'regression', 4)
+    D = descs[0].dim
+    torch.manual_seed(3)
+    q = hb.util.flatten(model).detach()[None] + 0.05 * torch.randn(264, D)
+    q[1:] = q[0]                                      # identical inputs across chains as well
+    for split in (0, 3, -1):
+        g1, lp1 = engine.grad_log_prob(descs, q, split=split)
+        g2, lp2 = engine.grad_log_prob(descs, q, split=split)
+        assert torch.equal(g1, g2) and torch.equal(lp1, lp2), split
+        assert bool((g1 == g1[0]).all()) and bool((lp1 == lp1[0]).all()), split
 
 
 @pytest.mark.parametrize('scheme,rows_per_split', [(N.SCHEME_SPLIT_SYM, 64), (N.SCHEME_SPLIT_SYM, 256),

@@ -1,5 +1,5 @@
 """GPU parity of the constant-metric RMHMC path (hmcx_rmhmc_dense_run: Gaussian targets, jitter=None, every flow a
-tcgen05 GEMM over all chains) against the live oracle -- which differentiates rm_hamiltonian by autograd through the
+tensor-core GEMM over all chains) against the live oracle -- which differentiates rm_hamiltonian by autograd through the
 Hessian, eigh and the Cholesky solve exactly like the reference (oracle/rmhmc_oracle.py).
 
 Tolerance: the kernel applies G^-1 as a matrix (3xTF32 GEMM), the reference solves two triangular systems per call:
@@ -14,7 +14,7 @@ from oracle import hmc_oracle as O, rmhmc_oracle as R
 from tests import parity
 
 pytestmark = pytest.mark.gpu
-RM_RTOL = 2e-3            # CEILING only: measured <= 8.6e-7 (flow kernel) / 2.1e-6 (tcgen05) -> tolerance 1e-5 .. 1.7e-5 (tests/parity.py)
+RM_RTOL = 2e-3            # CEILING only: per-quantity tolerances from measured errors (tests/parity.py)
 
 
 def _full_gaussian(D, seed):
@@ -39,7 +39,7 @@ CASES = {
 @pytest.mark.parametrize('name', sorted(CASES))
 def test_constant_metric_rmhmc_parity_vs_live_oracle(name, path, monkeypatch):
     # D <= 128: the persistent small-D kernel (hmcx_flow.cu, exact fp32 FMAs) by default; HMCX_FLOW_SMALL=0 keeps the
-    # step-synchronous tcgen05 GEMM path (the default above D = 128) under the same test
+    # step-synchronous tensor-core GEMM path (the default above D = 128) under the same test
     monkeypatch.setenv('HMCX_FLOW_SMALL', '1' if path == 'flow' else '0')
     cs = CASES[name]
     D, S, burn, C = cs['D'], 6, 2, 3
@@ -71,7 +71,7 @@ def test_constant_metric_rmhmc_parity_vs_live_oracle(name, path, monkeypatch):
         o = os_[c]
         assert not any(o['diverged'])
         ham = res.ham[c].cpu().numpy().astype(np.float64)
-        tag = 'rmhmc_const/%s/%s/c%d' % (name, path, c)            # tolerance = 8 x the error measured on B200 (tests/parity.py)
+        tag = 'rmhmc_const/%s/%s/c%d' % (name, path, c)            # tolerance = 8 x the measured error (tests/parity.py)
         parity.assert_close(tag + '/ham_old', ham[:, 0], np.array(o['ham_old']), RM_RTOL)
         parity.assert_close(tag + '/ham_new', ham[:, 1], np.array(o['ham_new']), RM_RTOL)
         m = parity.first_decision_mismatch(res.accepted[c].cpu().numpy(), o['accepted'])

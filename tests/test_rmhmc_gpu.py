@@ -17,7 +17,7 @@ from tests import parity
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
-RM_RTOL = 2e-3            # CEILING only: every compared quantity passes within 8x its error measured on B200 (tests/parity.py;
+RM_RTOL = 2e-3            # CEILING only: every compared quantity passes within 8x its measured error (tests/parity.py;
                           # 12 of 14 fixtures <= 1.3e-5, the chaotic ones up to 1.5e-3 on H of trajectories both sides reject)
 
 
@@ -78,7 +78,7 @@ def test_golden_chain_parity(name):
             assert not (div & ~rdiv).any()
         ok = ~div & ~rdiv & ~(dH_ref > 50.0)      # a blown-up trajectory (reject on both sides) has no meaningful H
         route = 'cta' if os.environ.get('HMCX_RMHMC_FORCE_CTA') == '1' else 'default'
-        tag = 'rmhmc/%s/%s/c%d' % (name, route, c)                 # tolerance = 8 x the error measured on B200 (tests/parity.py)
+        tag = 'rmhmc/%s/%s/c%d' % (name, route, c)                 # tolerance = 8 x the measured error (tests/parity.py)
         parity.assert_close(tag + '/ham_old', ham[ok, 0], d['ham_old_%d' % c][ok], RM_RTOL)
         parity.assert_close(tag + '/ham_new', ham[ok, 1], d['ham_new_%d' % c][ok], RM_RTOL)
         m = parity.first_decision_mismatch(res.accepted[c].cpu().numpy(), d['accepted_%d' % c])

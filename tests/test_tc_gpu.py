@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 / TMEM GEMM building block (3xTF32 split operands) against an fp64 reference."""
+"""GPU: the wgmma GEMM building block (3xTF32 split operands) against an fp64 reference."""
 import pytest
 import torch
 
@@ -35,7 +35,7 @@ def _corr_gaussian(D, seed):
 @pytest.mark.parametrize('D', [200, 96, 128])
 @pytest.mark.parametrize('variant', ['hmc', 'diag_mass', 'nuts'])
 def test_dense_gaussian_full_chain_parity_vs_live_oracle(variant, D):
-    """Full-covariance Gaussian at D=200 (> 16: the tcgen05 step-synchronous path, one GEMM over all chains per
+    """Full-covariance Gaussian at D=200 (> 16: the tensor-core step-synchronous path, one GEMM over all chains per
     leapfrog step) against the oracle under the injected stream.  The gradient is a 3xTF32 tensor-core contraction
     (~1e-6 relative), the reference's an fp32 mv: states agree to 2e-4, decisions identical."""
     import numpy as np
@@ -43,7 +43,7 @@ def test_dense_gaussian_full_chain_parity_vs_live_oracle(variant, D):
     from hamiltorch_b200 import engine
     from oracle import hmc_oracle as O
     from tests import parity
-    # D = 200: the tcgen05 step-synchronous path; D = 96 / 128: the persistent small-D kernel (hmcx_flow.cu) with 3 / 4
+    # D = 200: the tensor-core step-synchronous path; D = 96 / 128: the persistent small-D kernel (hmcx_flow.cu) with 3 / 4
     # register slots per lane
     C, S, L, burn = 5, 12, 6, 3
     tgt = _corr_gaussian(D, 1)
@@ -106,14 +106,14 @@ def _spd(D, seed, scale=1.0):
 @pytest.mark.parametrize('variant', ['full_target', 'diag_target', 'iso_target_nuts'])
 def test_full_inv_mass_large_d_chain_parity_vs_live_oracle(variant, D):
     """2-D inv_mass at D > 16 (samplers.py:199 gibbs through the Cholesky factor of inverse(inv_mass), :294 drift
-    q += eps*(M^-1 p), :812 kinetic): momentum refresh, every drift and both kinetic energies are tcgen05 GEMMs over
+    q += eps*(M^-1 p), :812 kinetic): momentum refresh, every drift and both kinetic energies are tensor-core GEMMs over
     all chains (dense_lin_kernel), the gradient one more GEMM (GaussianFull) or element-wise (GaussianIso / Diag).
     3xTF32 contractions vs the reference's fp32 matmuls: states to 2e-4, identical decisions."""
     import numpy as np
     import hamiltorch_b200.targets as T
     from oracle import hmc_oracle as O
     from tests import parity
-    C, S, L, burn = 4, 10, 5, 3            # D = 150: tcgen05 GEMMs; D = 96 / 128: the persistent small-D kernel
+    C, S, L, burn = 4, 10, 5, 3            # D = 150: tensor-core GEMMs; D = 96 / 128: the persistent small-D kernel
     nuts = variant.endswith('nuts')
     if variant == 'full_target':
         tgt = _corr_gaussian(D, 11)
