@@ -63,6 +63,38 @@ __device__ __forceinline__ uint4 philox_draw(const PhiloxKeys& K, uint64_t chain
     return c;
 }
 
+// A persistent kernel draws the same (vec, stream, chain) counter at every iteration: only the iteration's low word
+// changes (iter < 2^32, so the high word is 0).  Everything of rounds 1-3 that does not depend on it is computed once per
+// thread: in round 1 all but the XOR with iter, in round 2 the product of word z, in round 3 the product of word x and
+// the XORs with the key.  philox_draw(K, PhiloxFixed, iter) then yields the bits of philox_draw(K, chain, iter, vec, stream).
+struct PhiloxFixed { uint32_t x1, w1k, y2k, z3k, w3; };
+__device__ __forceinline__ void philox_fix(const PhiloxKeys& K, uint64_t chain, uint32_t vec, uint32_t stream,
+                                           PhiloxFixed& F) {
+    const uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u;
+    const uint32_t cz = stream << 24;
+    const uint32_t x1 = __umulhi(M1, cz) ^ K.x[0], y1 = M1 * cz;              // round 1 (x1 ^ iter is the real x)
+    const uint32_t z1 = __umulhi(M0, vec) ^ (uint32_t)chain ^ K.y[0], w1 = M0 * vec;
+    const uint32_t x2 = __umulhi(M1, z1) ^ y1 ^ K.x[1], y2 = M1 * z1;        // round 2
+    F.x1 = x1;
+    F.w1k = w1 ^ K.y[1];
+    F.y2k = y2 ^ K.x[2];                                                      // round 3
+    F.z3k = __umulhi(M0, x2) ^ K.y[2];
+    F.w3 = M0 * x2;
+}
+__device__ __forceinline__ uint4 philox_draw(const PhiloxKeys& K, const PhiloxFixed& F, uint32_t iter) {
+    const uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u;
+    const uint32_t x1 = F.x1 ^ iter;
+    const uint32_t z2 = __umulhi(M0, x1) ^ F.w1k, w2 = M0 * x1;
+    uint4 c = make_uint4(__umulhi(M1, z2) ^ F.y2k, M1 * z2, F.z3k ^ w2, F.w3);
+#pragma unroll
+    for (int r = 3; r < 10; ++r) {
+        const uint32_t hi0 = __umulhi(M0, c.x), lo0 = M0 * c.x;
+        const uint32_t hi1 = __umulhi(M1, c.z), lo1 = M1 * c.z;
+        c = make_uint4(hi1 ^ c.y ^ K.x[r], lo1, hi0 ^ c.w ^ K.y[r], lo0);
+    }
+    return c;
+}
+
 __device__ __forceinline__ uint4 philox_draw(uint64_t seed, uint64_t chain, uint64_t iter, uint32_t vec,
                                              uint32_t stream) {
     uint4 c = make_uint4(vec, (uint32_t)iter, (uint32_t)(iter >> 32) | (stream << 24), (uint32_t)chain);
@@ -102,10 +134,11 @@ __device__ __forceinline__ void philox_normal2(uint64_t seed, uint64_t chain, ui
     if (pair & 1) box_muller(r.z, r.w, z[0], z[1]);
     else box_muller(r.x, r.y, z[0], z[1]);
 }
-// the same streams from a precomputed key schedule
-template <int E> __device__ __forceinline__ void philox_normals(const PhiloxKeys& K, uint64_t chain, uint64_t iter,
+// the same streams from a precomputed key schedule and the thread's fixed rounds (F from philox_fix with
+// vec = E == 4 ? grp : grp >> 1, STREAM_MOMENTUM)
+template <int E> __device__ __forceinline__ void philox_normals(const PhiloxKeys& K, const PhiloxFixed& F, uint32_t iter,
                                                                 uint32_t grp, float* z) {
-    const uint4 r = philox_draw(K, chain, iter, E == 4 ? grp : grp >> 1, STREAM_MOMENTUM);
+    const uint4 r = philox_draw(K, F, iter);
     if (E == 4) {
         box_muller(r.x, r.y, z[0], z[1]);
         box_muller(r.z, r.w, z[2], z[3]);

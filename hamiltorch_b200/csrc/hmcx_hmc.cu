@@ -77,26 +77,27 @@ __device__ __forceinline__ float kterm1(float p, float im) {
     if (MK == HMCX_MASS_NONE) return mul(p, p);
     return mul(p, mul(im, p));
 }
+// s + x for the terms of a per-thread partial sum (s = 0 before the first).  A first term that is a square is never -0,
+// so 0 + x == x bit for bit and the sum starts with it: the ISO potential and the kinetic term without a mass matrix.
+template <bool SQUARE>
+__device__ __forceinline__ float sum_in(float s, float x, bool first) { return (SQUARE && first) ? x : add(s, x); }
 
 // log p from the reduced sum, targets.py op order: -0.5*sum (+ log_norm)
 __device__ __forceinline__ float log_prob_from_sum(float s, float log_norm) { return add(mul(-0.5f, s), log_norm); }
 
 // One group of E elements through a whole trajectory (samplers.py:281-302).  Optionally records the L clones.
+// The gradient is recomputed for the final half-kick rather than carried out of the step loop: the same value, and a
+// loop-carried g would have to be materialised (one negation or more per element and step) on every trip.
 template <int TK, int MK, int E, bool TRAJ>
 __device__ __forceinline__ void trajectory(float* q, float* p, const VecConst<E>& c, float eps, float half, int L,
                                            float* q_traj, float* p_traj, size_t traj_stride) {
-    float g[E];
 #pragma unroll
-    for (int j = 0; j < E; ++j) {
-        g[j] = grad1<TK>(q[j], c.mean[j], c.ivar[j]);
-        p[j] = add(p[j], mul(half, g[j]));                                   // :281
-    }
+    for (int j = 0; j < E; ++j) p[j] = add(p[j], mul(half, grad1<TK>(q[j], c.mean[j], c.ivar[j])));   // :281
     auto one_step = [&](int l) {
 #pragma unroll
         for (int j = 0; j < E; ++j) {
             q[j] = drift1<MK>(q[j], eps, c.im[j], p[j]);                     // :284 / :296
-            g[j] = grad1<TK>(q[j], c.mean[j], c.ivar[j]);                    // :297
-            p[j] = add(p[j], mul(eps, g[j]));                                // :298
+            p[j] = add(p[j], mul(eps, grad1<TK>(q[j], c.mean[j], c.ivar[j])));   // :297-298
         }
         if (TRAJ) {
             if (l + 1 < L) {                                                 // :299-300
@@ -112,7 +113,7 @@ __device__ __forceinline__ void trajectory(float* q, float* p, const VecConst<E>
                                                                              // inside the instruction cache
     if (l < L) one_step(l);
 #pragma unroll
-    for (int j = 0; j < E; ++j) p[j] = sub(p[j], mul(half, g[j]));           // :302
+    for (int j = 0; j < E; ++j) p[j] = sub(p[j], mul(half, grad1<TK>(q[j], c.mean[j], c.ivar[j])));   // :302
     if (TRAJ) {
         stE_stream<E>(q_traj + (size_t)(L - 1) * traj_stride, q);
         stE_stream<E>(p_traj + (size_t)(L - 1) * traj_stride, p);
@@ -172,7 +173,13 @@ __device__ __forceinline__ void comp_add(float& s, float& c, float x) {
 // block_sum3 for CTAs of at most 8 warps: the second level reads the warps' partials with broadcast LDS.128 and adds them
 // in warp order (3 independent 8-term chains) instead of a second shuffle butterfly: ~90 cycles less latency on the
 // per-iteration critical path, same instruction count, every thread ends with the same bits.
-// `sbuf` holds 4*8+1 floats; callers alternate between two buffers on consecutive calls.
+// `sbuf` holds 4*8+1 floats; callers alternate between two buffers on consecutive calls.  The slots of the warps the CTA
+// does not have hold -0.0f (block_sum3_small_init): x + -0 == x for every x, so the second level adds all 8 slots
+// without re-deriving from blockDim which warps exist.
+__device__ __forceinline__ void block_sum3_small_init(float (*sbuf)[100]) {
+    const int nwarp = (blockDim.x + 31) >> 5;
+    if ((int)threadIdx.x >= 4 * nwarp && threadIdx.x < 32) sbuf[0][threadIdx.x] = sbuf[1][threadIdx.x] = -0.0f;
+}
 __device__ __forceinline__ void block_sum3_small(float& a, float& b, float& c, float& extra, float* sbuf) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = (blockDim.x + 31) >> 5;
     if (nwarp == 1) {
@@ -188,10 +195,8 @@ __device__ __forceinline__ void block_sum3_small(float& a, float& b, float& c, f
     a = v.x; b = v.y; c = v.z;
 #pragma unroll
     for (int w = 1; w < 8; ++w) {
-        if (w < nwarp) {
-            v = *reinterpret_cast<const float4*>(sbuf + 4 * w);
-            a = add(a, v.x); b = add(b, v.y); c = add(c, v.z);
-        }
+        v = *reinterpret_cast<const float4*>(sbuf + 4 * w);
+        a = add(a, v.x); b = add(b, v.y); c = add(c, v.z);
     }
     extra = sbuf[32];
 }
@@ -281,6 +286,7 @@ hmc_run_kernel(const RunArgs a) {
     VecConst<E> vc[K];
     float qc[K][E], q[K][E], p[K][E];
     bool live[K];                 // group lies inside the padded row
+    uint32_t zmask[K][E];         // ~0 for an element of the chain, 0 for padding (whose normals are zeroed)
 #pragma unroll
     for (int k = 0; k < K; ++k) {
         const int e0 = E * (gt + k * G);
@@ -288,9 +294,12 @@ hmc_run_kernel(const RunArgs a) {
         load_consts<TK, MK, E>(t, e0, vc[k]);
         if (live[k]) ldE<E>(a.q_cur + row + e0, qc[k]);
 #pragma unroll
-        for (int j = 0; j < E; ++j)
+        for (int j = 0; j < E; ++j) {
             if (!live[k] || e0 + j >= D) qc[k][j] = 0.0f;
+            zmask[k][j] = e0 + j < D ? 0xFFFFFFFFu : 0u;
+        }
     }
+    if (CS == 1 && MAXT <= 256) block_sum3_small_init(s_red);
 
     // U(q_cur) once; afterwards it is carried (the reference recomputes the identical value, :971)
     float lp_cur;
@@ -345,7 +354,15 @@ hmc_run_kernel(const RunArgs a) {
     // that the Philox/Box-Muller arithmetic of iteration n+1 overlaps the shuffle/barrier latency of iteration n
     float zn[K][E];
     PhiloxKeys keys;
-    if (PHILOX) philox_make_keys(a.seed, chain_id, keys);
+    PhiloxFixed pfix[K];
+    if (PHILOX) {
+        philox_make_keys(a.seed, chain_id, keys);
+#pragma unroll
+        for (int k = 0; k < K; ++k) {
+            const uint32_t grp = gt + k * G;
+            philox_fix(keys, chain_id, E == 4 ? grp : grp >> 1, STREAM_MOMENTUM, pfix[k]);
+        }
+    }
     auto draw = [&](int n) {
 #pragma unroll
         for (int k = 0; k < K; ++k) {
@@ -353,14 +370,13 @@ hmc_run_kernel(const RunArgs a) {
 #pragma unroll
             for (int j = 0; j < E; ++j) zn[k][j] = 0.0f;
             if (PHILOX) {
-                philox_normals<E>(keys, chain_id, (uint64_t)n, (uint32_t)grp, zn[k]);
+                philox_normals<E>(keys, pfix[k], (uint32_t)n, (uint32_t)grp, zn[k]);
             } else if (live[k]) {
                 if (a.rng_mode == HMCX_RNG_INJECTED) ldE_stream<E>(a.normals + ((size_t)(n - a.it0) * t.C + c) * ld + e0, zn[k]);
                 else philox_normals<E>(a.seed, chain_id, (uint64_t)n, (uint32_t)grp, zn[k]);
             }
 #pragma unroll
-            for (int j = 0; j < E; ++j)
-                if (e0 + j >= D) zn[k][j] = 0.0f;
+            for (int j = 0; j < E; ++j) zn[k][j] = __uint_as_float(__float_as_uint(zn[k][j]) & zmask[k][j]);
         }
     };
     if (a.it0 < a.it1) draw(a.it0);
@@ -400,7 +416,7 @@ hmc_run_kernel(const RunArgs a) {
 #pragma unroll
             for (int j = 0; j < E; ++j) {
                 p[k][j] = (MK == HMCX_MASS_DIAG) ? mul(zn[k][j], vc[k].sd[j]) : zn[k][j];
-                kin0 = add(kin0, kterm1<MK>(p[k][j], vc[k].im[j]));
+                kin0 = sum_in<MK == HMCX_MASS_NONE>(kin0, kterm1<MK>(p[k][j], vc[k].im[j]), k == 0 && j == 0);
                 q[k][j] = qc[k][j];
             }
         }
@@ -414,8 +430,8 @@ hmc_run_kernel(const RunArgs a) {
         for (int k = 0; k < K; ++k)
 #pragma unroll
             for (int j = 0; j < E; ++j) {
-                r1 = add(r1, uterm1<TK>(q[k][j], vc[k].mean[j], vc[k].ivar[j]));
-                r2 = add(r2, kterm1<MK>(p[k][j], vc[k].im[j]));
+                r1 = sum_in<TK == HMCX_TARGET_GAUSS_ISO>(r1, uterm1<TK>(q[k][j], vc[k].mean[j], vc[k].ivar[j]), k == 0 && j == 0);
+                r2 = sum_in<MK == HMCX_MASS_NONE>(r2, kterm1<MK>(p[k][j], vc[k].im[j]), k == 0 && j == 0);
             }
         // next iteration's normals: independent work.  In Philox mode the draw is branch-free and unconditional (one
         // unused draw after the last iteration) so that it shares a basic block with the reduction's shuffle chain.
