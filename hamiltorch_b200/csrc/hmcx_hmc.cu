@@ -120,6 +120,35 @@ __device__ __forceinline__ void trajectory(float* q, float* p, const VecConst<E>
     }
 }
 
+// The same trajectory for NG groups of one thread in one step loop: every trip advances all NG*E elements, so a thread
+// with two groups runs 8 independent element chains per step instead of two loops of 4.  Element-wise, so the bits are
+// those of trajectory<> on each group.
+template <int TK, int MK, int E, int NG>
+__device__ __forceinline__ void trajectory_groups(float (*q)[E], float (*p)[E], const VecConst<E>* c, float eps,
+                                                  float half, int L) {
+#pragma unroll
+    for (int g = 0; g < NG; ++g)
+#pragma unroll
+        for (int j = 0; j < E; ++j) p[g][j] = add(p[g][j], mul(half, grad1<TK>(q[g][j], c[g].mean[j], c[g].ivar[j])));
+    auto one_step = [&]() {
+#pragma unroll
+        for (int g = 0; g < NG; ++g)
+#pragma unroll
+            for (int j = 0; j < E; ++j) {
+                q[g][j] = drift1<MK>(q[g][j], eps, c[g].im[j], p[g][j]);
+                p[g][j] = add(p[g][j], mul(eps, grad1<TK>(q[g][j], c[g].mean[j], c[g].ivar[j])));
+            }
+    };
+    int l = 0;
+#pragma unroll 1
+    for (; l + 2 <= L; l += 2) { one_step(); one_step(); }
+    if (l < L) one_step();
+#pragma unroll
+    for (int g = 0; g < NG; ++g)
+#pragma unroll
+        for (int j = 0; j < E; ++j) p[g][j] = sub(p[g][j], mul(half, grad1<TK>(q[g][j], c[g].mean[j], c[g].ivar[j])));
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // persistent sample() kernel
 // ---------------------------------------------------------------------------------------------------------
@@ -175,10 +204,21 @@ __device__ __forceinline__ void comp_add(float& s, float& c, float x) {
 // per-iteration critical path, same instruction count, every thread ends with the same bits.
 // `sbuf` holds 4*8+1 floats; callers alternate between two buffers on consecutive calls.  The slots of the warps the CTA
 // does not have hold -0.0f (block_sum3_small_init): x + -0 == x for every x, so the second level adds all 8 slots
-// without re-deriving from blockDim which warps exist.
-__device__ __forceinline__ void block_sum3_small_init(float (*sbuf)[100]) {
+// without re-deriving from blockDim which warps exist.  `groups` = partial sums per thread (block_sum3_pair: 2).
+__device__ __forceinline__ void block_sum3_small_init(float (*sbuf)[100], int groups = 1) {
     const int nwarp = (blockDim.x + 31) >> 5;
-    if ((int)threadIdx.x >= 4 * nwarp && threadIdx.x < 32) sbuf[0][threadIdx.x] = sbuf[1][threadIdx.x] = -0.0f;
+    if ((int)threadIdx.x >= 4 * groups * nwarp && threadIdx.x < 32) sbuf[0][threadIdx.x] = sbuf[1][threadIdx.x] = -0.0f;
+}
+// second level: every thread adds the 8 slots in warp order
+__device__ __forceinline__ void block_sum3_slots(float& a, float& b, float& c, float& extra, const float* sbuf) {
+    float4 v = *reinterpret_cast<const float4*>(sbuf);
+    a = v.x; b = v.y; c = v.z;
+#pragma unroll
+    for (int w = 1; w < 8; ++w) {
+        v = *reinterpret_cast<const float4*>(sbuf + 4 * w);
+        a = add(a, v.x); b = add(b, v.y); c = add(c, v.z);
+    }
+    extra = sbuf[32];
 }
 __device__ __forceinline__ void block_sum3_small(float& a, float& b, float& c, float& extra, float* sbuf) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = (blockDim.x + 31) >> 5;
@@ -191,14 +231,51 @@ __device__ __forceinline__ void block_sum3_small(float& a, float& b, float& c, f
     if ((lane & 7) == 0 && lane < 24) sbuf[4 * warp + (lane >> 3)] = a;
     if (threadIdx.x == 0) sbuf[32] = extra;
     __syncthreads();
-    float4 v = *reinterpret_cast<const float4*>(sbuf);
-    a = v.x; b = v.y; c = v.z;
+    block_sum3_slots(a, b, c, extra, sbuf);
+}
+
+// The same sums for a CTA of at most 4 warps whose threads hold two element groups (K=2), each with its own partial
+// (a[k], b[k], c[k]).  Group k of thread t takes the place of lane t&31 of warp (t>>5) + k*nwarp in the CTA of twice
+// as many threads with one group each, so the sums have that CTA's block_sum3_small tree and bits.
+// publish: one packed butterfly over both groups' 6 values with warp_sum3's xor pairing (16, 8, 4, 2, 1) for each,
+// 8 shuffles instead of 2 x 6; lanes 0/4/8 end with group 0's a/b/c, lanes 16/20/24 with group 1's.  Then the 6 slots
+// and the extra scalar are stored.  The caller puts independent work between publish and collect.
+__device__ __forceinline__ void block_sum3_pair_publish(const float (&a)[2], const float (&b)[2], const float (&c)[2],
+                                                        float extra, float* sbuf) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = (blockDim.x + 31) >> 5;
+    const bool h16 = lane & 16, h8 = lane & 8, h4 = lane & 4;
+    // xor 16: lanes [0,16) keep group 0's three values, lanes [16,32) group 1's
+    const float x0 = add(h16 ? a[1] : a[0], __shfl_xor_sync(0xffffffffu, h16 ? a[0] : a[1], 16));
+    float x1 = add(h16 ? b[1] : b[0], __shfl_xor_sync(0xffffffffu, h16 ? b[0] : b[1], 16));
+    const float x2 = add(h16 ? c[1] : c[0], __shfl_xor_sync(0xffffffffu, h16 ? c[0] : c[1], 16));
+    // xor 8: lanes with bit 8 clear finish a, set finish c; both halves finish b
+    float k = add(h8 ? x2 : x0, __shfl_xor_sync(0xffffffffu, h8 ? x0 : x2, 8));
+    x1 = add(x1, __shfl_xor_sync(0xffffffffu, x1, 8));
+    // xor 4: lanes with bit 4 clear keep a / c, set keep b
+    k = add(h4 ? x1 : k, __shfl_xor_sync(0xffffffffu, h4 ? k : x1, 4));
+    k = add(k, __shfl_xor_sync(0xffffffffu, k, 2));
+    k = add(k, __shfl_xor_sync(0xffffffffu, k, 1));
+    if ((lane & 3) == 0 && (lane & 12) != 12) sbuf[4 * (warp + (lane >> 4) * nwarp) + ((lane >> 2) & 3)] = k;
+    if (threadIdx.x == 0) sbuf[32] = extra;
+}
+__device__ __forceinline__ void block_sum3_pair_collect(float& a, float& b, float& c, float& extra, const float* sbuf) {
+    __syncthreads();
+    block_sum3_slots(a, b, c, extra, sbuf);
+}
+
+// block_sum<1> with the same correspondence for a thread holding K partials: partial k is lane t&31 of warp
+// (t>>5) + k*nwarp.  `sbuf` holds 32 floats.
+template <int K>
+__device__ __forceinline__ float block_sum1_groups(float (&v)[K], float* sbuf) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = (blockDim.x + 31) >> 5;
 #pragma unroll
-    for (int w = 1; w < 8; ++w) {
-        v = *reinterpret_cast<const float4*>(sbuf + 4 * w);
-        a = add(a, v.x); b = add(b, v.y); c = add(c, v.z);
+    for (int k = 0; k < K; ++k) v[k] = warp_sum(v[k]);
+    if (lane == 0) {
+#pragma unroll
+        for (int k = 0; k < K; ++k) sbuf[warp + k * nwarp] = v[k];
     }
-    extra = sbuf[32];
+    __syncthreads();
+    return warp_sum(lane < K * nwarp ? sbuf[lane] : 0.0f);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -266,10 +343,16 @@ constexpr int run_max_threads(int E, int K) { return (E * K <= 4) ? 1024 : (E * 
 // sit in one basic block and the scheduler interleaves them.
 // CS > 1: the chain is owned by a cluster of CS CTAs (see above); CTA `rank` holds float4 groups [rank*G, (rank+1)*G).
 // NUTS = false compiles the dual-averaging path out (the plain sample() loop then carries no trace of it).
+// K = 2 with MAXT <= 128 (PAIR): every group keeps its own partial sums and enters the reductions in the place it has
+// in the K = 1 CTA of twice the threads (block_sum3_pair_*, block_sum1_groups), so the run is bit-identical to that
+// geometry; the other K > 1 forms sum their groups per thread first (a different tree).
 template <int TK, int MK, int E, int K, int MAXT, bool SINK = false, bool PHILOX = false, int CS = 1, bool NUTS = true>
 __global__ void __launch_bounds__(MAXT)
 hmc_run_kernel(const RunArgs a) {
     static_assert(CS == 1 || (K == 1 && !SINK), "cluster form: one group per thread, no sink");
+    constexpr bool PAIR = K == 2 && MAXT <= 128 && CS == 1;
+    constexpr int KP = PAIR ? K : 1;                          // partial sums per thread
+    static_assert(!PAIR || E == 4, "the paired form mirrors the float4 (K = 1) geometry");
     __shared__ __align__(16) float s_red[2][100];
     __shared__ __align__(16) float4 s_part[3][8];           // CS > 1: per-warp partials (two iteration parities + misc)
     __shared__ float s_eps[2];
@@ -299,17 +382,21 @@ hmc_run_kernel(const RunArgs a) {
             zmask[k][j] = e0 + j < D ? 0xFFFFFFFFu : 0u;
         }
     }
-    if (CS == 1 && MAXT <= 256) block_sum3_small_init(s_red);
+    if (CS == 1 && MAXT <= 256) block_sum3_small_init(s_red, KP);
 
     // U(q_cur) once; afterwards it is carried (the reference recomputes the identical value, :971)
     float lp_cur;
     {
-        float r[1] = {0.0f};
+        float r[KP];
+#pragma unroll
+        for (int i = 0; i < KP; ++i) r[i] = 0.0f;
 #pragma unroll
         for (int k = 0; k < K; ++k)
 #pragma unroll
-            for (int j = 0; j < E; ++j) r[0] = add(r[0], uterm1<TK>(qc[k][j], vc[k].mean[j], vc[k].ivar[j]));
-        if (CS > 1) r[0] = cluster_sum1<CS>(r[0], s_part[2]);
+            for (int j = 0; j < E; ++j)
+                r[PAIR ? k : 0] = add(r[PAIR ? k : 0], uterm1<TK>(qc[k][j], vc[k].mean[j], vc[k].ivar[j]));
+        if constexpr (PAIR) r[0] = block_sum1_groups<KP>(r, s_red[1]);
+        else if (CS > 1) r[0] = cluster_sum1<CS>(r[0], s_part[2]);
         else block_sum<1>(r, s_red[1]);
         lp_cur = log_prob_from_sum(r[0], t.log_norm);
         __syncthreads();
@@ -410,39 +497,55 @@ hmc_run_kernel(const RunArgs a) {
             logu = __shfl_sync(0xffffffffu, logu_lanes, phase);
         }
         // ---- gibbs (:969): p = z (*sqrt(mass)) ----
-        float kin0 = 0.0f;
+        // partial sums: index k for group k in the paired form, index 0 for all groups otherwise
+        float r0[KP], r1[KP], r2[KP];
+#pragma unroll
+        for (int i = 0; i < KP; ++i) { r0[i] = 0.0f; r1[i] = 0.0f; r2[i] = 0.0f; }
 #pragma unroll
         for (int k = 0; k < K; ++k) {
+            const int i = PAIR ? k : 0;
+            const bool first = i == k;                               // the partial's first group
 #pragma unroll
             for (int j = 0; j < E; ++j) {
                 p[k][j] = (MK == HMCX_MASS_DIAG) ? mul(zn[k][j], vc[k].sd[j]) : zn[k][j];
-                kin0 = sum_in<MK == HMCX_MASS_NONE>(kin0, kterm1<MK>(p[k][j], vc[k].im[j]), k == 0 && j == 0);
+                r0[i] = sum_in<MK == HMCX_MASS_NONE>(r0[i], kterm1<MK>(p[k][j], vc[k].im[j]), first && j == 0);
                 q[k][j] = qc[k][j];
             }
         }
         // ---- leapfrog (:973) : thread-private ----
+        if (PAIR) {
+            trajectory_groups<TK, MK, E, K>(q, p, vc, eps, half, a.L);
+        } else {
 #pragma unroll
-        for (int k = 0; k < K; ++k)
-            trajectory<TK, MK, E, false>(q[k], p[k], vc[k], eps, half, a.L, nullptr, nullptr, 0);
+            for (int k = 0; k < K; ++k)
+                trajectory<TK, MK, E, false>(q[k], p[k], vc[k], eps, half, a.L, nullptr, nullptr, 0);
+        }
         // ---- both Hamiltonians with one fused reduction (:971, :995) ----
-        float r0 = kin0, r1 = 0.0f, r2 = 0.0f;
 #pragma unroll
-        for (int k = 0; k < K; ++k)
+        for (int k = 0; k < K; ++k) {
+            const int i = PAIR ? k : 0;
+            const bool first = i == k;
 #pragma unroll
             for (int j = 0; j < E; ++j) {
-                r1 = sum_in<TK == HMCX_TARGET_GAUSS_ISO>(r1, uterm1<TK>(q[k][j], vc[k].mean[j], vc[k].ivar[j]), k == 0 && j == 0);
-                r2 = sum_in<MK == HMCX_MASS_NONE>(r2, kterm1<MK>(p[k][j], vc[k].im[j]), k == 0 && j == 0);
+                r1[i] = sum_in<TK == HMCX_TARGET_GAUSS_ISO>(r1[i], uterm1<TK>(q[k][j], vc[k].mean[j], vc[k].ivar[j]),
+                                                            first && j == 0);
+                r2[i] = sum_in<MK == HMCX_MASS_NONE>(r2[i], kterm1<MK>(p[k][j], vc[k].im[j]), first && j == 0);
             }
+        }
         // next iteration's normals: independent work.  In Philox mode the draw is branch-free and unconditional (one
         // unused draw after the last iteration) so that it shares a basic block with the reduction's shuffle chain.
-        if (CS > 1) cluster_sum3_publish(r0, r1, r2, logu, s_part[n & 1]);      // ... the draw below overlaps the barrier
+        // The cluster and paired forms publish their partials first: the draw then sits between the stores and the
+        // barrier.
+        if constexpr (PAIR) block_sum3_pair_publish(r0, r1, r2, logu, s_red[n & 1]);
+        else if (CS > 1) cluster_sum3_publish(r0[0], r1[0], r2[0], logu, s_part[n & 1]);
         if (PHILOX || n + 1 < a.it1) draw(n + 1);
-        if (CS > 1) cluster_sum3_collect<CS>(r0, r1, r2, logu, s_part[n & 1]);
-        else if (MAXT <= 256) block_sum3_small(r0, r1, r2, logu, s_red[n & 1]);
-        else block_sum3(r0, r1, r2, logu, s_red[n & 1]);
-        const float lp_new = log_prob_from_sum(r1, t.log_norm);
-        const float h_old = add(-lp_cur, mul(0.5f, r0));                     // potential + kinetic (:815)
-        const float h_new = add(-lp_new, mul(0.5f, r2));
+        if (PAIR) block_sum3_pair_collect(r0[0], r1[0], r2[0], logu, s_red[n & 1]);
+        else if (CS > 1) cluster_sum3_collect<CS>(r0[0], r1[0], r2[0], logu, s_part[n & 1]);
+        else if (MAXT <= 256) block_sum3_small(r0[0], r1[0], r2[0], logu, s_red[n & 1]);
+        else block_sum3(r0[0], r1[0], r2[0], logu, s_red[n & 1]);
+        const float lp_new = log_prob_from_sum(r1[0], t.log_norm);
+        const float h_old = add(-lp_cur, mul(0.5f, r0[0]));                  // potential + kinetic (:815)
+        const float h_new = add(-lp_new, mul(0.5f, r2[0]));
         const bool bad = !finite_f(lp_cur) || !finite_f(lp_new);            // LogProbError (:783-785)
         // ---- MH (:1000-1004) ----
         const float x = add(-h_new, h_old);                                  // acceptance(), :626
@@ -459,7 +562,9 @@ hmc_run_kernel(const RunArgs a) {
             if (n == a.burn + 1) {
                 // reference quirk (:1018): the first stored iteration restores ret_params[-1] == params_init,
                 // not the pre-trajectory state.  Rare path: re-read params_init and recompute its log p.
-                float s[1] = {0.0f};
+                float s[KP];
+#pragma unroll
+                for (int i = 0; i < KP; ++i) s[i] = 0.0f;
 #pragma unroll
                 for (int k = 0; k < K; ++k) {
                     const int e0 = E * (gt + k * G);
@@ -467,10 +572,11 @@ hmc_run_kernel(const RunArgs a) {
 #pragma unroll
                     for (int j = 0; j < E; ++j) {
                         if (!live[k] || e0 + j >= D) qc[k][j] = 0.0f;
-                        s[0] = add(s[0], uterm1<TK>(qc[k][j], vc[k].mean[j], vc[k].ivar[j]));
+                        s[PAIR ? k : 0] = add(s[PAIR ? k : 0], uterm1<TK>(qc[k][j], vc[k].mean[j], vc[k].ivar[j]));
                     }
                 }
-                if (CS > 1) s[0] = cluster_sum1<CS>(s[0], s_part[2]);       // every CTA of the cluster takes this branch
+                if constexpr (PAIR) s[0] = block_sum1_groups<KP>(s, s_red[(n & 1) ^ 1]);
+                else if (CS > 1) s[0] = cluster_sum1<CS>(s[0], s_part[2]);  // every CTA of the cluster takes this branch
                 else block_sum<1>(s, s_red[(n & 1) ^ 1]);
                 lp_cur = log_prob_from_sum(s[0], t.log_norm);
                 __syncthreads();          // the next iteration reduces through the same buffer
@@ -880,15 +986,21 @@ int elem_gibbs(const hmcx_mass_t* mass, const hmcx_rng_t* rng, int D, int C, int
 }
 
 // Register-resident geometry (one CTA per chain): each thread owns K groups of E contiguous elements.
-//   tuning 0 (auto): one float4 per thread (E=4,K=1) for D <= 2560, two (K=2) above.  At BASELINE config 2 (D=1024)
-//                    the per-warp fixed cost of an iteration (reduction, loop, RNG for the MH test) makes both thinner
-//                    threads (E=2) and fatter threads (K=2, K=4) slower than float4; at D >= 3072 (config 5: D=4096)
-//                    CTAs of 768-1024 threads are slower than 512 x 2.
+//   tuning 0 (auto): one float4 per thread (E=4,K=1), except
+//                    * 768 < ld <= 1024 in the plain Philox loop (pair_ok): two float4 per thread in CTAs of <= 128
+//                      threads (the paired form, bit-identical to K=1).  The loop is issue-bound there, and every warp
+//                      pays the iteration's fixed cost (reduction, barrier, MH, loop) once: half the warps, ~20 % fewer
+//                      instructions per chain.  Measured at 256 chains (2 CTAs per SM; H100 80GB HBM3, 400 W), launch
+//                      time paired / K=1: 1.05 at ld 512, 1.12 at 768, 0.98 at 832 and 896, 0.94 at 960 and 1024.  Below
+//                      ~7 warps per K=1 CTA the halved warp count leaves the schedulers short of warps and latency wins;
+//                    * D > 2560: K=2 in CTAs of <= 512 threads (at config 5, D=4096, CTAs of 768-1024 threads x 1 are
+//                      slower).
 //   tuning 1: E=4, K=1 forced.
-//   tuning 2 / 4: E=4 with K = 2 / 4 groups per thread;  21: E=2,K=1 (D <= 2048);  22: E=2,K=2.
-static bool pick_geometry(int ld, int tuning, int& E, int& K, int& G) {
+//   tuning 2 / 4: E=4 with K = 2 / 4 groups per thread, each thread's groups summed first (the tree of neither the
+//                 paired form nor K=1);  21: E=2,K=1 (D <= 2048);  22: E=2,K=2.
+static bool pick_geometry(int ld, int tuning, bool pair_ok, int& E, int& K, int& G) {
     if (ld > 4096) return false;
-    if (tuning == 0) { E = 4; K = ld > 2560 ? 2 : 1; }       // D >= 3072: 512 threads x 2 float4 beat 768-1024 x 1
+    if (tuning == 0) { E = 4; K = (ld > 2560 || (pair_ok && ld > 768 && ld <= 1024)) ? 2 : 1; }
     else if (tuning == 1) { E = 4; K = 1; }
     else if (tuning == 21) { E = 2; K = 1; }
     else if (tuning == 2 || tuning == 4) { E = 4; K = tuning; }
@@ -953,7 +1065,7 @@ int elem_hmc_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmc
         if (ld > 4096 || (tuning != 0 && tuning != 1)) return HMCX_ERR_UNSUPPORTED;
         a.thin = sink->thin; a.msum = sink->sum; a.msumsq = sink->sumsq;
         a.msum_lo = sink->sum_lo; a.msumsq_lo = sink->sumsq_lo;
-        pick_geometry(ld, 1, E, K, G);
+        pick_geometry(ld, 1, false, E, K, G);
 #define CALLSINK(TK, MK)                                                                                \
         if (G <= 256) hmc_run_kernel<TK, MK, 4, 1, 256, true><<<C, G, 0, st>>>(a);                      \
         else hmc_run_kernel<TK, MK, 4, 1, 1024, true><<<C, G, 0, st>>>(a)
@@ -968,11 +1080,14 @@ int elem_hmc_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmc
 #undef CALLBIG
         return cuda_status();
     }
-    if (!pick_geometry(ld, tuning, E, K, G)) return tuning ? HMCX_ERR_INVALID_ARG : HMCX_ERR_UNSUPPORTED;
-    a.lp_carry = workspace;                                // [C] floats (hmcx_hmc_workspace_bytes) or NULL
     const bool philox = a.rng_mode == HMCX_RNG_PHILOX;
+    const bool pair_ok = philox && !a.nuts;                // the paired K = 2 form is compiled for this loop only
+    if (!pick_geometry(ld, tuning, pair_ok, E, K, G)) return tuning ? HMCX_ERR_INVALID_ARG : HMCX_ERR_UNSUPPORTED;
+    a.lp_carry = workspace;                                // [C] floats (hmcx_hmc_workspace_bytes) or NULL
+    const bool pair = tuning == 0 && K == 2 && G <= 128 && pair_ok;
 #define CALL(TK, MK)                                                                                    \
-    if (E == 2 && K == 1) hmc_run_kernel<TK, MK, 2, 1, 1024><<<C, G, 0, st>>>(a);                       \
+    if (pair) hmc_run_kernel<TK, MK, 4, 2, 128, false, true, 1, false><<<C, G, 0, st>>>(a);             \
+    else if (E == 2 && K == 1) hmc_run_kernel<TK, MK, 2, 1, 1024><<<C, G, 0, st>>>(a);                  \
     else if (E == 2) hmc_run_kernel<TK, MK, 2, 2, 1024><<<C, G, 0, st>>>(a);                            \
     else if (K == 1 && G <= 256 && philox && !a.nuts)                                                   \
         hmc_run_kernel<TK, MK, 4, 1, 256, false, true, 1, false><<<C, G, 0, st>>>(a);                   \
