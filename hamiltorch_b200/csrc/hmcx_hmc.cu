@@ -342,7 +342,9 @@ constexpr int run_max_threads(int E, int K) { return (E * K <= 4) ? 1024 : (E * 
 // masked): the Philox / Box-Muller arithmetic of iteration n+1 and the shuffle chain of iteration n's reduction then
 // sit in one basic block and the scheduler interleaves them.
 // CS > 1: the chain is owned by a cluster of CS CTAs (see above); CTA `rank` holds float4 groups [rank*G, (rank+1)*G).
-// NUTS = false compiles the dual-averaging path out (the plain sample() loop then carries no trace of it).
+// NUTS = false compiles the dual-averaging path out (the plain sample() loop then carries no trace of it), and with it
+// the step-size schedule and trace, which elem_hmc_run sets only for NUTS: their per-iteration null tests and the
+// reload of eps were ~20 warp-instructions of the paired loop's 1,023.
 // K = 2 with MAXT <= 128 (PAIR): every group keeps its own partial sums and enters the reductions in the place it has
 // in the K = 1 CTA of twice the threads (block_sum3_pair_*, block_sum1_groups), so the run is bit-identical to that
 // geometry; the other K > 1 forms sum their groups per thread first (a different tree).
@@ -475,7 +477,7 @@ hmc_run_kernel(const RunArgs a) {
     const bool warp0 = tid < 32 && rank == 0;
 
     for (int n = a.it0; n < a.it1; ++n) {
-        if (a.eps_schedule) eps = a.eps_schedule[(size_t)n * t.C + c];
+        if (NUTS && a.eps_schedule) eps = a.eps_schedule[(size_t)n * t.C + c];
         const float half = mul(0.5f, eps);
         if (nuts && tid == 0 && n <= a.burn) {
             // dual averaging is a serial scalar recurrence on the critical path (all other threads wait for the new step
@@ -632,7 +634,7 @@ hmc_run_kernel(const RunArgs a) {
             }
             __syncthreads();
             eps = s_eps[n & 1];
-        } else if (a.eps_trace && lead) {
+        } else if (NUTS && a.eps_trace && lead) {
             a.eps_trace[(size_t)c * a.S + n] = eps;
         }
     }
