@@ -15,7 +15,7 @@ LIB_PATH = os.path.join(_HERE, 'lib', 'libhmcx.so')
 OK, ERR_INVALID_ARG, ERR_UNSUPPORTED, ERR_CUDA = 0, -1, -2, -3
 MASS_NONE, MASS_DIAG, MASS_FULL = 0, 1, 2
 RNG_INJECTED, RNG_PHILOX = 0, 1
-ABI_VERSION = 7
+ABI_VERSION = 8
 
 
 class NativeError(RuntimeError):
@@ -114,6 +114,11 @@ _PROTOS = {
                                     C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p,
                                     C.POINTER(SinkStruct), C.c_void_p]),
+    'hmcx_split_run_sink': (C.c_int, [C.POINTER(TargetStruct), C.POINTER(MassStruct), C.POINTER(RngStruct),
+                                      C.POINTER(NutsStruct), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.POINTER(SinkStruct), C.c_void_p]),
     'hmcx_gemm_nt_tf32x3': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     'hmcx_copy_rows_async': (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p]),
     'hmcx_grad_log_prob': (C.c_int, [C.POINTER(TargetStruct), C.c_void_p, C.c_int32, C.c_int32, C.c_int32,

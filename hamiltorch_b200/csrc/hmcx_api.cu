@@ -21,7 +21,7 @@ int dense_rmhmc_run(const hmcx_target_t*, const hmcx_rmhmc_t*, const hmcx_const_
                     float*, int32_t*, float*, cudaStream_t);
 int mlp_split_run(const hmcx_target_t*, const hmcx_mass_t*, const hmcx_rng_t*, const hmcx_nuts_t*, int, const float*,
                   float*, float*, int, int, int, int, int, int, int, float*, uint8_t*, uint8_t*, float*, int32_t*,
-                  cudaStream_t, const float*, float*, float*);
+                  cudaStream_t, const float*, float*, float*, const hmcx_sink_t*);
 int mlp_leapfrog(const hmcx_target_t*, const hmcx_mass_t*, const hmcx_rng_t*, int, double, const float*, const float*, float*,
                  int, int, int, float*, float*, cudaStream_t);
 int mlp_grad_log_prob(const hmcx_target_t*, const float*, int, int, int, float*, float*, cudaStream_t);
@@ -133,7 +133,7 @@ int hmcx_hmc_run_sink(const hmcx_target_t* target, const hmcx_mass_t* mass, cons
     if (target->kind == HMCX_TARGET_MLP)      // un-split Bayesian NN == sample_model (samplers.py:1261)
         return hmcx::mlp_split_run(target, mass, rng, nuts, HMCX_SCHEME_PLAIN, q_init, q_cur, eps, C, ld, L,
                                    num_samples, burn, iter_begin, iter_end, samples_out, accept_out, diverged_out,
-                                   ham_out, num_rejected, (cudaStream_t)stream, nullptr, nullptr, nullptr);
+                                   ham_out, num_rejected, (cudaStream_t)stream, nullptr, nullptr, nullptr, nullptr);
     return HMCX_ERR_UNSUPPORTED;
 }
 
@@ -142,11 +142,23 @@ int hmcx_split_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const h
                    int32_t ld, int32_t L, int32_t num_samples, int32_t burn, int32_t iter_begin, int32_t iter_end,
                    float* samples_out, uint8_t* accept_out, uint8_t* diverged_out, float* ham_out,
                    int32_t* num_rejected, void* stream) {
+    return hmcx_split_run_sink(target, mass, rng, nuts, scheme, q_init, q_cur, eps, C, ld, L, num_samples, burn,
+                               iter_begin, iter_end, samples_out, accept_out, diverged_out, ham_out, num_rejected,
+                               nullptr, stream);
+}
+
+int hmcx_split_run_sink(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmcx_rng_t* rng,
+                        const hmcx_nuts_t* nuts, int32_t scheme, const float* q_init, float* q_cur, float* eps,
+                        int32_t C, int32_t ld, int32_t L, int32_t num_samples, int32_t burn, int32_t iter_begin,
+                        int32_t iter_end, float* samples_out, uint8_t* accept_out, uint8_t* diverged_out,
+                        float* ham_out, int32_t* num_rejected, const hmcx_sink_t* sink, void* stream) {
     if (!target) return HMCX_ERR_INVALID_ARG;
+    if (sink && (sink->thin < 1 || (sink->sum_lo && !sink->sum) || (sink->sumsq_lo && !sink->sumsq)))
+        return HMCX_ERR_INVALID_ARG;
     if (target->kind != HMCX_TARGET_MLP) return HMCX_ERR_UNSUPPORTED;
     return hmcx::mlp_split_run(target, mass, rng, nuts, scheme, q_init, q_cur, eps, C, ld, L, num_samples, burn,
                                iter_begin, iter_end, samples_out, accept_out, diverged_out, ham_out, num_rejected,
-                               (cudaStream_t)stream, nullptr, nullptr, nullptr);
+                               (cudaStream_t)stream, nullptr, nullptr, nullptr, sink);
 }
 
 int hmcx_split_leapfrog(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmcx_rng_t* rng, int32_t scheme,

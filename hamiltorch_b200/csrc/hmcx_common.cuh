@@ -19,6 +19,16 @@ __device__ __forceinline__ float sub(float a, float b) { return __fsub_rn(a, b);
 
 __device__ __forceinline__ bool finite_f(float x) { return fabsf(x) <= 3.402823466e+38f; }
 
+// Neumaier's compensated accumulation: s + c carries the running sum to ~2^-46 relative whatever the number of terms
+// (the sample sink exists for LONG runs: a naive fp32 running sum of x^2 loses the variance once |mean| >> std).  Plain
+// fp32 adds, never contracted or re-associated.
+__device__ __forceinline__ void comp_add(float& s, float& c, float x) {
+    const float t = add(s, x);
+    const float e = (fabsf(s) >= fabsf(x)) ? add(sub(s, t), x) : add(sub(x, t), s);
+    c = add(c, e);
+    s = t;
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // Philox4x32-10 counter RNG (Salmon et al. 2011).  Counter = (element-vector index, iteration lo, iteration hi
 // | stream<<24, chain lo), key = seed ^ (chain hi).  One call yields the 4 normals of one float4 vector.

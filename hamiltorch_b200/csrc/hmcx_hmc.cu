@@ -189,16 +189,6 @@ struct RunArgs {
     float* lp_carry;
 };
 
-// Neumaier's compensated accumulation: s + c carries the running sum to ~2^-46 relative whatever the number of terms
-// (the sink exists for LONG runs: a naive fp32 running sum of x^2 loses the variance once |mean| >> std).  Plain fp32
-// adds, never contracted or re-associated.
-__device__ __forceinline__ void comp_add(float& s, float& c, float x) {
-    const float t = add(s, x);
-    const float e = (fabsf(s) >= fabsf(x)) ? add(sub(s, t), x) : add(sub(x, t), s);
-    c = add(c, e);
-    s = t;
-}
-
 // block_sum3 for CTAs of at most 8 warps: the second level reads the warps' partials with broadcast LDS.128 and adds them
 // in warp order (3 independent 8-term chains) instead of a second shuffle butterfly: ~90 cycles less latency on the
 // per-iteration critical path, same instruction count, every thread ends with the same bits.

@@ -1028,9 +1028,42 @@ struct MlpRunArgs {
     const float* p_given;         // [C, ld] or NULL
     float* q_traj;                // [L, C, ld]: params after every step (ret_params)
     float* p_traj;                // [L, C, ld]: momentum after every step (ret_momenta)
+    // sample sink (hmcx_sink_t), read by the SINK instantiations only: thinning + running moments of the post-burn states
+    int thin;
+    float* msum;
+    float* msumsq;
+    float* msum_lo;               // optional compensation terms (true sum = hi + lo)
+    float* msumsq_lo;
 };
 
-template <int CS>
+// One sink accumulator [C, ld] (sum, or sum of squares when `squares`) += the float4 x at element offset `off`, read and
+// written in place: the chain state fills shared memory, so the running sums stay in the caller's arrays (in L2 at the
+// sizes this kernel runs).  Without a compensation array the term is folded into the sum every time, i.e. the sum is a
+// plain fp32 running sum.
+__device__ __forceinline__ void sink_accumulate(float* hi, float* lo, size_t off, float4 x, bool squares) {
+    float4 s = *reinterpret_cast<const float4*>(hi + off);
+    float4 e = lo ? *reinterpret_cast<const float4*>(lo + off) : make_float4(0.f, 0.f, 0.f, 0.f);
+    float* sp = &s.x;
+    float* ep = &e.x;
+    const float* xp = &x.x;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+        if (squares) {
+            const float xx = mul(xp[j], xp[j]);
+            comp_add(sp[j], ep[j], xx);
+            ep[j] = add(ep[j], fmaf(xp[j], xp[j], -xx));      // the rounding error of x*x itself (exact)
+        } else {
+            comp_add(sp[j], ep[j], xp[j]);
+        }
+    }
+    if (lo) *reinterpret_cast<float4*>(lo + off) = e;
+    else s = make_float4(add(s.x, e.x), add(s.y, e.y), add(s.z, e.z), add(s.w, e.w));
+    *reinterpret_cast<float4*>(hi + off) = s;
+}
+
+// SINK = false: the plain sample() loop (rank 0 stores every post-burn row); SINK = true adds the sample sink, its row
+// work divided over the cluster's ranks (see sink_row below)
+template <int CS, bool SINK>
 __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArgs a) {
     extern __shared__ __align__(128) float sm[];
     __shared__ float sred[64];
@@ -1042,7 +1075,7 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
     const MlpDev& m = a.m;
     ClusterCtx cc = {0, 1};
     if (CS > 1) { cc.rank = (int)cg::this_cluster().block_rank(); cc.size = CS; }
-    const bool lead = cc.rank == 0;                            // rank 0 owns every global-memory output
+    const bool lead = cc.rank == 0;                            // rank 0 owns every global-memory output but the sink rows
     const int c = blockIdx.x / CS, tid = threadIdx.x, D = m.D, M = m.M;
     float* q = sm;
     float* p = q + m.Dp;
@@ -1061,10 +1094,26 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
     double h_bar = 0.0, eps_bar = 1.0;
     if (a.nuts && tid == 0) { h_bar = a.h_bar[c]; eps_bar = a.eps_bar[c]; }
     int rejected = 0;
-    const int keep = a.S - a.burn;
-    float* const my_samples = (a.samples && lead) ? a.samples + (size_t)c * keep * a.ld : nullptr;
-    if (a.it0 == 0 && my_samples)
-        for (int i = tid; i < a.ld; i += MLP_THREADS) my_samples[i] = i < D ? q[i] : 0.0f;
+    const int keep = SINK ? 1 + (a.S - a.burn - 1) / a.thin : a.S - a.burn;      // slots per chain in samples_out
+    float* const my_samples = (a.samples && (SINK || lead)) ? a.samples + (size_t)c * keep * a.ld : nullptr;
+    // Sink: rank r owns the float4 vectors [sv0, sv1) of the row -- their thinned stores (16-byte streaming stores, which is
+    // what lets rows leave over PCIe when samples_out is pinned host memory) and their moment updates.  Every rank holds a
+    // bit-identical replica of q, so this needs no DSMEM traffic and no barrier beyond the loop's own.
+    const int sv_rank = ((a.ld >> 2) + CS - 1) / CS;
+    const int sv0 = cc.rank * sv_rank, sv1 = min(a.ld >> 2, sv0 + sv_rank);
+    auto sink_row = [&](float* dst, bool moments) {
+        const float4* q4 = reinterpret_cast<const float4*>(q);
+        for (int v = sv0 + tid; v < sv1; v += MLP_THREADS) {
+            const float4 x = 4 * v < m.Dp ? q4[v] : make_float4(0.f, 0.f, 0.f, 0.f);   // q's padding lanes are zero
+            if (dst) __stcs(reinterpret_cast<float4*>(dst) + v, x);
+            if (moments && a.msum) sink_accumulate(a.msum, a.msum_lo, row + 4 * v, x, false);
+            if (moments && a.msumsq) sink_accumulate(a.msumsq, a.msumsq_lo, row + 4 * v, x, true);
+        }
+    };
+    if (a.it0 == 0 && my_samples) {
+        if constexpr (SINK) sink_row(my_samples, false);
+        else for (int i = tid; i < a.ld; i += MLP_THREADS) my_samples[i] = i < D ? q[i] : 0.0f;
+    }
 
     auto kinetic = [&]() {                                    // 2*K: p.p or p.(im*p)   (samplers.py:801, :814)
         float s[1] = {0.0f};
@@ -1366,7 +1415,11 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
             }
         }
         if (CS > 1) cg::this_cluster().sync();                 // q_cur is stable before any rank re-reads it
-        if (n > a.burn && my_samples) {
+        if constexpr (SINK) {
+            if (n > a.burn)
+                sink_row((my_samples && (n - a.burn) % a.thin == 0) ? my_samples + (size_t)((n - a.burn) / a.thin) * a.ld
+                                                                    : nullptr, true);
+        } else if (n > a.burn && my_samples) {
             float* dst = my_samples + (size_t)(n - a.burn) * a.ld;
             for (int i = tid; i < a.ld; i += MLP_THREADS) dst[i] = i < D ? q[i] : 0.0f;
         }
@@ -1582,9 +1635,14 @@ static int prepare_smem(Kern kern, size_t bytes) {
 int mlp_split_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmcx_rng_t* rng, const hmcx_nuts_t* nuts,
                   int scheme, const float* q_init, float* q_cur, float* eps, int C, int ld, int L, int S, int burn,
                   int it0, int it1, float* samples, uint8_t* accept, uint8_t* diverged, float* ham,
-                  int32_t* num_rejected, cudaStream_t st, const float* p_given, float* q_traj, float* p_traj) {
+                  int32_t* num_rejected, cudaStream_t st, const float* p_given, float* q_traj, float* p_traj,
+                  const hmcx_sink_t* sink) {
     MlpRunArgs a = {};
     a.p_given = p_given; a.q_traj = q_traj; a.p_traj = p_traj;
+    if (sink) {
+        a.thin = sink->thin; a.msum = sink->sum; a.msumsq = sink->sumsq;
+        a.msum_lo = sink->sum_lo; a.msumsq_lo = sink->sumsq_lo;
+    }
     int rc = fill_mlp(target, a.m);
     if (rc != HMCX_OK) return rc;
     const int mk = mass ? mass->kind : HMCX_MASS_NONE;
@@ -1641,11 +1699,13 @@ int mlp_split_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hm
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = cs; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
-    cudaError_t err;
-    if (cs == 4) { rc = prepare_smem(mlp_run_kernel<4>, smem); if (rc != HMCX_OK) return rc; err = cudaLaunchKernelEx(&cfg, mlp_run_kernel<4>, a); }
-    else if (cs == 2) { rc = prepare_smem(mlp_run_kernel<2>, smem); if (rc != HMCX_OK) return rc; err = cudaLaunchKernelEx(&cfg, mlp_run_kernel<2>, a); }
-    else { rc = prepare_smem(mlp_run_kernel<1>, smem); if (rc != HMCX_OK) return rc; err = cudaLaunchKernelEx(&cfg, mlp_run_kernel<1>, a); }
-    if (err != cudaSuccess) { cudaGetLastError(); return HMCX_ERR_CUDA; }
+    void (*kern)(MlpRunArgs);
+    if (cs == 4) kern = sink ? mlp_run_kernel<4, true> : mlp_run_kernel<4, false>;
+    else if (cs == 2) kern = sink ? mlp_run_kernel<2, true> : mlp_run_kernel<2, false>;
+    else kern = sink ? mlp_run_kernel<1, true> : mlp_run_kernel<1, false>;
+    rc = prepare_smem(kern, smem);
+    if (rc != HMCX_OK) return rc;
+    if (cudaLaunchKernelEx(&cfg, kern, a) != cudaSuccess) { cudaGetLastError(); return HMCX_ERR_CUDA; }
     return cuda_status();
 }
 
@@ -1687,7 +1747,7 @@ int mlp_leapfrog(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmc
     hmcx_nuts_t no_nuts = {};
     no_nuts.step_size_init = step_size;                        // the Python double the drifts divide (:513, :558)
     return mlp_split_run(target, mass, rng, &no_nuts, scheme, q_in, const_cast<float*>(q_in), eps, C, ld, L, 1, 0, 0, 1,
-                         nullptr, nullptr, nullptr, nullptr, nullptr, st, p_in, q_traj, p_traj);
+                         nullptr, nullptr, nullptr, nullptr, nullptr, st, p_in, q_traj, p_traj, nullptr);
 }
 
 // packed X operands of the tensor-core path (hmcx_mlp_t.x_packed): size in floats (0: the stack does not use it) / build

@@ -418,9 +418,9 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
     (N.SCHEME_PLAIN / SPLIT_SYM / SPLIT_RAND / SPLIT_KMID); ``perms`` (S, C, M) injects SPLITTING_RAND's randperm.
     NUTS only: ``eps_schedule`` (S, C) forces the step size of every iteration (parity tests replay the reference's
     schedule); ``record_eps`` returns the kernel's own adapted step sizes in ``result.eps_trace`` (C, S).
-    Sample sink (include/hmcx.h hmcx_sink_t; element-wise targets): ``thin`` keeps every thin-th post-burn state,
-    ``moments`` accumulates per-chain running sum / sum of squares over every post-burn iteration in the kernel's
-    registers with compensated (Neumaier) summation (``result.moment_sum``, ``result.moment_sumsq``: fp64 tensors
+    Sample sink (include/hmcx.h hmcx_sink_t; element-wise targets and Bayesian-NN targets): ``thin`` keeps every
+    thin-th post-burn state, ``moments`` accumulates per-chain running sum / sum of squares over every post-burn
+    iteration with compensated (Neumaier) summation (``result.moment_sum``, ``result.moment_sumsq``: fp64 tensors
     relative error ~ n*eps^2 instead of the naive n*eps; ``result.moment_count``), ``keep_samples=False`` stores no
     samples at all, ``host_samples=True`` makes the kernel stream the retained rows straight into pinned host memory
     (the reference's ``store_on_GPU=False``, samplers.py:1008-1012) -- ``result.samples`` is then a CPU tensor, valid
@@ -457,8 +457,6 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
         else:
             host_samples = True                    # caller-provided pinned sample block: the kernel streams into it
     use_sink = thin > 1 or moments or not keep_samples or host_samples
-    if use_sink and scheme is not None:
-        raise NotImplementedError('the sample sink is implemented for element-wise targets')
     keep = 1 + (S - burn - 1) // thin
     if not keep_samples:
         samples = None
@@ -522,18 +520,19 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
             nuts_s.eps_trace = eps_trace.data_ptr()
 
     msum = msq = msum_lo = msq_lo = None
+    sink = None
+    if use_sink:
+        sink = N.SinkStruct()
+        sink.thin = thin
+        if moments:
+            msum, msq, msum_lo, msq_lo = (torch.zeros((Cn, ld), dtype=torch.float32, device=device) for _ in range(4))
+            sink.sum, sink.sumsq = msum.data_ptr(), msq.data_ptr()
+            sink.sum_lo, sink.sumsq_lo = msum_lo.data_ptr(), msq_lo.data_ptr()
     with torch.cuda.device(device):
         if scheme is None:
             ws_bytes = lib.hmcx_hmc_workspace_bytes(nt.ref(), nm.ref(), Cn, ld)
             ws = torch.empty(ws_bytes // 4, dtype=torch.float32, device=device) if ws_bytes else None
             if use_sink:
-                sink = N.SinkStruct()
-                sink.thin = thin
-                if moments:
-                    msum, msq, msum_lo, msq_lo = (torch.zeros((Cn, ld), dtype=torch.float32, device=device)
-                                                  for _ in range(4))
-                    sink.sum, sink.sumsq = msum.data_ptr(), msq.data_ptr()
-                    sink.sum_lo, sink.sumsq_lo = msum_lo.data_ptr(), msq_lo.data_ptr()
                 rc = lib.hmcx_hmc_run_sink(nt.ref(), nm.ref(), C.byref(rng), C.byref(nuts_s), N.ptr(q_init),
                                            N.ptr(q_cur), N.ptr(eps), Cn, ld, L, S, burn, 0, S, N.ptr(samples),
                                            N.ptr(accepted), N.ptr(diverged), N.ptr(ham), N.ptr(num_rejected),
@@ -575,11 +574,11 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
                                       N.stream_ptr(device))
                 N.check(rc, 'hmcx_hmc_run')
         else:
-            rc = lib.hmcx_split_run(nt.ref(), nm.ref(), C.byref(rng), C.byref(nuts_s), int(scheme), N.ptr(q_init),
-                                    N.ptr(q_cur), N.ptr(eps), Cn, ld, L, S, burn, 0, S, N.ptr(samples),
-                                    N.ptr(accepted), N.ptr(diverged), N.ptr(ham), N.ptr(num_rejected),
-                                    N.stream_ptr(device))
-            N.check(rc, 'hmcx_split_run')
+            rc = lib.hmcx_split_run_sink(nt.ref(), nm.ref(), C.byref(rng), C.byref(nuts_s), int(scheme), N.ptr(q_init),
+                                         N.ptr(q_cur), N.ptr(eps), Cn, ld, L, S, burn, 0, S, N.ptr(samples),
+                                         N.ptr(accepted), N.ptr(diverged), N.ptr(ham), N.ptr(num_rejected),
+                                         None if sink is None else C.byref(sink), N.stream_ptr(device))
+            N.check(rc, 'hmcx_split_run_sink')
     res = HMCResult(samples, accepted, diverged, ham, eps, num_rejected, D, S)
     res.eps_trace = eps_trace
     res.thin = thin

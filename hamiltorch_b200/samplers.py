@@ -223,6 +223,19 @@ def hamiltonian(params, momentum, log_prob_func, jitter=0.01, normalizing_const=
 # ----------------------------------------------------------------------------------------------------------
 # sample()
 # ----------------------------------------------------------------------------------------------------------
+def _sink_supported(log_prob_func, sampler, integrator, inv_mass):
+    """The kernels with a sample sink (thin / moments / keep_samples / store_on_GPU=False): plain HMC / HMC_NUTS on an
+    element-wise target (GaussianIso, GaussianDiag) and the Bayesian-NN kernel (an MLPRegression, or a list of them with a
+    SPLITTING integrator), with inv_mass None or 1-D."""
+    if sampler not in (Sampler.HMC, Sampler.HMC_NUTS) or isinstance(inv_mass, list) or \
+            (torch.is_tensor(inv_mass) and inv_mass.dim() == 2):
+        return False
+    if isinstance(log_prob_func, list):
+        return integrator in _SPLIT_INTEGRATORS and all(isinstance(f, T.MLPRegression) for f in log_prob_func)
+    return integrator not in _SPLIT_INTEGRATORS and isinstance(log_prob_func, (T.GaussianIso, T.GaussianDiag,
+                                                                               T.MLPRegression))
+
+
 def _check_sample_args(params_init_dim_ok, num_samples, burn, sampler):
     if not params_init_dim_ok:
         raise RuntimeError('params_init must be a 1d tensor.')                  # :925-926
@@ -279,10 +292,7 @@ def sample(log_prob_func, params_init, num_samples=10, num_steps_per_sample=10, 
                       fixed_point_max_iterations, jitter_max_tries, sampler, integrator, metric,
                       desired_accept_rate, rng=rng, seed=seed, record_ham=(debug == 1),
                       sink=dict(host_samples=True) if (
-                          not store_on_GPU and sampler in (Sampler.HMC, Sampler.HMC_NUTS) and
-                          isinstance(log_prob_func, (T.GaussianIso, T.GaussianDiag)) and
-                          integrator not in _SPLIT_INTEGRATORS and
-                          not (torch.is_tensor(inv_mass) and inv_mass.dim() == 2)) else None)
+                          not store_on_GPU and _sink_supported(log_prob_func, sampler, integrator, inv_mass)) else None)
     if not res.samples_padded.is_cuda:
         torch.cuda.current_stream().synchronize()       # the kernel wrote the samples into pinned host memory
     nuts = sampler == Sampler.HMC_NUTS
@@ -326,7 +336,8 @@ def sample_chains(log_prob_func, params_init, num_samples=10, num_steps_per_samp
     ``log_prob_func`` may be a Gaussian / funnel descriptor, an ``MLPRegression`` (sample_model) or the list of split
     descriptors ``define_split_model_log_prob`` returns (with a SPLITTING integrator).
 
-    Sample sink (plain HMC / HMC_NUTS on GaussianIso / GaussianDiag): ``thin`` keeps every thin-th post-burn state;
+    Sample sink (plain HMC / HMC_NUTS on GaussianIso / GaussianDiag, and the Bayesian-NN targets with any of their
+    integrators; inv_mass None or 1-D): ``thin`` keeps every thin-th post-burn state;
     ``moments=True`` returns per-chain running sums / sums of squares over all post-burn iterations
     (``.moment_sum``, ``.moment_sumsq``, ``.moment_count``); ``keep_samples=False`` stores no samples;
     ``store_on_GPU=False`` (the reference's flag, samplers.py:1008-1012) streams the retained samples from the kernel
@@ -357,13 +368,9 @@ def _run_chains(log_prob_func, q0, num_samples, L, step_size, burn, jitter, inv_
     nuts = sampler == Sampler.HMC_NUTS
     sink = sink or {}
     if (sink.get('thin', 1) != 1 or sink.get('moments') or not sink.get('keep_samples', True) or
-            sink.get('host_samples')) and not (sampler in (Sampler.HMC, Sampler.HMC_NUTS) and
-                                               isinstance(log_prob_func, (T.GaussianIso, T.GaussianDiag)) and
-                                               integrator not in _SPLIT_INTEGRATORS and
-                                               not (torch.is_tensor(inv_mass) and inv_mass.dim() == 2) and
-                                               not isinstance(inv_mass, list)):
+            sink.get('host_samples')) and not _sink_supported(log_prob_func, sampler, integrator, inv_mass):
         raise NotImplementedError('thin / moments / keep_samples / store_on_GPU=False: plain HMC on element-wise targets '
-                                  'with inv_mass None or 1-D')
+                                  'and the Bayesian-NN targets, with inv_mass None or 1-D')
     if nuts:
         sampler = Sampler.HMC                                                     # :932-936
     if sampler == Sampler.HMC and integrator not in _SPLIT_INTEGRATORS:
@@ -428,7 +435,7 @@ def _run_chains(log_prob_func, q0, num_samples, L, step_size, burn, jitter, inv_
         return engine.hmc_run(log_prob_func, q0, num_samples, L, step_size, burn=burn, inv_mass=inv_mass, nuts=nuts,
                               desired_accept_rate=desired_accept_rate, seed=seed or 0, chain_offset=chain_offset,
                               normals=normals, log_uniforms=log_uniforms, record_ham=record_ham, out=out,
-                              scheme=scheme, perms=perms)
+                              scheme=scheme, perms=perms, **sink)
     if sampler == Sampler.RMHMC and integrator in (Integrator.EXPLICIT, Integrator.IMPLICIT):
         if isinstance(log_prob_func, list) or not isinstance(log_prob_func, (T.Funnel, T.GaussianIso, T.GaussianDiag,
                                                                              T.GaussianFull)):

@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define HMCX_ABI_VERSION 7
+#define HMCX_ABI_VERSION 8
 
 #define HMCX_MLP_TC_AUTO 0
 #define HMCX_MLP_TC_OFF  1
@@ -377,8 +377,9 @@ int hmcx_rmhmc_dense_run(const hmcx_target_t* target, const hmcx_rmhmc_t* cfg, c
  *          params_init, slot j = the chain state after iteration burn + j*thin  (thin = 1: the reference's list)
  *   sum, sumsq   optional [C, ld] in/out accumulators: running sum / sum of squares of the chain state over EVERY
  *          iteration n > burn (= elements 1.. of the reference's returned list), so posterior means and variances
- *          need no sample storage at all (samples_out may then be NULL).  Accumulated in registers with Neumaier
- *          compensation (the rounding of x*x included): relative error ~ n*eps^2 after n iterations (eps = 2^-24)
+ *          need no sample storage at all (samples_out may then be NULL).  Accumulated with Neumaier compensation (the
+ *          rounding of x*x included; element-wise kernel: in registers, Bayesian-NN kernel: in place in these arrays at
+ *          every iteration, see hmcx_split_run_sink): relative error ~ n*eps^2 after n iterations (eps = 2^-24)
  *          instead of the ~ n*eps of a plain fp32 running sum:
  *   sum_lo, sumsq_lo   optional [C, ld] in/out: the compensation terms; the sums are hi + lo (combine in fp64: var =
  *          E[x^2] - mean^2 then holds for |mean| >> std; measured 1.6e-7 on a variance of 1 at mean 100, n = 2e4, where
@@ -404,6 +405,20 @@ int hmcx_hmc_run_sink(const hmcx_target_t* target, const hmcx_mass_t* mass, cons
                       int32_t iter_begin, int32_t iter_end,
                       float* samples_out, uint8_t* accept_out, uint8_t* diverged_out, float* ham_out,
                       int32_t* num_rejected, int32_t tuning, float* workspace, const hmcx_sink_t* sink, void* stream);
+
+/* hmcx_split_run with a sample sink (sink == NULL: identical to hmcx_split_run).  Any non-NULL sink selects the sink form of
+ * the Bayesian-NN kernel: the CTAs of a chain's cluster divide each retained row and its moment updates between them, and
+ * the rows go out as 16-byte streaming stores (what pinned host samples_out wants); samples, flags and step sizes are those
+ * of hmcx_split_run.  sum / sumsq are read and updated in place at every post-burn iteration, so without sum_lo / sumsq_lo
+ * they are plain fp32 running sums: pass both for the compensated sums.  Windows of iterations chain through the
+ * accumulators.  thin < 1, sum_lo without sum or sumsq_lo without sumsq: HMCX_ERR_INVALID_ARG. */
+int hmcx_split_run_sink(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmcx_rng_t* rng,
+                        const hmcx_nuts_t* nuts, int32_t scheme,
+                        const float* q_init, float* q_cur, float* eps,
+                        int32_t C, int32_t ld, int32_t L, int32_t num_samples, int32_t burn,
+                        int32_t iter_begin, int32_t iter_end,
+                        float* samples_out, uint8_t* accept_out, uint8_t* diverged_out, float* ham_out,
+                        int32_t* num_rejected, const hmcx_sink_t* sink, void* stream);
 
 /*
  * hmcx_copy_rows_async: `height` rows of `width` bytes from `src` (row pitch `spitch`) to `dst` (row pitch `dpitch`), either
