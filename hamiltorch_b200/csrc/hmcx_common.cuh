@@ -178,6 +178,19 @@ __device__ __forceinline__ float philox_log_uniform(uint64_t seed, uint64_t chai
     return logf(u01(r.x));
 }
 
+// Jitter stream: the torch.rand(D) that fisher() call `call` of an iteration draws (samplers.py:115).  Each call owns
+// JITTER_VECS_PER_CALL counter vectors, one Philox call per 4 elements, so a row of up to 64 elements never reaches the
+// next call's counters (hmcx_rmhmc_cta.cu ties this to its largest D).  Element 4*vec+j <- (word j >> 8) * 2^-24 in [0, 1).
+constexpr int JITTER_VECS_PER_CALL = 16;
+__device__ __forceinline__ void philox_jitter4(uint64_t seed, uint64_t chain, uint64_t iter, int call, int vec,
+                                               float u[4]) {
+    const uint4 r = philox_draw(seed, chain, iter, (uint32_t)(call * JITTER_VECS_PER_CALL + vec), STREAM_JITTER);
+    u[0] = (float)(r.x >> 8) * 5.9604645e-8f;
+    u[1] = (float)(r.y >> 8) * 5.9604645e-8f;
+    u[2] = (float)(r.z >> 8) * 5.9604645e-8f;
+    u[3] = (float)(r.w >> 8) * 5.9604645e-8f;
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // reductions.  xor-butterflies: every lane ends with the same bits (fp add is commutative and each level pairs
 // identical operands), so all threads of a CTA take identical decisions without a broadcast.

@@ -395,9 +395,9 @@ struct JitterSrc {                // the jitter uniforms of fisher() (:115), one
             for (int i = 0; i < d; ++i) buf[i] = src[i];
         } else {
             for (int v = 0; 4 * v < d; ++v) {
-                const uint4 r = philox_draw(a.seed, chain_id, (uint64_t)n, (uint32_t)(idx * 8 + v), STREAM_JITTER);
-                const uint32_t rr[4] = {r.x, r.y, r.z, r.w};
-                for (int j = 0; j < 4 && 4 * v + j < d; ++j) buf[4 * v + j] = (float)(rr[j] >> 8) * 5.9604645e-8f;  // [0,1)
+                float u[4];
+                philox_jitter4(a.seed, chain_id, (uint64_t)n, idx, v, u);
+                for (int j = 0; j < 4 && 4 * v + j < d; ++j) buf[4 * v + j] = u[j];
             }
         }
         ++idx;
@@ -605,9 +605,10 @@ __device__ __forceinline__ const float* rm2_jitter_row(const RmRunArgs& a, int c
         const float* src = a.uniforms + (((size_t)(n - a.it0) * a.C + c) * a.J + j) * a.ld;
         buf[0] = src[0]; buf[1] = src[1];
     } else {
-        const uint4 r = philox_draw(a.seed, chain_id, (uint64_t)n, (uint32_t)(idx * 8), STREAM_JITTER);
-        buf[0] = (float)(r.x >> 8) * 5.9604645e-8f;
-        buf[1] = (float)(r.y >> 8) * 5.9604645e-8f;
+        float u[4];
+        philox_jitter4(a.seed, chain_id, (uint64_t)n, idx, 0, u);
+        buf[0] = u[0];
+        buf[1] = u[1];
     }
     return buf;
 }

@@ -26,6 +26,7 @@ namespace hmcx {
 
 constexpr int RC_T = 256;                 // threads per chain
 constexpr int RC_DMAX = 64;
+static_assert(4 * JITTER_VECS_PER_CALL >= RC_DMAX, "a fisher() call's jitter row would overlap the next call's counters");
 
 struct RcArgs {
     RmTarget t;
@@ -472,9 +473,9 @@ __global__ void __launch_bounds__(RC_T) rmhmc_cta_kernel(const RcArgs a) {
                 for (int i = tid; i < d; i += RC_T) c.ub[i] = src[i];
             } else {
                 for (int v = tid; 4 * v < d; v += RC_T) {
-                    const uint4 r = philox_draw(a.seed, chain_id, (uint64_t)n, (uint32_t)(k * 8 + v), STREAM_JITTER);
-                    const uint32_t rr[4] = {r.x, r.y, r.z, r.w};
-                    for (int j = 0; j < 4 && 4 * v + j < d; ++j) c.ub[4 * v + j] = (float)(rr[j] >> 8) * 5.9604645e-8f;
+                    float u[4];
+                    philox_jitter4(a.seed, chain_id, (uint64_t)n, k, v, u);
+                    for (int j = 0; j < 4 && 4 * v + j < d; ++j) c.ub[4 * v + j] = u[j];
                 }
             }
             __syncthreads();
