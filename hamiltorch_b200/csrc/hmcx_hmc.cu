@@ -123,9 +123,12 @@ __device__ __forceinline__ void trajectory(float* q, float* p, const VecConst<E>
 // The same trajectory for NG groups of one thread in one step loop: every trip advances all NG*E elements, so a thread
 // with two groups runs 8 independent element chains per step instead of two loops of 4.  Element-wise, so the bits are
 // those of trajectory<> on each group.
-template <int TK, int MK, int E, int NG>
+// `side()` is independent work (the next iteration's normals) placed after the first half-kick and the first step,
+// which are peeled out of the step loop (L >= 1) so that the three share one basic block: the side work's dependent
+// chains then interleave with 8 independent element chains instead of standing alone in the iteration's serial tail.
+template <int TK, int MK, int E, int NG, typename F>
 __device__ __forceinline__ void trajectory_groups(float (*q)[E], float (*p)[E], const VecConst<E>* c, float eps,
-                                                  float half, int L) {
+                                                  float half, int L, F&& side) {
 #pragma unroll
     for (int g = 0; g < NG; ++g)
 #pragma unroll
@@ -139,7 +142,9 @@ __device__ __forceinline__ void trajectory_groups(float (*q)[E], float (*p)[E], 
                 p[g][j] = add(p[g][j], mul(eps, grad1<TK>(q[g][j], c[g].mean[j], c[g].ivar[j])));
             }
     };
-    int l = 0;
+    one_step();
+    side();
+    int l = 1;
 #pragma unroll 1
     for (; l + 2 <= L; l += 2) { one_step(); one_step(); }
     if (l < L) one_step();
@@ -229,7 +234,7 @@ __device__ __forceinline__ void block_sum3_small(float& a, float& b, float& c, f
 // as many threads with one group each, so the sums have that CTA's block_sum3_small tree and bits.
 // publish: one packed butterfly over both groups' 6 values with warp_sum3's xor pairing (16, 8, 4, 2, 1) for each,
 // 8 shuffles instead of 2 x 6; lanes 0/4/8 end with group 0's a/b/c, lanes 16/20/24 with group 1's.  Then the 6 slots
-// and the extra scalar are stored.  The caller puts independent work between publish and collect.
+// and the extra scalar are stored.
 __device__ __forceinline__ void block_sum3_pair_publish(const float (&a)[2], const float (&b)[2], const float (&c)[2],
                                                         float extra, float* sbuf) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = (blockDim.x + 31) >> 5;
@@ -324,6 +329,23 @@ __device__ __forceinline__ float cluster_sum1(float v, float4* slot) {
 
 constexpr int run_max_threads(int E, int K) { return (E * K <= 4) ? 1024 : (E * K <= 8 ? 512 : 256); }
 
+// Developer build only (-DHMCX_HMC_PROF, scripts/prof_hmc_phases.py): clock64() stamps of the paired loop, lane 0 of every
+// warp of the first HMC_PROF_CTAS CTAs, iterations [HMC_PROF_IT0, HMC_PROF_IT0 + HMC_PROF_ITS) of the launch, 8 stamp ids
+// per iteration, and each CTA's SM id so that the co-resident chains can be matched.
+#ifdef HMCX_HMC_PROF
+constexpr int HMC_PROF_CTAS = 256, HMC_PROF_WARPS = 4, HMC_PROF_IT0 = 256, HMC_PROF_ITS = 64, HMC_PROF_IDS = 8;
+__device__ long long g_hmc_prof[HMC_PROF_CTAS * HMC_PROF_WARPS * HMC_PROF_ITS * HMC_PROF_IDS];
+__device__ int g_hmc_prof_sm[HMC_PROF_CTAS];
+__device__ __forceinline__ long long* hmc_prof_row(int n, int it0) {
+    const int i = n - it0 - HMC_PROF_IT0, w = threadIdx.x >> 5;
+    if ((threadIdx.x & 31) || blockIdx.x >= HMC_PROF_CTAS || w >= HMC_PROF_WARPS || i < 0 || i >= HMC_PROF_ITS) return nullptr;
+    return g_hmc_prof + ((size_t)(blockIdx.x * HMC_PROF_WARPS + w) * HMC_PROF_ITS + i) * HMC_PROF_IDS;
+}
+#define HMC_MARK(row, id) do { if (row) (row)[id] = clock64(); } while (0)
+#else
+#define HMC_MARK(row, id) do {} while (0)
+#endif
+
 // MAXT = CTA size the instantiation is compiled for (register budget 64K/MAXT): chains of D <= 1024 run with <= 256
 // threads and get a generous budget, which lets the compiler software-pipeline the next iteration's RNG.
 // SINK = true adds the sample sink to the bookkeeping step (thinned stores, register-resident moment accumulators); it is
@@ -375,6 +397,13 @@ hmc_run_kernel(const RunArgs a) {
         }
     }
     if (CS == 1 && MAXT <= 256) block_sum3_small_init(s_red, KP);
+#ifdef HMCX_HMC_PROF
+    if (PAIR && tid == 0 && blockIdx.x < HMC_PROF_CTAS) {
+        int sm;
+        asm volatile("mov.u32 %0, %%smid;" : "=r"(sm));
+        g_hmc_prof_sm[blockIdx.x] = sm;
+    }
+#endif
 
     // U(q_cur) once; afterwards it is carried (the reference recomputes the identical value, :971)
     float lp_cur;
@@ -430,7 +459,8 @@ hmc_run_kernel(const RunArgs a) {
     }
 
     // the standard normals of iteration n: produced one iteration AHEAD (they do not depend on the MH decision), so
-    // that the Philox/Box-Muller arithmetic of iteration n+1 overlaps the shuffle/barrier latency of iteration n
+    // that the Philox/Box-Muller arithmetic of iteration n+1 overlaps the shuffle/barrier latency of iteration n, or, in
+    // the paired form, the first leapfrog step of iteration n
     float zn[K][E];
     PhiloxKeys keys;
     PhiloxFixed pfix[K];
@@ -467,6 +497,10 @@ hmc_run_kernel(const RunArgs a) {
     const bool warp0 = tid < 32 && rank == 0;
 
     for (int n = a.it0; n < a.it1; ++n) {
+#ifdef HMCX_HMC_PROF
+        long long* const prow = PAIR ? hmc_prof_row(n, a.it0) : nullptr;
+#endif
+        HMC_MARK(prow, 0);                  // the iteration starts
         if (NUTS && a.eps_schedule) eps = a.eps_schedule[(size_t)n * t.C + c];
         const float half = mul(0.5f, eps);
         if (nuts && tid == 0 && n <= a.burn) {
@@ -506,7 +540,8 @@ hmc_run_kernel(const RunArgs a) {
         }
         // ---- leapfrog (:973) : thread-private ----
         if (PAIR) {
-            trajectory_groups<TK, MK, E, K>(q, p, vc, eps, half, a.L);
+            // the normals of iteration n+1 (zn is consumed above; branch-free, one unused draw after the last iteration)
+            trajectory_groups<TK, MK, E, K>(q, p, vc, eps, half, a.L, [&]() { draw(n + 1); });
         } else {
 #pragma unroll
             for (int k = 0; k < K; ++k)
@@ -526,12 +561,18 @@ hmc_run_kernel(const RunArgs a) {
         }
         // next iteration's normals: independent work.  In Philox mode the draw is branch-free and unconditional (one
         // unused draw after the last iteration) so that it shares a basic block with the reduction's shuffle chain.
-        // The cluster and paired forms publish their partials first: the draw then sits between the stores and the
-        // barrier.
+        // The cluster form publishes its partials first: the draw then sits between the stores and the barrier.
+        HMC_MARK(prow, 1);                  // trajectory and per-thread sums done
         if constexpr (PAIR) block_sum3_pair_publish(r0, r1, r2, logu, s_red[n & 1]);
         else if (CS > 1) cluster_sum3_publish(r0[0], r1[0], r2[0], logu, s_part[n & 1]);
-        if (PHILOX || n + 1 < a.it1) draw(n + 1);
-        if (PAIR) block_sum3_pair_collect(r0[0], r1[0], r2[0], logu, s_red[n & 1]);
+        HMC_MARK(prow, 2);                  // slots stored
+        if (!PAIR && (PHILOX || n + 1 < a.it1)) draw(n + 1);     // the paired form draws inside the trajectory
+        HMC_MARK(prow, 3);                  // next normals drawn
+        if (PAIR) {
+            __syncthreads();                // block_sum3_pair_collect, with a stamp after its barrier
+            HMC_MARK(prow, 4);
+            block_sum3_slots(r0[0], r1[0], r2[0], logu, s_red[n & 1]);
+        }
         else if (CS > 1) cluster_sum3_collect<CS>(r0[0], r1[0], r2[0], logu, s_part[n & 1]);
         else if (MAXT <= 256) block_sum3_small(r0[0], r1[0], r2[0], logu, s_red[n & 1]);
         else block_sum3(r0[0], r1[0], r2[0], logu, s_red[n & 1]);
@@ -599,6 +640,7 @@ hmc_run_kernel(const RunArgs a) {
                 if (live[k]) stE_stream<E>(row_ptr + E * k * G, qc[k]);
             row_ptr += ld;
         }
+        HMC_MARK(prow, 5);                  // MH decided, state selected, row stored
         if (lead) {
             const size_t o = (size_t)c * a.S + n;
             if (a.accept) a.accept[o] = acc ? 1 : 0;
@@ -1094,5 +1136,20 @@ int elem_hmc_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmc
 #undef CALL
     return cuda_status();
 }
+
+#ifdef HMCX_HMC_PROF
+// developer build only (scripts/prof_hmc_phases.py): copies out and clears the stamps; returns the number of stamps
+extern "C" int hmcx_debug_hmc_prof(long long* stamps, int* sm) {
+    const int n = HMC_PROF_CTAS * HMC_PROF_WARPS * HMC_PROF_ITS * HMC_PROF_IDS;
+    cudaDeviceSynchronize();
+    cudaMemcpyFromSymbol(stamps, g_hmc_prof, sizeof(long long) * n);
+    cudaMemcpyFromSymbol(sm, g_hmc_prof_sm, sizeof(int) * HMC_PROF_CTAS);
+    void* p = nullptr;
+    cudaGetSymbolAddress(&p, g_hmc_prof);
+    cudaMemset(p, 0, sizeof(long long) * n);
+    cudaDeviceSynchronize();
+    return n;
+}
+#endif
 
 }  // namespace hmcx
