@@ -257,19 +257,48 @@ __device__ __forceinline__ void block_sum3_pair_collect(float& a, float& b, floa
     __syncthreads();
     block_sum3_slots(a, b, c, extra, sbuf);
 }
+// The producer form's publish: the kinetic sums of the momentum come from the producer warps (hmc_produce), so only
+// (b[k], c[k]) are reduced here, with the same xor pairing and into the same slot positions (.y, .z) as
+// block_sum3_pair_publish.  Lanes 0/8 end with group 0's b/c, lanes 16/24 with group 1's; 6 shuffles.
+__device__ __forceinline__ void block_sum2_pair_publish(const float (&b)[2], const float (&c)[2], float* sbuf, int nwarp) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const bool h16 = lane & 16, h8 = lane & 8;
+    const float x1 = add(h16 ? b[1] : b[0], __shfl_xor_sync(0xffffffffu, h16 ? b[0] : b[1], 16));
+    const float x2 = add(h16 ? c[1] : c[0], __shfl_xor_sync(0xffffffffu, h16 ? c[0] : c[1], 16));
+    // xor 8: lanes with bit 8 clear finish b, set finish c
+    float k = add(h8 ? x2 : x1, __shfl_xor_sync(0xffffffffu, h8 ? x1 : x2, 8));
+    k = add(k, __shfl_xor_sync(0xffffffffu, k, 4));
+    k = add(k, __shfl_xor_sync(0xffffffffu, k, 2));
+    k = add(k, __shfl_xor_sync(0xffffffffu, k, 1));
+    if ((lane & 7) == 0) sbuf[4 * (warp + (lane >> 4) * nwarp) + 1 + ((lane >> 3) & 1)] = k;
+}
+
+// Named barriers of the producer form (PW > 0): 0 is __syncthreads, 1 the compute threads' own barrier.  The momentum
+// slot has a "full" barrier (producers arrive once the slot holds iteration n, compute threads wait) and an "empty" one
+// (compute threads arrive when iteration n's trajectory is done, by which time they hold the slot's contents in
+// registers; producers wait before they draw iteration n+1 into it).
+constexpr int BAR_CHAIN = 1, BAR_SLOT_FULL = 2, BAR_SLOT_EMPTY = 3;
+__device__ __forceinline__ void bar_sync(int id, int n) { asm volatile("bar.sync %0, %1;" :: "r"(id), "r"(n) : "memory"); }
+__device__ __forceinline__ void bar_arrive(int id, int n) { asm volatile("bar.arrive %0, %1;" :: "r"(id), "r"(n) : "memory"); }
+// the barrier of the threads that hold the chain's state: the whole CTA, or the G compute threads of the producer form
+template <int PW>
+__device__ __forceinline__ void chain_sync(int G) {
+    if constexpr (PW == 0) __syncthreads();
+    else bar_sync(BAR_CHAIN, G);
+}
 
 // block_sum<1> with the same correspondence for a thread holding K partials: partial k is lane t&31 of warp
-// (t>>5) + k*nwarp.  `sbuf` holds 32 floats.
-template <int K>
+// (t>>5) + k*nwarp.  `sbuf` holds 32 floats.  PW = the CTA's producer warps, which do not take part.
+template <int K, int PW = 0>
 __device__ __forceinline__ float block_sum1_groups(float (&v)[K], float* sbuf) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = (blockDim.x + 31) >> 5;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarp = ((blockDim.x + 31) >> 5) - PW;
 #pragma unroll
     for (int k = 0; k < K; ++k) v[k] = warp_sum(v[k]);
     if (lane == 0) {
 #pragma unroll
         for (int k = 0; k < K; ++k) sbuf[warp + k * nwarp] = v[k];
     }
-    __syncthreads();
+    chain_sync<PW>(nwarp * 32);
     return warp_sum(lane < K * nwarp ? sbuf[lane] : 0.0f);
 }
 
@@ -331,11 +360,18 @@ constexpr int run_max_threads(int E, int K) { return (E * K <= 4) ? 1024 : (E * 
 
 // Developer build only (-DHMCX_HMC_PROF, scripts/prof_hmc_phases.py): clock64() stamps of the paired loop, lane 0 of every
 // warp of the first HMC_PROF_CTAS CTAs, iterations [HMC_PROF_IT0, HMC_PROF_IT0 + HMC_PROF_ITS) of the launch, 8 stamp ids
-// per iteration, and each CTA's SM id so that the co-resident chains can be matched.
+// per iteration, and each CTA's SM id so that the co-resident chains can be matched.  The producer form also stamps, per
+// iteration, when producer warp 0 published the iteration's momentum slot.
 #ifdef HMCX_HMC_PROF
 constexpr int HMC_PROF_CTAS = 256, HMC_PROF_WARPS = 4, HMC_PROF_IT0 = 256, HMC_PROF_ITS = 64, HMC_PROF_IDS = 8;
 __device__ long long g_hmc_prof[HMC_PROF_CTAS * HMC_PROF_WARPS * HMC_PROF_ITS * HMC_PROF_IDS];
+__device__ long long g_hmc_prof_pub[HMC_PROF_CTAS * HMC_PROF_ITS];
 __device__ int g_hmc_prof_sm[HMC_PROF_CTAS];
+__device__ __forceinline__ void hmc_prof_publish(int n, int it0, int pt) {
+    const int i = n - it0 - HMC_PROF_IT0;
+    if (pt == 0 && blockIdx.x < HMC_PROF_CTAS && i >= 0 && i < HMC_PROF_ITS)
+        g_hmc_prof_pub[blockIdx.x * HMC_PROF_ITS + i] = clock64();
+}
 __device__ __forceinline__ long long* hmc_prof_row(int n, int it0) {
     const int i = n - it0 - HMC_PROF_IT0, w = threadIdx.x >> 5;
     if ((threadIdx.x & 31) || blockIdx.x >= HMC_PROF_CTAS || w >= HMC_PROF_WARPS || i < 0 || i >= HMC_PROF_ITS) return nullptr;
@@ -345,6 +381,91 @@ __device__ __forceinline__ long long* hmc_prof_row(int n, int it0) {
 #else
 #define HMC_MARK(row, id) do {} while (0)
 #endif
+
+// The producer form of the paired loop (PW > 0): PW producer warps behind the G compute threads draw each iteration's
+// momentum, its kinetic sums and the MH log-uniform into one shared-memory slot.  None of that work depends on the
+// chain's state, so it leaves the compute warps' instruction stream.  The producers draw iteration n once iteration
+// n-1's trajectory is done, i.e. while the compute warps sit in the serial tail (butterfly, barrier, MH, row store),
+// where a scheduler has idle issue slots; drawing further ahead competes with the trajectory for them and measured
+// slower (DESIGN §3.1), and since the compute threads have read the slot before their trajectory, one slot suffices.
+// Producer thread pt mirrors compute threads pt + u*32*PW: the same groups, Philox counters and normals, and for each
+// virtual warp of block_sum3_pair_publish the same 32 lanes, so the kinetic sums (a plain xor butterfly, the pairing
+// warp_sum3 gives every value) have that tree's bits.
+struct MomentumSlot {
+    float4 p[2][128];     // the momentum of group k of compute thread t
+    float kin[8];         // the kinetic sum of virtual warp w (slot .x of block_sum3_pair_publish)
+    float logu;
+};
+
+template <int TK, int MK, int PW, int MAXT>
+__device__ __forceinline__ void hmc_produce(const RunArgs& a, int pt, int G, uint64_t chain_id, MomentumSlot& r) {
+    constexpr int NT = MAXT / (32 * PW);             // compute threads per producer thread
+    const int lane = pt & 31, nwarp = G >> 5, nthr = G + 32 * PW;
+    PhiloxKeys keys;
+    philox_make_keys(a.seed, chain_id, keys);
+    VecConst<4> vc[NT][2];
+    PhiloxFixed pfix[NT][2];
+    uint32_t zmask[NT][2][4];
+#pragma unroll
+    for (int u = 0; u < NT; ++u)
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+            const int grp = pt + 32 * PW * u + k * G;
+            load_consts<TK, MK, 4>(a.t, 4 * grp, vc[u][k]);
+            philox_fix(keys, chain_id, grp, STREAM_MOMENTUM, pfix[u][k]);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) zmask[u][k][j] = 4 * grp + j < a.t.D ? 0xFFFFFFFFu : 0u;
+        }
+    float logu_lanes = 0.0f;
+    for (int n = a.it0, m = 0; n < a.it1; ++n, ++m) {
+        if (m > 0) bar_sync(BAR_SLOT_EMPTY, nthr);        // the compute warps have finished iteration n-1's trajectory
+        float4 pv[NT][2];
+        float kin[NT][2];
+#pragma unroll
+        for (int u = 0; u < NT; ++u)
+#pragma unroll
+            for (int k = 0; k < 2; ++k) {
+                float z[4], p[4];
+                philox_normals<4>(keys, pfix[u][k], (uint32_t)n, (uint32_t)(pt + 32 * PW * u + k * G), z);
+                kin[u][k] = 0.0f;
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    z[j] = __uint_as_float(__float_as_uint(z[j]) & zmask[u][k][j]);
+                    p[j] = (MK == HMCX_MASS_DIAG) ? mul(z[j], vc[u][k].sd[j]) : z[j];
+                    kin[u][k] = sum_in<MK == HMCX_MASS_NONE>(kin[u][k], kterm1<MK>(p[j], vc[u][k].im[j]), j == 0);
+                }
+                pv[u][k] = make_float4(p[0], p[1], p[2], p[3]);
+            }
+#pragma unroll
+        for (int u = 0; u < NT; ++u) {                // both groups in one butterfly: lanes [0,16) group 0, [16,32) 1
+            const bool h16 = lane & 16;
+            float x = add(h16 ? kin[u][1] : kin[u][0], __shfl_xor_sync(0xffffffffu, h16 ? kin[u][0] : kin[u][1], 16));
+#pragma unroll
+            for (int o = 8; o > 0; o >>= 1) x = add(x, __shfl_xor_sync(0xffffffffu, x, o));
+            kin[u][0] = x;
+        }
+        float logu = 0.0f;
+        if (pt < 32) {                                // 32 iterations per Philox call, lane l for iteration n + l
+            const int phase = m & 31;
+            if (phase == 0) logu_lanes = philox_log_uniform(keys, chain_id, (uint64_t)(n + lane));
+            logu = __shfl_sync(0xffffffffu, logu_lanes, phase);
+        }
+#pragma unroll
+        for (int u = 0; u < NT; ++u) {
+            const int tt = pt + 32 * PW * u;
+            if (tt < G) {
+                r.p[0][tt] = pv[u][0];
+                r.p[1][tt] = pv[u][1];
+                if ((lane & 15) == 0) r.kin[(tt >> 5) + (lane >> 4) * nwarp] = kin[u][0];
+            }
+        }
+        if (pt == 0) r.logu = logu;
+        bar_arrive(BAR_SLOT_FULL, nthr);
+#ifdef HMCX_HMC_PROF
+        hmc_prof_publish(n, a.it0, pt);
+#endif
+    }
+}
 
 // MAXT = CTA size the instantiation is compiled for (register budget 64K/MAXT): chains of D <= 1024 run with <= 256
 // threads and get a generous budget, which lets the compiler software-pipeline the next iteration's RNG.
@@ -360,18 +481,23 @@ __device__ __forceinline__ long long* hmc_prof_row(int n, int it0) {
 // K = 2 with MAXT <= 128 (PAIR): every group keeps its own partial sums and enters the reductions in the place it has
 // in the K = 1 CTA of twice the threads (block_sum3_pair_*, block_sum1_groups), so the run is bit-identical to that
 // geometry; the other K > 1 forms sum their groups per thread first (a different tree).
-template <int TK, int MK, int E, int K, int MAXT, bool SINK = false, bool PHILOX = false, int CS = 1, bool NUTS = true>
-__global__ void __launch_bounds__(MAXT)
+// PW > 0 (paired Philox loop only): the CTA is G compute threads followed by PW producer warps (hmc_produce).
+template <int TK, int MK, int E, int K, int MAXT, bool SINK = false, bool PHILOX = false, int CS = 1, bool NUTS = true,
+          int PW = 0>
+__global__ void __launch_bounds__(MAXT + 32 * PW)
 hmc_run_kernel(const RunArgs a) {
     static_assert(CS == 1 || (K == 1 && !SINK), "cluster form: one group per thread, no sink");
     constexpr bool PAIR = K == 2 && MAXT <= 128 && CS == 1;
     constexpr int KP = PAIR ? K : 1;                          // partial sums per thread
     static_assert(!PAIR || E == 4, "the paired form mirrors the float4 (K = 1) geometry");
+    static_assert(PW == 0 || (PAIR && PHILOX && !SINK && !NUTS && MAXT % (32 * PW) == 0),
+                  "producer warps: the paired Philox loop only");
     __shared__ __align__(16) float s_red[2][100];
     __shared__ __align__(16) float4 s_part[3][8];           // CS > 1: per-warp partials (two iteration parities + misc)
     __shared__ float s_eps[2];
+    __shared__ MomentumSlot s_slot;                        // PW > 0 only (unreferenced, and dropped, otherwise)
 
-    const int c = blockIdx.x / CS, rank = blockIdx.x % CS, G = blockDim.x;
+    const int c = blockIdx.x / CS, rank = blockIdx.x % CS, G = blockDim.x - 32 * PW;
     const int tid = threadIdx.x, gt = rank * G + tid;       // thread index within the CTA / within the chain
     const bool lead = tid == 0 && rank == 0;                // writes the chain's scalar outputs
     const bool nuts = NUTS && a.nuts;
@@ -379,6 +505,12 @@ hmc_run_kernel(const RunArgs a) {
     const int ld = t.ld, D = t.D;
     const size_t row = (size_t)c * ld;
     const uint64_t chain_id = a.chain_offset + (uint64_t)c;
+    if constexpr (PW > 0) {
+        if (tid >= G) {
+            hmc_produce<TK, MK, PW, MAXT>(a, tid - G, G, chain_id, s_slot);
+            return;
+        }
+    }
 
     VecConst<E> vc[K];
     float qc[K][E], q[K][E], p[K][E];
@@ -396,7 +528,8 @@ hmc_run_kernel(const RunArgs a) {
             zmask[k][j] = e0 + j < D ? 0xFFFFFFFFu : 0u;
         }
     }
-    if (CS == 1 && MAXT <= 256) block_sum3_small_init(s_red, KP);
+    // PW > 0 stores the .y / .z of all 8 slots and uses nothing else from them (.x comes from the producers)
+    if (CS == 1 && MAXT <= 256 && PW == 0) block_sum3_small_init(s_red, KP);
 #ifdef HMCX_HMC_PROF
     if (PAIR && tid == 0 && blockIdx.x < HMC_PROF_CTAS) {
         int sm;
@@ -416,11 +549,11 @@ hmc_run_kernel(const RunArgs a) {
 #pragma unroll
             for (int j = 0; j < E; ++j)
                 r[PAIR ? k : 0] = add(r[PAIR ? k : 0], uterm1<TK>(qc[k][j], vc[k].mean[j], vc[k].ivar[j]));
-        if constexpr (PAIR) r[0] = block_sum1_groups<KP>(r, s_red[1]);
+        if constexpr (PAIR) r[0] = block_sum1_groups<KP, PW>(r, s_red[1]);
         else if (CS > 1) r[0] = cluster_sum1<CS>(r[0], s_part[2]);
         else block_sum<1>(r, s_red[1]);
         lp_cur = log_prob_from_sum(r[0], t.log_norm);
-        __syncthreads();
+        chain_sync<PW>(G);
     }
     if (a.lp_carry && a.it0 > 0) lp_cur = a.lp_carry[c];
 
@@ -464,7 +597,7 @@ hmc_run_kernel(const RunArgs a) {
     float zn[K][E];
     PhiloxKeys keys;
     PhiloxFixed pfix[K];
-    if (PHILOX) {
+    if (PHILOX && PW == 0) {
         philox_make_keys(a.seed, chain_id, keys);
 #pragma unroll
         for (int k = 0; k < K; ++k) {
@@ -488,18 +621,35 @@ hmc_run_kernel(const RunArgs a) {
             for (int j = 0; j < E; ++j) zn[k][j] = __uint_as_float(__float_as_uint(zn[k][j]) & zmask[k][j]);
         }
     };
-    if (a.it0 < a.it1) draw(a.it0);
+    if (PW == 0 && a.it0 < a.it1) draw(a.it0);
 
     // the MH test's log-uniforms: warp 0 produces them 32 iterations at a time, lane l for iteration n+l, so the ~70
     // dependent instructions of Philox + logf leave the per-iteration critical path (every other warp waits for warp 0 at
-    // the reduction's barrier) and cost 1/32 of the issue slots
+    // the reduction's barrier) and cost 1/32 of the issue slots.  The producer form draws them in its producer warps.
     float logu_lanes = 0.0f;
-    const bool warp0 = tid < 32 && rank == 0;
+    const bool warp0 = PW == 0 && tid < 32 && rank == 0;
 
     for (int n = a.it0; n < a.it1; ++n) {
 #ifdef HMCX_HMC_PROF
         long long* const prow = PAIR ? hmc_prof_row(n, a.it0) : nullptr;
 #endif
+        // producer form: this iteration's momentum, kinetic sum (the 8 virtual warps' slots added in warp order, as
+        // block_sum3_slots adds them) and log-uniform from the producers' slot
+        float slot_kin = 0.0f, slot_logu = 0.0f;
+        if constexpr (PW > 0) {
+            HMC_MARK(prow, 6);              // before the slot-full wait
+            bar_sync(BAR_SLOT_FULL, G + 32 * PW);
+            HMC_MARK(prow, 7);
+            const MomentumSlot& r = s_slot;
+#pragma unroll
+            for (int k = 0; k < K; ++k) {
+                const float4 v = r.p[k][tid];
+                p[k][0] = v.x; p[k][1] = v.y; p[k][2] = v.z; p[k][3] = v.w;
+            }
+            const float4 k0 = *reinterpret_cast<const float4*>(r.kin), k1 = *reinterpret_cast<const float4*>(r.kin + 4);
+            slot_kin = add(add(add(add(add(add(add(k0.x, k0.y), k0.z), k0.w), k1.x), k1.y), k1.z), k1.w);
+            slot_logu = r.logu;
+        }
         HMC_MARK(prow, 0);                  // the iteration starts
         if (NUTS && a.eps_schedule) eps = a.eps_schedule[(size_t)n * t.C + c];
         const float half = mul(0.5f, eps);
@@ -533,13 +683,19 @@ hmc_run_kernel(const RunArgs a) {
             const bool first = i == k;                               // the partial's first group
 #pragma unroll
             for (int j = 0; j < E; ++j) {
-                p[k][j] = (MK == HMCX_MASS_DIAG) ? mul(zn[k][j], vc[k].sd[j]) : zn[k][j];
-                r0[i] = sum_in<MK == HMCX_MASS_NONE>(r0[i], kterm1<MK>(p[k][j], vc[k].im[j]), first && j == 0);
+                if (PW == 0) {
+                    p[k][j] = (MK == HMCX_MASS_DIAG) ? mul(zn[k][j], vc[k].sd[j]) : zn[k][j];
+                    r0[i] = sum_in<MK == HMCX_MASS_NONE>(r0[i], kterm1<MK>(p[k][j], vc[k].im[j]), first && j == 0);
+                }
                 q[k][j] = qc[k][j];
             }
         }
         // ---- leapfrog (:973) : thread-private ----
-        if (PAIR) {
+        if (PW > 0) {
+            trajectory_groups<TK, MK, E, K>(q, p, vc, eps, half, a.L, []() {});
+            // the producers draw iteration n+1 while this iteration is in its serial tail
+            if (n + 1 < a.it1) bar_arrive(BAR_SLOT_EMPTY, G + 32 * PW);
+        } else if (PAIR) {
             // the normals of iteration n+1 (zn is consumed above; branch-free, one unused draw after the last iteration)
             trajectory_groups<TK, MK, E, K>(q, p, vc, eps, half, a.L, [&]() { draw(n + 1); });
         } else {
@@ -563,12 +719,21 @@ hmc_run_kernel(const RunArgs a) {
         // unused draw after the last iteration) so that it shares a basic block with the reduction's shuffle chain.
         // The cluster form publishes its partials first: the draw then sits between the stores and the barrier.
         HMC_MARK(prow, 1);                  // trajectory and per-thread sums done
-        if constexpr (PAIR) block_sum3_pair_publish(r0, r1, r2, logu, s_red[n & 1]);
+        if constexpr (PW > 0) block_sum2_pair_publish(r1, r2, s_red[n & 1], G >> 5);
+        else if constexpr (PAIR) block_sum3_pair_publish(r0, r1, r2, logu, s_red[n & 1]);
         else if (CS > 1) cluster_sum3_publish(r0[0], r1[0], r2[0], logu, s_part[n & 1]);
         HMC_MARK(prow, 2);                  // slots stored
         if (!PAIR && (PHILOX || n + 1 < a.it1)) draw(n + 1);     // the paired form draws inside the trajectory
         HMC_MARK(prow, 3);                  // next normals drawn
-        if (PAIR) {
+        if (PW > 0) {
+            chain_sync<PW>(G);
+            HMC_MARK(prow, 4);
+            // .x and sbuf[32] are never stored in this form: their sums are dead code, which the compiler drops
+            float unused_a, unused_extra;
+            block_sum3_slots(unused_a, r1[0], r2[0], unused_extra, s_red[n & 1]);
+            r0[0] = slot_kin;
+            logu = slot_logu;
+        } else if (PAIR) {
             __syncthreads();                // block_sum3_pair_collect, with a stamp after its barrier
             HMC_MARK(prow, 4);
             block_sum3_slots(r0[0], r1[0], r2[0], logu, s_red[n & 1]);
@@ -608,11 +773,11 @@ hmc_run_kernel(const RunArgs a) {
                         s[PAIR ? k : 0] = add(s[PAIR ? k : 0], uterm1<TK>(qc[k][j], vc[k].mean[j], vc[k].ivar[j]));
                     }
                 }
-                if constexpr (PAIR) s[0] = block_sum1_groups<KP>(s, s_red[(n & 1) ^ 1]);
+                if constexpr (PAIR) s[0] = block_sum1_groups<KP, PW>(s, s_red[(n & 1) ^ 1]);
                 else if (CS > 1) s[0] = cluster_sum1<CS>(s[0], s_part[2]);  // every CTA of the cluster takes this branch
                 else block_sum<1>(s, s_red[(n & 1) ^ 1]);
                 lp_cur = log_prob_from_sum(s[0], t.log_norm);
-                __syncthreads();          // the next iteration reduces through the same buffer
+                chain_sync<PW>(G);        // the next iteration reduces through the same buffer
             }
         }
         // ---- bookkeeping (:1007-1026): store only for n > burn ----
@@ -1026,7 +1191,8 @@ int elem_gibbs(const hmcx_mass_t* mass, const hmcx_rng_t* rng, int D, int C, int
 //                      pays the iteration's fixed cost (reduction, barrier, MH, loop) once: half the warps, ~20 % fewer
 //                      instructions per chain.  Measured at 256 chains (2 CTAs per SM; H100 80GB HBM3, 400 W), launch
 //                      time paired / K=1: 1.05 at ld 512, 1.12 at 768, 0.98 at 832 and 896, 0.94 at 960 and 1024.  Below
-//                      ~7 warps per K=1 CTA the halved warp count leaves the schedulers short of warps and latency wins;
+//                      ~7 warps per K=1 CTA the halved warp count leaves the schedulers short of warps and latency wins.
+//                      Up to 2 chains per SM it runs with two producer warps per CTA (PW = 2, hmc_produce);
 //                    * D > 2560: K=2 in CTAs of <= 512 threads (at config 5, D=4096, CTAs of 768-1024 threads x 1 are
 //                      slower).
 //   tuning 1: E=4, K=1 forced.
@@ -1119,8 +1285,12 @@ int elem_hmc_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmc
     if (!pick_geometry(ld, tuning, pair_ok, E, K, G)) return tuning ? HMCX_ERR_INVALID_ARG : HMCX_ERR_UNSUPPORTED;
     a.lp_carry = workspace;                                // [C] floats (hmcx_hmc_workspace_bytes) or NULL
     const bool pair = tuning == 0 && K == 2 && G <= 128 && pair_ok;
+    // the producer form's CTAs have 1.5x the threads and ~1.5x the registers per thread: it runs while every chain's CTA
+    // finds an SM beside at most one other, and the plain paired form above that (measured at 512 chains, DESIGN §3.1)
+    const bool producers = pair && C <= 2 * sm_count();
 #define CALL(TK, MK)                                                                                    \
-    if (pair) hmc_run_kernel<TK, MK, 4, 2, 128, false, true, 1, false><<<C, G, 0, st>>>(a);             \
+    if (producers) hmc_run_kernel<TK, MK, 4, 2, 128, false, true, 1, false, 2><<<C, G + 64, 0, st>>>(a);  \
+    else if (pair) hmc_run_kernel<TK, MK, 4, 2, 128, false, true, 1, false><<<C, G, 0, st>>>(a);        \
     else if (E == 2 && K == 1) hmc_run_kernel<TK, MK, 2, 1, 1024><<<C, G, 0, st>>>(a);                  \
     else if (E == 2) hmc_run_kernel<TK, MK, 2, 2, 1024><<<C, G, 0, st>>>(a);                            \
     else if (K == 1 && G <= 256 && philox && !a.nuts)                                                   \
@@ -1138,15 +1308,19 @@ int elem_hmc_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmc
 }
 
 #ifdef HMCX_HMC_PROF
-// developer build only (scripts/prof_hmc_phases.py): copies out and clears the stamps; returns the number of stamps
-extern "C" int hmcx_debug_hmc_prof(long long* stamps, int* sm) {
+// developer build only (scripts/prof_hmc_phases.py): copies out and clears the stamps (and the producer form's
+// publication stamps, [CTA][iteration]); returns the number of stamps
+extern "C" int hmcx_debug_hmc_prof(long long* stamps, int* sm, long long* pub) {
     const int n = HMC_PROF_CTAS * HMC_PROF_WARPS * HMC_PROF_ITS * HMC_PROF_IDS;
     cudaDeviceSynchronize();
     cudaMemcpyFromSymbol(stamps, g_hmc_prof, sizeof(long long) * n);
     cudaMemcpyFromSymbol(sm, g_hmc_prof_sm, sizeof(int) * HMC_PROF_CTAS);
+    cudaMemcpyFromSymbol(pub, g_hmc_prof_pub, sizeof(long long) * HMC_PROF_CTAS * HMC_PROF_ITS);
     void* p = nullptr;
     cudaGetSymbolAddress(&p, g_hmc_prof);
     cudaMemset(p, 0, sizeof(long long) * n);
+    cudaGetSymbolAddress(&p, g_hmc_prof_pub);
+    cudaMemset(p, 0, sizeof(long long) * HMC_PROF_CTAS * HMC_PROF_ITS);
     cudaDeviceSynchronize();
     return n;
 }

@@ -7,10 +7,15 @@ every CTA over 64 consecutive iterations (from iteration 256):
   0 the iteration's trajectory starts (gibbs)      1 trajectory and per-thread sums done
   2 slots published                                3 next iteration's normals drawn
   4 the reduction's barrier passed                 5 MH decided, state selected, row stored
+  6, 7 (producer form) before and after the wait for the iteration's momentum slot, just before stamp 0
+and, in the producer form, when producer warp 0 published each iteration's slot.
 Reported per stamp id k: cycles from stamp 0 of the same iteration (mean, std, p10, p90); `iter`: stamp 0 to the next
 iteration's stamp 0; `tail`: stamp 1 to the next iteration's stamp 0 (the serial section between two trajectories).
 `both_in_tail`: for SMs holding two of the chains, cycles per iteration during which warp 0 of both chains sat in
-their tail at once (clock64 is per SM, so the two chains' stamps share a time base)."""
+their tail at once (clock64 is per SM, so the two chains' stamps share a time base).  `slot_wait`: stamp 6 to
+stamp 7, how long the compute warps waited for the producer warps (all zero without them).  `published`: the slot's
+publication minus stamp 6 of compute warp 0 in the same iteration (negative: the slot was ready before the compute
+warps asked for it; null without producer warps)."""
 import argparse, ctypes as C, json, os, subprocess, sys, tempfile
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -72,18 +77,23 @@ def main():
     out = torch.empty((256, 1000, 1024), dtype=torch.float32, device=dev)
     stamps = (C.c_longlong * (CTAS * WARPS * ITS * IDS))()
     sm = (C.c_int * CTAS)()
+    pub = (C.c_longlong * (CTAS * ITS))()
     engine.hmc_run(tgt, q0, 1000, 10, args.eps, seed=0, out=out, device=dev)
-    lib.hmcx_debug_hmc_prof(stamps, sm)
+    lib.hmcx_debug_hmc_prof(stamps, sm, pub)
     rel = {k: [] for k in range(1, 6)}
-    it, tail, both, rate = [], [], [], []
+    it, tail, both, rate, wait, published = [], [], [], [], [], []
     for rep in range(args.reps):
         r = engine.hmc_run(tgt, q0, 1000, 10, args.eps, seed=1 + rep, out=out, device=dev)
-        lib.hmcx_debug_hmc_prof(stamps, sm)
+        lib.hmcx_debug_hmc_prof(stamps, sm, pub)
         rate.append(float(r.accepted.float().mean()))
         s = np.frombuffer(stamps, dtype=np.int64).reshape(CTAS, WARPS, ITS, IDS).astype(np.float64)
         for k in rel:
             rel[k].append((s[..., k] - s[..., 0]).ravel())
         it.append((s[:, :, 1:, 0] - s[:, :, :-1, 0]).ravel())
+        wait.append((s[..., 7] - s[..., 6]).ravel())
+        pb = np.frombuffer(pub, dtype=np.int64).reshape(CTAS, ITS).astype(np.float64)
+        if pb.all():
+            published.append((pb - s[:, 0, :, 6]).ravel())
         tail.append((s[:, :, 1:, 0] - s[:, :, :-1, 1]).ravel())
         by_sm = {}
         for b in range(CTAS):
@@ -101,7 +111,8 @@ def main():
             both.append(overlap(*clip) / n_it)
     line = {'eps': args.eps, 'init_scale': args.init_scale, 'accept_rate': rate,
             'since_stamp0': {str(k): stats(np.concatenate(v)) for k, v in rel.items()},
-            'iter': stats(np.concatenate(it)), 'tail': stats(np.concatenate(tail)),
+            'iter': stats(np.concatenate(it)), 'slot_wait': stats(np.concatenate(wait)),
+            'published': stats(np.concatenate(published)) if published else None, 'tail': stats(np.concatenate(tail)),
             'both_in_tail': stats(both) if both else None, 'sm_pairs': len(both) // args.reps}
     print(json.dumps(line))
 
