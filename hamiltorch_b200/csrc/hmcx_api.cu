@@ -41,6 +41,9 @@ int mlp_pack_x(const hmcx_target_t*, float*, cudaStream_t);
 int rmhmc_cta_run(const hmcx_target_t*, const hmcx_rmhmc_t*, const hmcx_rng_t*, const float*, float*, const float*, int,
                   int, int, int, int, int, int, float*, uint8_t*, uint8_t*, float*, int32_t*, const float*, float*, float*,
                   float*, float*, int, float*, cudaStream_t);
+int diag_means(const float*, long long, long long, int, int, int, double*, double*, cudaStream_t);
+int diag_acov(const float*, long long, long long, int, int, int, const double*, const double*, int, double*, double*,
+              cudaStream_t);
 }  // namespace hmcx
 
 static inline bool is_elem(const hmcx_target_t* t) {
@@ -252,6 +255,26 @@ int hmcx_copy_rows_async(void* dst, size_t dpitch, const void* src, size_t spitc
     if (width == 0 || height == 0) return HMCX_OK;
     return cudaMemcpy2DAsync(dst, dpitch, src, spitch, width, height, cudaMemcpyDefault, (cudaStream_t)stream) == cudaSuccess
                ? HMCX_OK : HMCX_ERR_CUDA;
+}
+
+static inline bool diag_args_ok(const float* x, int64_t cs, int64_t ds, int32_t C, int32_t n, int32_t D) {
+    return x && cs >= 0 && ds >= 0 && C >= 1 && n >= 4 && D >= 1;
+}
+
+int hmcx_diag_means(const float* x, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t D,
+                    double* mu_out, double* mu_sum_out, void* stream) {
+    if (!diag_args_ok(x, chain_stride, draw_stride, C, n, D) || !mu_out || !mu_sum_out) return HMCX_ERR_INVALID_ARG;
+    return hmcx::diag_means(x, chain_stride, draw_stride, C, n, D, mu_out, mu_sum_out, (cudaStream_t)stream);
+}
+
+int hmcx_diag_acov(const float* x, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t D,
+                   const double* mu, const double* mu_bar, int32_t lag_begin, double* acov_out, double* between_out,
+                   void* stream) {
+    if (!diag_args_ok(x, chain_stride, draw_stride, C, n, D) || !mu || !acov_out || lag_begin < 0 ||
+        (mu_bar && !between_out))
+        return HMCX_ERR_INVALID_ARG;
+    return hmcx::diag_acov(x, chain_stride, draw_stride, C, n, D, mu, mu_bar, lag_begin, acov_out, between_out,
+                           (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -66,7 +66,29 @@ def pooled_moments(moment_sum, moment_sumsq, count_per_chain, group=None):
     return mean, var.clamp_min(0.0), total
 
 
-def sample_chains_sharded(log_prob_func, params_init, gather_samples=False, runner=None, **kwargs):
+def pooled_diagnostics(local_samples, partials=None, group=None):
+    """Split-R-hat, ESS and MCSE (``diagnostics.summary``) over the chains of ALL ranks, without moving a sample: each
+    rank runs the two streaming passes over its own (C_local, n, D) block and the per-stage sums over half-chains are
+    all-reduced -- the half-chain means with the half-chain count (D+1 values), the first lag block with the
+    between-chain sum ((32+1)*D), then one (32, D) reduction per further lag block.  Every rank ends with identical
+    results.  ``local_samples``: anything ``diagnostics.summary`` accepts (n and D equal on every rank).
+    ``partials`` replaces the CUDA stages: a callable local_samples -> an object with ``means`` / ``acov`` stages (used
+    by the CPU tests of this host logic)."""
+    from . import diagnostics
+    rank, world = _world()
+    part = partials(local_samples) if partials is not None else diagnostics.NativePartials(local_samples)
+
+    def all_reduce(t):
+        t = t.contiguous()
+        if world > 1:
+            dist.all_reduce(t, op=dist.ReduceOp.SUM, group=group)
+        return t
+
+    return diagnostics.summary_from_partials(part, all_reduce, num_draws=part.n)
+
+
+def sample_chains_sharded(log_prob_func, params_init, gather_samples=False, runner=None, diagnostics=False,
+                          diagnostics_partials=None, **kwargs):
     """``sample_chains`` over all ranks.  ``params_init`` is the FULL (C, D) batch on every rank (it is tiny next to
     the samples); each rank advances its block of chains on its own GPU.
 
@@ -74,7 +96,10 @@ def sample_chains_sharded(log_prob_func, params_init, gather_samples=False, runn
     ``local`` (this rank's HMCResult) and, when ``gather_samples``, ``samples`` (C, S-burn, D) collected with one
     all-gather.  With the sample sink's ``moments=True`` the per-chain running sums are pooled over all ranks by one
     O(D) all-reduce: ``posterior_mean`` / ``posterior_var`` (D,) fp64, ``posterior_n`` -- no sample ever leaves its GPU.  Injected-stream arguments ``normals`` (S, C, D) / ``log_uniforms`` (S, C) are sliced per rank.
-    ``runner`` replaces ``samplers.sample_chains`` (used by the CPU tests of this host logic).
+    With ``diagnostics=True``, ``diagnostics`` holds split-R-hat / ESS / MCSE over all chains of all ranks
+    (``pooled_diagnostics`` of each rank's samples; needs the samples on the GPU).
+    ``runner`` replaces ``samplers.sample_chains`` and ``diagnostics_partials`` the diagnostics' CUDA stages (used by
+    the CPU tests of this host logic).
     """
     from . import samplers
     rank, world = _world()
@@ -104,4 +129,8 @@ def sample_chains_sharded(log_prob_func, params_init, gather_samples=False, runn
     if getattr(local, 'moment_sum', None) is not None:          # sink moments requested: pool them over all ranks
         out['posterior_mean'], out['posterior_var'], out['posterior_n'] = pooled_moments(
             local.moment_sum, local.moment_sumsq, local.moment_count)
+    if diagnostics:
+        from .engine import HMCResult
+        src = local if isinstance(local, HMCResult) else local.samples_padded[..., :local.dim]
+        out['diagnostics'] = pooled_diagnostics(src, partials=diagnostics_partials)
     return out

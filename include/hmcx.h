@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define HMCX_ABI_VERSION 8
+#define HMCX_ABI_VERSION 9
 
 #define HMCX_MLP_TC_AUTO 0
 #define HMCX_MLP_TC_OFF  1
@@ -429,6 +429,28 @@ int hmcx_split_run_sink(const hmcx_target_t* target, const hmcx_mass_t* mass, co
  */
 int hmcx_copy_rows_async(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t height,
                          void* stream);
+
+/*
+ * Convergence diagnostics of a sample block (ABI v9): the two streaming passes behind split-R-hat, effective sample size
+ * and Monte-Carlo standard error (Stan reference manual; hamiltorch_b200/diagnostics.py runs the Geyer scan on their
+ * output).  The block is fp32 x[c, s, d] = x[c*chain_stride + s*draw_stride + d] (strides in elements, unit stride along
+ * D): C chains of n >= 4 draws.  Half-chain 2c is draws [0, m) of chain c and 2c+1 is draws [n-m, n), m = n/2 (an odd n
+ * drops the middle draw).  All sums are fp64 and run in a fixed order (no atomics): the same block gives the same bits.
+ * The stages are separate calls so that ranks holding different chains can all-reduce between them.
+ *   hmcx_diag_means  mu_out [2C, D] fp64: the mean of every half-chain;  mu_sum_out [D] fp64: sum over half-chains of mu
+ *   hmcx_diag_acov   acov_out [HMCX_DIAG_LAG_BLOCK, D] fp64: row k = sum_j gamma_j(lag_begin + k),
+ *                    gamma_j(t) = (1/m) sum_{s < m-t} (x_s - mu_j)(x_{s+t} - mu_j) over half-chain j (0 for t >= m);
+ *                    mu = hmcx_diag_means' mu_out.  With mu_bar [D] (the pooled mean of the half-chain means, may be
+ *                    NULL) between_out [D] = sum_j (mu_j - mu_bar)^2.
+ * NULL x / outputs, C < 1, n < 4, D < 1, negative strides or lag_begin: HMCX_ERR_INVALID_ARG.
+ */
+#define HMCX_DIAG_LAG_BLOCK 32
+
+int hmcx_diag_means(const float* x, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t D,
+                    double* mu_out, double* mu_sum_out, void* stream);
+int hmcx_diag_acov(const float* x, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t D,
+                   const double* mu, const double* mu_bar, int32_t lag_begin, double* acov_out, double* between_out,
+                   void* stream);
 
 #ifdef __cplusplus
 }
