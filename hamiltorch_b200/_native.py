@@ -15,7 +15,7 @@ LIB_PATH = os.path.join(_HERE, 'lib', 'libhmcx.so')
 OK, ERR_INVALID_ARG, ERR_UNSUPPORTED, ERR_CUDA = 0, -1, -2, -3
 MASS_NONE, MASS_DIAG, MASS_FULL = 0, 1, 2
 RNG_INJECTED, RNG_PHILOX = 0, 1
-ABI_VERSION = 9
+ABI_VERSION = 10
 
 
 class NativeError(RuntimeError):
@@ -134,9 +134,17 @@ _PROTOS = {
                                   C.c_void_p, C.c_void_p]),
     'hmcx_diag_acov': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                  C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    'hmcx_rank_workspace_bytes': (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
+    'hmcx_rank_pass': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                 C.c_int32, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_int64,
+                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    'hmcx_rank_indicator': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                      C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
 }
 
 DIAG_LAG_BLOCK = 32                     # HMCX_DIAG_LAG_BLOCK: lags per hmcx_diag_acov pass
+RANK_MAX_DRAWS = 2147418112             # HMCX_RANK_MAX_DRAWS: largest C*n hmcx_rank_pass takes
+RANK_MAX_SLAB = 65535                   # HMCX_RANK_MAX_SLAB: most dimensions per hmcx_rank_pass
 
 EXPORTED_SYMBOLS = tuple(_PROTOS)
 

@@ -44,6 +44,11 @@ int rmhmc_cta_run(const hmcx_target_t*, const hmcx_rmhmc_t*, const hmcx_rng_t*, 
 int diag_means(const float*, long long, long long, int, int, int, double*, double*, cudaStream_t);
 int diag_acov(const float*, long long, long long, int, int, int, const double*, const double*, int, double*, double*,
               cudaStream_t);
+size_t rank_workspace_bytes(int, int, int);
+int rank_pass(const float*, long long, long long, int, int, int, int, int, float*, long long, long long, float*,
+              long long, long long, double*, int*, void*, cudaStream_t);
+int rank_indicator(const float*, long long, long long, int, int, int, const double*, float*, long long, long long,
+                   cudaStream_t);
 }  // namespace hmcx
 
 static inline bool is_elem(const hmcx_target_t* t) {
@@ -275,6 +280,42 @@ int hmcx_diag_acov(const float* x, int64_t chain_stride, int64_t draw_stride, in
         return HMCX_ERR_INVALID_ARG;
     return hmcx::diag_acov(x, chain_stride, draw_stride, C, n, D, mu, mu_bar, lag_begin, acov_out, between_out,
                            (cudaStream_t)stream);
+}
+
+static inline bool rank_shape_ok(int32_t C, int32_t n) {
+    return C >= 1 && n >= 4 && (int64_t)C * n <= HMCX_RANK_MAX_DRAWS;
+}
+
+static inline bool rank_slab_ok(int32_t k) {
+    return k >= 1 && k <= HMCX_RANK_MAX_SLAB;
+}
+
+size_t hmcx_rank_workspace_bytes(int32_t C, int32_t n, int32_t k) {
+    if (!rank_shape_ok(C, n) || !rank_slab_ok(k)) return 0;
+    return hmcx::rank_workspace_bytes(C, n, k);
+}
+
+int hmcx_rank_pass(const float* x, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t D,
+                   int32_t d0, int32_t k, float* bulk_z, int64_t bulk_chain_stride, int64_t bulk_draw_stride,
+                   float* fold_z, int64_t fold_chain_stride, int64_t fold_draw_stride, double* quantiles,
+                   int32_t* nonfinite, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!diag_args_ok(x, chain_stride, draw_stride, C, n, D) || !rank_shape_ok(C, n) || !bulk_z || !fold_z ||
+        !quantiles || !nonfinite || !workspace || bulk_chain_stride < 0 || bulk_draw_stride < 0 ||
+        fold_chain_stride < 0 || fold_draw_stride < 0 || d0 < 0 || !rank_slab_ok(k) || (int64_t)d0 + k > D ||
+        workspace_bytes < hmcx::rank_workspace_bytes(C, n, k))
+        return HMCX_ERR_INVALID_ARG;
+    return hmcx::rank_pass(x, chain_stride, draw_stride, C, n, D, d0, k, bulk_z, bulk_chain_stride, bulk_draw_stride,
+                           fold_z, fold_chain_stride, fold_draw_stride, quantiles, nonfinite, workspace,
+                           (cudaStream_t)stream);
+}
+
+int hmcx_rank_indicator(const float* x, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t D,
+                        const double* thr, float* out, int64_t out_chain_stride, int64_t out_draw_stride, void* stream) {
+    if (!diag_args_ok(x, chain_stride, draw_stride, C, n, D) || !thr || !out || out_chain_stride < 0 ||
+        out_draw_stride < 0)
+        return HMCX_ERR_INVALID_ARG;
+    return hmcx::rank_indicator(x, chain_stride, draw_stride, C, n, D, thr, out, out_chain_stride, out_draw_stride,
+                                (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -12,6 +12,10 @@ into ESS is O(lags * D) and runs here with torch ops on the device; it asks for 
 dimension's initial positive sequence has not ended.  Every stage returns sums over half-chains, so the chains of several
 GPUs pool with one all-reduce per stage (``distributed.pooled_diagnostics``) instead of a gather of their samples.
 
+``rank_summary`` adds the rank-normalised, folded split-R-hat, bulk-ESS and tail-ESS of Vehtari et al. (2021) --
+ArviZ's ``rhat(method="rank")`` / ``ess(method="bulk"|"tail")`` -- and the 5 / 50 / 95 % quantiles: a segmented radix
+sort per dimension on the GPU (hmcx_rank.cu) turns the draws into normal scores, which then run through the same passes.
+
 Edge cases per dimension: a non-finite draw makes every output NaN (``max_lag`` 0); when all split draws are equal
 ESS = N, R-hat = 1, MCSE = 0 (``max_lag`` 0); W = 0 with B > 0 gives R-hat = +inf.  Both are read off the exact fp64
 sums: a finite fp32 block cannot overflow them, and equal draws give exactly zero within- and between-chain sums.
@@ -184,12 +188,9 @@ def _ess_from_rho(rho, pairs, I, N):
     return N / torch.clamp(tau, min=1.0 / math.log10(N))
 
 
-def summary_from_partials(partials, all_reduce=None, num_chains=None, num_draws=None):
-    """The diagnostics of the chains behind ``partials`` (a NativePartials, a PooledPartials or any object with the same
-    ``means`` / ``acov`` stages), with ``all_reduce`` summing each stage's output over ranks: one reduction of the
-    half-chain means and count, one of the first lag block together with the between-chain sum, one per further block.
-    Every decision is taken on reduced values, so all ranks take the same ones."""
-    red = all_reduce or (lambda t: t)
+def _first_stage(partials, red):
+    """The means stage and the first lag block, reduced: (K, mu_bar, G (lag_block, D) summed autocovariances, between,
+    W, varp, nonfinite, constant) -- everything split-R-hat needs, and the start of the ESS scan."""
     m, D, TB = partials.m, partials.D, partials.lag_block
     mu_sum, K_local = partials.means()
     buf = red(torch.cat([mu_sum.double(), torch.tensor([float(K_local)], dtype=torch.float64, device=mu_sum.device)]))
@@ -198,12 +199,32 @@ def summary_from_partials(partials, all_reduce=None, num_chains=None, num_draws=
     acov, between = partials.acov(mu_bar, 0)
     buf = red(torch.cat([acov.double(), between.double()[None]]))
     G, between = buf[:TB], buf[TB]
-    Nd = K * m
     W = m / (m - 1) * (G[0] / K)
     Bm = between / (K - 1)
     varp = (m - 1) / m * W + Bm
     nonfinite = ~torch.isfinite(mu_bar)
     constant = (G[0] == 0) & (between == 0) & ~nonfinite
+    return K, mu_bar, G, between, W, varp, nonfinite, constant
+
+
+def _rhat_from_partials(partials):
+    """Split-R-hat alone of the chains behind ``partials``: the means stage and the first lag block, no Geyer scan.
+    Equals ``summary_from_partials(partials).rhat`` bit for bit."""
+    _, _, _, _, W, varp, nonfinite, constant = _first_stage(partials, lambda t: t)
+    rhat = torch.sqrt(varp / W)
+    rhat = torch.where(constant, torch.ones_like(rhat), rhat)
+    return torch.where(nonfinite, torch.full_like(rhat, float('nan')), rhat)
+
+
+def summary_from_partials(partials, all_reduce=None, num_chains=None, num_draws=None):
+    """The diagnostics of the chains behind ``partials`` (a NativePartials, a PooledPartials or any object with the same
+    ``means`` / ``acov`` stages), with ``all_reduce`` summing each stage's output over ranks: one reduction of the
+    half-chain means and count, one of the first lag block together with the between-chain sum, one per further block.
+    Every decision is taken on reduced values, so all ranks take the same ones."""
+    red = all_reduce or (lambda t: t)
+    m = partials.m
+    K, mu_bar, G, between, W, varp, nonfinite, constant = _first_stage(partials, red)
+    Nd = K * m
     active = ~nonfinite & ~constant
     blocks = 1
     while True:
@@ -240,3 +261,103 @@ def summary(samples):
     Returns a ``Diagnostics``; the same block gives the same bits on every call."""
     x = as_block(samples)
     return summary_from_partials(NativePartials(x), num_chains=int(x.shape[0]), num_draws=int(x.shape[1]))
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# Rank-normalised diagnostics (Vehtari, Gelman, Simpson, Carpenter & Buerkner 2021)
+# ------------------------------------------------------------------------------------------------------------------
+class RankDiagnostics:
+    """Per-dimension results of ``rank_summary``, (D,) fp64 on the samples' device: ``rhat`` = max(``rhat_bulk``,
+    ``rhat_tail``), ``ess_bulk``, ``ess_tail``, ``q05``, ``median``, ``q95``; ``num_chains`` and ``num_draws`` of the
+    block; ``max_lag`` (3, D) int64, the largest lag the Geyer scan read on the bulk z, I05 and I95 series, and
+    ``num_lag_blocks``, the autocovariance passes each of the three took."""
+
+    def __init__(self, rhat, rhat_bulk, rhat_tail, ess_bulk, ess_tail, q05, median, q95, num_chains, num_draws,
+                 max_lag, num_lag_blocks):
+        self.rhat, self.rhat_bulk, self.rhat_tail, self.ess_bulk, self.ess_tail = rhat, rhat_bulk, rhat_tail, ess_bulk, ess_tail
+        self.q05, self.median, self.q95 = q05, median, q95
+        self.num_chains, self.num_draws, self.max_lag, self.num_lag_blocks = num_chains, num_draws, max_lag, num_lag_blocks
+
+    def __repr__(self):
+        return ('RankDiagnostics(num_chains=%d, num_draws=%d, D=%d, max rhat=%.4f, min ess_bulk=%.1f, min ess_tail=%.1f)'
+                % (self.num_chains, self.num_draws, self.median.numel(), float(self.rhat.max()),
+                   float(self.ess_bulk.min()), float(self.ess_tail.min())))
+
+
+RANK_WORKSPACE_BUDGET = 256 << 20       # bytes of sort workspace one rank_summary call allocates (at least one dimension)
+_slab_dims_override = None              # tests: force this many dimensions per slab
+
+
+def _slab_dims(lib, C, n, D):
+    if _slab_dims_override is not None:
+        return max(1, min(D, N.RANK_MAX_SLAB, int(_slab_dims_override)))
+    k = max(1, min(D, N.RANK_MAX_SLAB, RANK_WORKSPACE_BUDGET // lib.hmcx_rank_workspace_bytes(C, n, 1)))
+    while k > 1 and lib.hmcx_rank_workspace_bytes(C, n, k) > RANK_WORKSPACE_BUDGET:
+        k -= 1
+    return k
+
+
+def _strides(t):
+    return t.stride(0), t.stride(1)
+
+
+def rank_summary(samples):
+    """Rank-normalised, folded split-R-hat, bulk-ESS, tail-ESS and the 5 / 50 / 95 % quantiles of every dimension of a
+    batched sample block, on its GPU: the defaults of current Stan, ArviZ (``rhat(method="rank")``,
+    ``ess(method="bulk")`` / ``ess(method="tail")``) and PyMC.  Unlike ``summary``'s split-R-hat they flag chains that
+    agree in location but not in scale, and they are defined for heavy-tailed posteriors.
+
+    ``samples``: what ``summary`` accepts (an ``HMCResult``, a strided (C, n, D) or (n, D) CUDA fp32 tensor, the list
+    ``hamiltorch_b200.sample`` returns), refused in the same cases with the same messages.  Per dimension, with the
+    split set = the draws of the half-chains ``summary`` uses (an odd n drops the middle draw) and the full set = all
+    draws: the ranks of the split draws (ties share their mean rank; -0.0 ties with +0.0) become normal scores
+    z = Phi^-1((r - 3/8) / (Ns + 1/4)) rounded to fp32, for the draws (bulk) and for |x - median| (folded); ``rhat_bulk``
+    / ``ess_bulk`` are ``summary``'s split-R-hat / ESS of the bulk scores, ``rhat_tail`` the split-R-hat of the folded
+    ones, ``ess_tail`` = min of the ESS of the indicators x <= q05 and x <= q95; the quantiles are numpy's ``median`` /
+    ``quantile(method='linear')`` of the full set.  A non-finite draw makes every output of its dimension NaN; a
+    constant series has ESS = Ns and R-hat = 1.  The same block gives the same bits on every call.
+
+    Device memory: two (C, n, D) fp32 blocks (the bulk and folded scores; the indicator series reuse them) and one
+    sort workspace of at most ``RANK_WORKSPACE_BUDGET`` bytes -- about 20 bytes per draw of a slab of dimensions, the
+    slab sized to fit (at least one dimension, so a single dimension of more than about 13 M draws takes more; at most
+    65535 dimensions).  The quantiles equal numpy's as values; a zero quantile comes out +0.0 where numpy may give
+    -0.0.  The ranks are global over all chains, so the chains of several GPUs
+    do not pool by all-reduce: run it where the whole block lives."""
+    x = as_block(samples)
+    N.require_cuda()
+    lib = N.load_library()
+    C, n, D = (int(s) for s in x.shape)
+    if C * n > N.RANK_MAX_DRAWS:
+        raise RuntimeError('rank_summary: %d chains x %d draws exceed the %d draws per dimension the rank pass indexes'
+                           % (C, n, N.RANK_MAX_DRAWS))
+    dev = x.device
+    bulk = torch.empty((C, n, D), dtype=torch.float32, device=dev)
+    fold = torch.empty((C, n, D), dtype=torch.float32, device=dev)
+    q = torch.empty((3, D), dtype=torch.float64, device=dev)
+    flag = torch.empty(D, dtype=torch.int32, device=dev)
+    k = _slab_dims(lib, C, n, D)
+    ws_bytes = lib.hmcx_rank_workspace_bytes(C, n, k)
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        st = N.stream_ptr(dev)
+        for d0 in range(0, D, k):
+            rc = lib.hmcx_rank_pass(N.ptr(x), *_strides(x), C, n, D, d0, min(k, D - d0), N.ptr(bulk), *_strides(bulk),
+                                    N.ptr(fold), *_strides(fold), N.ptr(q), N.ptr(flag), N.ptr(ws), ws_bytes, st)
+            N.check(rc, 'hmcx_rank_pass')
+        del ws
+        b = summary_from_partials(NativePartials(bulk))
+        rhat_tail = _rhat_from_partials(NativePartials(fold))
+        tails = []
+        for row, out in ((0, bulk), (2, fold)):          # I05 over the bulk scores, I95 over the folded ones
+            rc = lib.hmcx_rank_indicator(N.ptr(x), *_strides(x), C, n, D, N.ptr(q[row]), N.ptr(out), *_strides(out), st)
+            N.check(rc, 'hmcx_rank_indicator')
+            tails.append(summary_from_partials(NativePartials(out)))
+    bad = flag != 0
+    nan = torch.full((D,), float('nan'), dtype=torch.float64, device=dev)
+    rhat_bulk = torch.where(bad, nan, b.rhat)
+    rhat_tail = torch.where(bad, nan, rhat_tail)
+    ess_tail = torch.where(bad, nan, torch.minimum(tails[0].ess, tails[1].ess))
+    max_lag = torch.stack([torch.where(bad, torch.zeros_like(t.max_lag), t.max_lag) for t in (b, *tails)])
+    return RankDiagnostics(torch.maximum(rhat_bulk, rhat_tail), rhat_bulk, rhat_tail, torch.where(bad, nan, b.ess),
+                           ess_tail, q[0], q[1], q[2], C, n, max_lag,
+                           tuple(t.num_lag_blocks for t in (b, *tails)))

@@ -73,7 +73,8 @@ def pooled_diagnostics(local_samples, partials=None, group=None):
     between-chain sum ((32+1)*D), then one (32, D) reduction per further lag block.  Every rank ends with identical
     results.  ``local_samples``: anything ``diagnostics.summary`` accepts (n and D equal on every rank).
     ``partials`` replaces the CUDA stages: a callable local_samples -> an object with ``means`` / ``acov`` stages (used
-    by the CPU tests of this host logic)."""
+    by the CPU tests of this host logic).  The rank-normalised diagnostics (``diagnostics.rank_summary``) do not pool
+    this way: their ranks are global over all draws of a dimension, so they need the whole block on one GPU."""
     from . import diagnostics
     rank, world = _world()
     part = partials(local_samples) if partials is not None else diagnostics.NativePartials(local_samples)
@@ -97,7 +98,8 @@ def sample_chains_sharded(log_prob_func, params_init, gather_samples=False, runn
     all-gather.  With the sample sink's ``moments=True`` the per-chain running sums are pooled over all ranks by one
     O(D) all-reduce: ``posterior_mean`` / ``posterior_var`` (D,) fp64, ``posterior_n`` -- no sample ever leaves its GPU.  Injected-stream arguments ``normals`` (S, C, D) / ``log_uniforms`` (S, C) are sliced per rank.
     With ``diagnostics=True``, ``diagnostics`` holds split-R-hat / ESS / MCSE over all chains of all ranks
-    (``pooled_diagnostics`` of each rank's samples; needs the samples on the GPU).
+    (``pooled_diagnostics`` of each rank's samples; needs the samples on the GPU) -- split-R-hat, not the
+    rank-normalised R-hat of ``diagnostics.rank_summary``, whose global ranks need every rank's draws.
     ``runner`` replaces ``samplers.sample_chains`` and ``diagnostics_partials`` the diagnostics' CUDA stages (used by
     the CPU tests of this host logic).
     """

@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define HMCX_ABI_VERSION 9
+#define HMCX_ABI_VERSION 10
 
 #define HMCX_MLP_TC_AUTO 0
 #define HMCX_MLP_TC_OFF  1
@@ -451,6 +451,37 @@ int hmcx_diag_means(const float* x, int64_t chain_stride, int64_t draw_stride, i
 int hmcx_diag_acov(const float* x, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t D,
                    const double* mu, const double* mu_bar, int32_t lag_begin, double* acov_out, double* between_out,
                    void* stream);
+
+/*
+ * Rank-normalised diagnostics (ABI v10): the passes behind rank-normalised, folded split-R-hat, bulk-ESS and tail-ESS
+ * (Vehtari, Gelman, Simpson, Carpenter & Buerkner 2021; hamiltorch_b200/diagnostics.py::rank_summary feeds their blocks
+ * through hmcx_diag_means / hmcx_diag_acov).  Same block layout as the v9 entries; L = C*n must be at most
+ * HMCX_RANK_MAX_DRAWS.  The split set is the draws of the half-chains above (Ns = 2*C*(n/2)); the full set is all L.
+ *   hmcx_rank_workspace_bytes  bytes of sort workspace a slab of k dimensions needs (0 for invalid arguments).  The
+ *                    library never allocates: the caller passes the workspace to every hmcx_rank_pass.
+ *   hmcx_rank_pass   for the dimensions d in [d0, d0 + k): per draw of the split set, with r its average rank (ties share
+ *                    the mean of their positions; -0.0 ties with +0.0) among the split draws,
+ *                    bulk_z[c, s, d] = (float) Phi^-1((r - 3/8) / (Ns + 1/4)), and fold_z the same with the ranks of
+ *                    |x - median|; both blocks hold 0 at the dropped middle draw of an odd n.  Each block has its own
+ *                    strides (unit stride along D).  quantiles [3, D] fp64: rows q05, median, q95 of the full set
+ *                    (np.quantile(method='linear') / np.median arithmetic; NaN for a non-finite dimension);
+ *                    nonfinite [D] int32: 1 where the dimension has a non-finite draw, else 0.  Deterministic: the
+ *                    outputs depend on the block only, not on the slab.
+ *   hmcx_rank_indicator  out[c, s, d] = x[c, s, d] <= thr[d] (fp64 comparison) as fp32 0 / 1, thr [D] fp64.
+ * NULL pointers, C < 1, n < 4, D < 1, L too large, negative strides, a slab outside [0, D), k > HMCX_RANK_MAX_SLAB
+ * or a workspace smaller than hmcx_rank_workspace_bytes(C, n, k): HMCX_ERR_INVALID_ARG.  The quantiles equal numpy's
+ * as values; a zero quantile is always +0.0 (numpy may return -0.0, which compares equal).
+ */
+#define HMCX_RANK_MAX_DRAWS 2147418112      /* 2^31 - 2^16: draw indices and tile arithmetic stay in int32 */
+#define HMCX_RANK_MAX_SLAB 65535            /* dimensions per hmcx_rank_pass: one grid row per dimension */
+
+size_t hmcx_rank_workspace_bytes(int32_t C, int32_t n, int32_t k);
+int hmcx_rank_pass(const float* x, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t D,
+                   int32_t d0, int32_t k, float* bulk_z, int64_t bulk_chain_stride, int64_t bulk_draw_stride,
+                   float* fold_z, int64_t fold_chain_stride, int64_t fold_draw_stride, double* quantiles,
+                   int32_t* nonfinite, void* workspace, size_t workspace_bytes, void* stream);
+int hmcx_rank_indicator(const float* x, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t D,
+                        const double* thr, float* out, int64_t out_chain_stride, int64_t out_draw_stride, void* stream);
 
 #ifdef __cplusplus
 }

@@ -21,6 +21,8 @@ run racecheck hmc 400 tests/test_hmc_gpu.py -k "iso256 or nuts or reversib"
 run racecheck rmhmc 400 tests/test_rmhmc_gpu.py -k "funnel2 or funnel32"
 run racecheck mlp 400 tests/test_mlp_tc_gpu.py -k "chain_parity"
 run racecheck dense 400 tests/test_tc_gpu.py -k "edge_shapes"
+run memcheck rank 500 tests/test_rank_diagnostics_gpu.py -k "edge_case or duplicates or slab or odd_dimension"
+run racecheck rank 400 tests/test_rank_diagnostics_gpu.py -k "edge_case or duplicates"
 run synccheck all 400 tests/test_hmc_gpu.py tests/test_rmhmc_gpu.py tests/test_mlp_tc_gpu.py -k "iso256 or funnel2 or funnel32 or chain_parity"
 fi
 # the persistent small-D flow kernel (hmcx_flow.cu): golden chains, live-oracle RMHMC, ragged shapes, all chains-per-warp forms
