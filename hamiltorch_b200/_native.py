@@ -15,7 +15,7 @@ LIB_PATH = os.path.join(_HERE, 'lib', 'libhmcx.so')
 OK, ERR_INVALID_ARG, ERR_UNSUPPORTED, ERR_CUDA = 0, -1, -2, -3
 MASS_NONE, MASS_DIAG, MASS_FULL = 0, 1, 2
 RNG_INJECTED, RNG_PHILOX = 0, 1
-ABI_VERSION = 10
+ABI_VERSION = 11
 
 
 class NativeError(RuntimeError):
@@ -65,13 +65,14 @@ class ConstMetricStruct(C.Structure):
 
 class SinkStruct(C.Structure):
     _fields_ = [('thin', C.c_int32), ('sum', C.c_void_p), ('sumsq', C.c_void_p), ('sum_lo', C.c_void_p),
-                ('sumsq_lo', C.c_void_p)]
+                ('sumsq_lo', C.c_void_p), ('moments_all', C.c_int32)]
 
 
 class NutsStruct(C.Structure):
     _fields_ = [('enabled', C.c_int32), ('desired_accept_rate', C.c_double), ('mu', C.c_double),
                 ('table', C.c_void_p), ('h_bar', C.c_void_p), ('eps_bar', C.c_void_p),
-                ('eps_schedule', C.c_void_p), ('eps_trace', C.c_void_p), ('step_size_init', C.c_double)]
+                ('eps_schedule', C.c_void_p), ('eps_trace', C.c_void_p), ('step_size_init', C.c_double),
+                ('mu_chain', C.c_void_p)]
 
 
 _PROTOS = {
@@ -138,6 +139,9 @@ _PROTOS = {
     'hmcx_rank_pass': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                  C.c_int32, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_int64,
                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    'hmcx_adapt_diag_mass': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                       C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p]),
     'hmcx_rank_indicator': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                       C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
 }

@@ -49,7 +49,11 @@ int rank_pass(const float*, long long, long long, int, int, int, int, int, float
               long long, long long, double*, int*, void*, cudaStream_t);
 int rank_indicator(const float*, long long, long long, int, int, int, const double*, float*, long long, long long,
                    cudaStream_t);
+int adapt_diag_mass(float*, float*, float*, float*, int, int, int, int, const float*, int, float*, float*, double*, double*,
+                    double*, cudaStream_t);
 }  // namespace hmcx
+
+static inline bool has_mu_chain(const hmcx_nuts_t* nuts) { return nuts && nuts->enabled && nuts->mu_chain; }
 
 static inline bool is_elem(const hmcx_target_t* t) {
     return t && (t->kind == HMCX_TARGET_GAUSS_ISO || t->kind == HMCX_TARGET_GAUSS_DIAG);
@@ -109,6 +113,7 @@ int hmcx_hmc_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmc
                  int32_t L, int32_t num_samples, int32_t burn, int32_t iter_begin, int32_t iter_end,
                  float* samples_out, uint8_t* accept_out, uint8_t* diverged_out, float* ham_out,
                  int32_t* num_rejected, int32_t tuning, float* workspace, void* stream) {
+    if (has_mu_chain(nuts)) return HMCX_ERR_UNSUPPORTED;            // per-chain mu: the sink forms only
     return hmcx_hmc_run_sink(target, mass, rng, nuts, q_init, q_cur, eps, C, ld, L, num_samples, burn, iter_begin,
                              iter_end, samples_out, accept_out, diverged_out, ham_out, num_rejected, tuning, workspace,
                              nullptr, stream);
@@ -121,7 +126,8 @@ int hmcx_hmc_run_sink(const hmcx_target_t* target, const hmcx_mass_t* mass, cons
                       int32_t* num_rejected, int32_t tuning, float* workspace, const hmcx_sink_t* sink, void* stream) {
     if (!target) return HMCX_ERR_INVALID_ARG;
     if (sink && sink->thin < 1) return HMCX_ERR_INVALID_ARG;
-    if (sink && sink->thin == 1 && !sink->sum && !sink->sumsq) sink = nullptr;
+    if (sink && sink->thin == 1 && !sink->sum && !sink->sumsq && !has_mu_chain(nuts)) sink = nullptr;
+    if (!sink && has_mu_chain(nuts)) return HMCX_ERR_UNSUPPORTED;
     const bool full_mass = mass && mass->kind == HMCX_MASS_FULL;
     if (is_elem(target) && !full_mass)
         return hmcx::elem_hmc_run(target, mass, rng, nuts, q_init, q_cur, eps, C, ld, L, num_samples, burn,
@@ -150,6 +156,7 @@ int hmcx_split_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const h
                    int32_t ld, int32_t L, int32_t num_samples, int32_t burn, int32_t iter_begin, int32_t iter_end,
                    float* samples_out, uint8_t* accept_out, uint8_t* diverged_out, float* ham_out,
                    int32_t* num_rejected, void* stream) {
+    if (has_mu_chain(nuts)) return HMCX_ERR_UNSUPPORTED;            // per-chain mu: the sink form only
     return hmcx_split_run_sink(target, mass, rng, nuts, scheme, q_init, q_cur, eps, C, ld, L, num_samples, burn,
                                iter_begin, iter_end, samples_out, accept_out, diverged_out, ham_out, num_rejected,
                                nullptr, stream);
@@ -164,6 +171,7 @@ int hmcx_split_run_sink(const hmcx_target_t* target, const hmcx_mass_t* mass, co
     if (sink && (sink->thin < 1 || (sink->sum_lo && !sink->sum) || (sink->sumsq_lo && !sink->sumsq)))
         return HMCX_ERR_INVALID_ARG;
     if (target->kind != HMCX_TARGET_MLP) return HMCX_ERR_UNSUPPORTED;
+    if (!sink && has_mu_chain(nuts)) return HMCX_ERR_UNSUPPORTED;
     return hmcx::mlp_split_run(target, mass, rng, nuts, scheme, q_init, q_cur, eps, C, ld, L, num_samples, burn,
                                iter_begin, iter_end, samples_out, accept_out, diverged_out, ham_out, num_rejected,
                                (cudaStream_t)stream, nullptr, nullptr, nullptr, sink);
@@ -316,6 +324,16 @@ int hmcx_rank_indicator(const float* x, int64_t chain_stride, int64_t draw_strid
         return HMCX_ERR_INVALID_ARG;
     return hmcx::rank_indicator(x, chain_stride, draw_stride, C, n, D, thr, out, out_chain_stride, out_draw_stride,
                                 (cudaStream_t)stream);
+}
+
+int hmcx_adapt_diag_mass(float* sum, float* sumsq, float* sum_lo, float* sumsq_lo, int32_t C, int32_t ld, int32_t D,
+                         int32_t n, const float* eps, int32_t C_chains, float* inv_mass, float* mass_factor,
+                         double* mu_chain, double* h_bar, double* eps_bar, void* stream) {
+    if (!sum || !sumsq || !sum_lo || !sumsq_lo || !eps || !inv_mass || !mass_factor || !mu_chain || !h_bar || !eps_bar ||
+        C < 1 || C_chains < 1 || n < 2 || D < 1 || ld < D || (ld & 3))
+        return HMCX_ERR_INVALID_ARG;
+    return hmcx::adapt_diag_mass(sum, sumsq, sum_lo, sumsq_lo, C, ld, D, n, eps, C_chains, inv_mass, mass_factor, mu_chain,
+                                 h_bar, eps_bar, (cudaStream_t)stream);
 }
 
 }  // extern "C"

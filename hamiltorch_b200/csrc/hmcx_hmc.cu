@@ -164,9 +164,16 @@ struct RunArgs {
     uint64_t seed, chain_offset;
     const float* normals;
     const float* logu;
-    // nuts
+    // nuts.  The mass-adaptation fields of the SINK instantiations (ABI v11) sit in what was alignment padding, so that
+    // every other instantiation keeps its parameter layout and code: mu_per_chain = 1 selects the per-chain mu of the
+    // restarted dual averaging (hmcx_nuts_t.mu_chain), which then shares the storage of the scalar mu
     int nuts;
-    double delta, mu;
+    int mu_per_chain;
+    double delta;
+    union {
+        double mu;
+        const double* mu_chain;
+    };
     const double* table;
     double* h_bar;
     double* eps_bar;
@@ -182,8 +189,10 @@ struct RunArgs {
     uint8_t* diverged;
     float* ham;
     int32_t* num_rejected;
-    // sample sink (hmcx_sink_t): thinning + running first / second moments of the post-burn states
+    // sample sink (hmcx_sink_t): thinning + running first / second moments of the post-burn states (of every iteration of
+    // the launch with moments_all: a mass-adaptation window)
     int thin;
+    int moments_all;
     float* msum;
     float* msumsq;
     float* msum_lo;           // optional: the compensation terms of the running sums (true sum = hi + lo)
@@ -560,6 +569,10 @@ hmc_run_kernel(const RunArgs a) {
     float eps = a.eps[c];
     double h_bar = 0.0, eps_bar = 1.0;
     if (nuts && tid == 0) { h_bar = a.h_bar[c]; eps_bar = a.eps_bar[c]; }
+    double mu_sink = 0.0;                                   // SINK: this chain's mu (the restarted dual averaging's)
+    if constexpr (SINK) {
+        if (nuts && tid == 0) mu_sink = a.mu_per_chain ? a.mu_chain[c] : a.mu;
+    }
     int rejected = 0;
     const int thin = SINK ? a.thin : 1;
     const int keep = SINK ? 1 + (a.S - a.burn - 1) / thin : a.S - a.burn;    // slots per chain in samples_out
@@ -782,7 +795,7 @@ hmc_run_kernel(const RunArgs a) {
         }
         // ---- bookkeeping (:1007-1026): store only for n > burn ----
         if (SINK) {
-            if (n > a.burn) {
+            if (n > a.burn || a.moments_all) {
 #pragma unroll
                 for (int k = 0; k < K; ++k)
 #pragma unroll
@@ -792,6 +805,8 @@ hmc_run_kernel(const RunArgs a) {
                         comp_add(msq[k][j], csq[k][j], xx);
                         csq[k][j] = add(csq[k][j], fmaf(x, x, -xx));      // the rounding error of x*x itself (exact)
                     }
+            }
+            if (n > a.burn) {
                 if (my_samples && (n - a.burn) % thin == 0) {
                     float* dst = my_samples + (size_t)((n - a.burn) / thin) * ld;
 #pragma unroll
@@ -820,7 +835,7 @@ hmc_run_kernel(const RunArgs a) {
                     const double* T = a.table + 5 * (size_t)n;               // t = n+1
                     const double alpha = bad ? 0.0 : (double)expf(rho);      // min(1, exp(rho)), rho <= 0
                     h_bar = __dadd_rn(__dmul_rn(T[0], h_bar), __dmul_rn(T[1], a.delta - alpha));
-                    const double x_new = a.mu - __dmul_rn(T[2], h_bar);
+                    const double x_new = (SINK ? mu_sink : a.mu) - __dmul_rn(T[2], h_bar);
                     e = expf((float)x_new);
                     const float xb = add((float)__dmul_rn(T[3], x_new), mul((float)T[4], logf((float)eps_bar)));
                     eps_bar = (double)expf(xb);
@@ -1265,6 +1280,9 @@ int elem_hmc_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmc
         if (ld > 4096 || (tuning != 0 && tuning != 1)) return HMCX_ERR_UNSUPPORTED;
         a.thin = sink->thin; a.msum = sink->sum; a.msumsq = sink->sumsq;
         a.msum_lo = sink->sum_lo; a.msumsq_lo = sink->sumsq_lo;
+        a.moments_all = sink->moments_all;
+        if (a.nuts && nuts->mu_chain) { a.mu_per_chain = 1; a.mu_chain = nuts->mu_chain; }
+        a.lp_carry = workspace;                            // windows of a sink run chain bit for bit, as the plain loop's
         pick_geometry(ld, 1, false, E, K, G);
 #define CALLSINK(TK, MK)                                                                                \
         if (G <= 256) hmc_run_kernel<TK, MK, 4, 1, 256, true><<<C, G, 0, st>>>(a);                      \

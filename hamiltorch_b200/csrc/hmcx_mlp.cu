@@ -1034,6 +1034,9 @@ struct MlpRunArgs {
     float* msumsq;
     float* msum_lo;               // optional compensation terms (true sum = hi + lo)
     float* msumsq_lo;
+    // mass adaptation (ABI v11), SINK only: moments over every iteration of the launch; per-chain mu (may be null)
+    int moments_all;
+    const double* mu_chain;
 };
 
 // One sink accumulator [C, ld] (sum, or sum of squares when `squares`) += the float4 x at element offset `off`, read and
@@ -1093,6 +1096,10 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
     float eps = a.eps[c];
     double h_bar = 0.0, eps_bar = 1.0;
     if (a.nuts && tid == 0) { h_bar = a.h_bar[c]; eps_bar = a.eps_bar[c]; }
+    double mu_sink = 0.0;                                      // SINK: this chain's mu (the restarted dual averaging's)
+    if constexpr (SINK) {
+        if (a.nuts && tid == 0) mu_sink = a.mu_chain ? a.mu_chain[c] : a.mu;
+    }
     int rejected = 0;
     const int keep = SINK ? 1 + (a.S - a.burn - 1) / a.thin : a.S - a.burn;      // slots per chain in samples_out
     float* const my_samples = (a.samples && (SINK || lead)) ? a.samples + (size_t)c * keep * a.ld : nullptr;
@@ -1419,6 +1426,8 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
             if (n > a.burn)
                 sink_row((my_samples && (n - a.burn) % a.thin == 0) ? my_samples + (size_t)((n - a.burn) / a.thin) * a.ld
                                                                     : nullptr, true);
+            else if (a.moments_all)
+                sink_row(nullptr, true);                                   // a warm-up window's moments
         } else if (n > a.burn && my_samples) {
             float* dst = my_samples + (size_t)(n - a.burn) * a.ld;
             for (int i = tid; i < a.ld; i += MLP_THREADS) dst[i] = i < D ? q[i] : 0.0f;
@@ -1436,7 +1445,7 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
                     const double* T = a.table + 5 * (size_t)n;
                     const double alpha = bad ? 0.0 : (double)expf(rho);
                     h_bar = __dadd_rn(__dmul_rn(T[0], h_bar), __dmul_rn(T[1], a.delta - alpha));
-                    const double x_new = a.mu - __dmul_rn(T[2], h_bar);
+                    const double x_new = (SINK ? mu_sink : a.mu) - __dmul_rn(T[2], h_bar);
                     e = expf((float)x_new);
                     const float xb = add((float)__dmul_rn(T[3], x_new), mul((float)T[4], logf((float)eps_bar)));
                     eps_bar = (double)expf(xb);
@@ -1642,6 +1651,8 @@ int mlp_split_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hm
     if (sink) {
         a.thin = sink->thin; a.msum = sink->sum; a.msumsq = sink->sumsq;
         a.msum_lo = sink->sum_lo; a.msumsq_lo = sink->sumsq_lo;
+        a.moments_all = sink->moments_all;
+        if (nuts && nuts->enabled) a.mu_chain = nuts->mu_chain;
     }
     int rc = fill_mlp(target, a.m);
     if (rc != HMCX_OK) return rc;

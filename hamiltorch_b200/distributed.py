@@ -100,6 +100,10 @@ def sample_chains_sharded(log_prob_func, params_init, gather_samples=False, runn
     With ``diagnostics=True``, ``diagnostics`` holds split-R-hat / ESS / MCSE over all chains of all ranks
     (``pooled_diagnostics`` of each rank's samples; needs the samples on the GPU) -- split-R-hat, not the
     rank-normalised R-hat of ``diagnostics.rank_summary``, whose global ranks need every rank's draws.
+    With ``adapt_mass=True`` every warm-up window's per-chain moment sums are gathered in global chain order
+    (``all_gather_rows``, one (C, ld) gather per sum) before the pooled estimate, so every rank adapts the same mass from
+    all C chains -- with Philox keyed by the global chain id the samples do not depend on the sharding.  ``inv_mass``
+    then holds the adapted (D,) mass.
     ``runner`` replaces ``samplers.sample_chains`` and ``diagnostics_partials`` the diagnostics' CUDA stages (used by
     the CPU tests of this host logic).
     """
@@ -117,11 +121,15 @@ def sample_chains_sharded(log_prob_func, params_init, gather_samples=False, runn
                 raise RuntimeError('%s must be (S, C=%d, ...), got %s' % (name, C, tuple(kw[name].shape)))
             kw[name] = kw[name][:, lo:hi]
     kw['chain_offset'] = kw.get('chain_offset', 0) + lo
+    if kw.get('adapt_mass'):
+        kw['mass_pool'] = lambda t: all_gather_rows(t, C)
     run = runner if runner is not None else samplers.sample_chains
     local = run(log_prob_func, params_init[lo:hi], **kw)
     out = {'bounds': (lo, hi), 'local': local,
            'num_rejected': all_gather_rows(local.num_rejected, C),
            'step_size': all_gather_rows(local.step_size, C)}
+    if kw.get('adapt_mass'):
+        out['inv_mass'] = local.inv_mass
     if gather_samples:
         blk = local.samples_padded
         if not blk.is_cuda and dist.is_initialized() and dist.get_backend() == 'nccl':

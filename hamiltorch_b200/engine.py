@@ -261,6 +261,58 @@ def nuts_table_device(burn, device):
     return t
 
 
+def mass_windows(burn):
+    """The slow windows of diagonal-mass adaptation over warm-up iterations 0 .. burn-1 as a list of (a, b) iteration ranges,
+    with Stan's windowed-adaptation defaults: an initial buffer of 75 iterations, slow windows of 25 iterations doubling,
+    a terminal buffer of 50.  A window is stretched to end at burn - 50 when the window after it (twice as long) would
+    cross into the terminal buffer, i.e. end past burn - 50 (Stan's compute_next_window, whose inclusive last index
+    makes its `>=` this `>`; the first window is never stretched).  When 75 + 25 + 50 > burn the buffers are
+    int(0.15 * burn) and int(0.1 * burn) and the one window is what remains.  burn = 1000: [75, 100), [100, 150),
+    [150, 250), [250, 450), [450, 950)."""
+    burn = int(burn)
+    if burn < 20:
+        raise RuntimeError('adapt_mass needs burn >= 20 (got %d)' % burn)
+    init, first, term = 75, 25, 50
+    if init + first + term > burn:
+        init, term = int(0.15 * burn), int(0.1 * burn)
+        first = burn - init - term
+    end = burn - term
+    windows = []
+    a, size = init, first
+    b = a + size
+    while True:
+        windows.append((a, b))
+        if b >= end:
+            return windows
+        a, size = b, 2 * size
+        b = a + size
+        if b + 2 * size > end:
+            b = end
+
+
+def nuts_table_restarted(burn):
+    """nuts_table() with the dual averaging restarted at the end of every mass-adaptation window (mass_windows(burn)): the
+    row of iteration n >= b, b the last window end <= n, holds the constants for t = n - b + 1."""
+    ends = [b for _, b in mass_windows(burn)]
+    rows, start = [], 0
+    for n in range(burn + 1):
+        if n in ends:
+            start = n
+        rows.append(n - start)                   # nuts_table()'s row n holds t = n + 1
+    return nuts_table(burn)[rows]
+
+
+def nuts_table_restarted_device(burn, device):
+    """nuts_table_restarted() on the device, built and uploaded once per (burn, device) like nuts_table_device."""
+    key = ('restarted', int(burn), str(torch.device(device)))
+    t = _NUTS_TABLES.get(key)
+    if t is None:
+        if len(_NUTS_TABLES) > 16:
+            _NUTS_TABLES.clear()
+        t = _NUTS_TABLES[key] = nuts_table_restarted(burn).to(device)
+    return t
+
+
 def nuts_mu(step_size_init):
     """samplers.py:664 -- fp32 log of fp32(10*eps0), returned as a Python float."""
     return float(torch.log(10 * torch.FloatTensor([step_size_init])))
@@ -407,7 +459,8 @@ class HMCResult:
 def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, burn=0, inv_mass=None,
             nuts=False, desired_accept_rate=0.8, seed=0, chain_offset=0, normals=None, log_uniforms=None,
             record_ham=False, out=None, device=None, tuning=0, eps_schedule=None, record_eps=False, scheme=None,
-            perms=None, thin=1, moments=False, keep_samples=True, host_samples=False, host_windows=0):
+            perms=None, thin=1, moments=False, keep_samples=True, host_samples=False, host_windows=0, adapt_mass=False,
+            mass_pool=None):
     """The reference's sample() loop for sampler in {HMC, HMC_NUTS} as one persistent kernel over C chains.
 
     params_init (C, D) | (D,).  Randomness: in-kernel Philox keyed by (seed, chain_offset+c, iteration), or -- when
@@ -425,6 +478,13 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
     samples at all, ``host_samples=True`` makes the kernel stream the retained rows straight into pinned host memory
     (the reference's ``store_on_GPU=False``, samplers.py:1008-1012) -- ``result.samples`` is then a CPU tensor, valid
     after a stream synchronisation.
+    ``adapt_mass`` (NUTS, sink-capable target, inv_mass None or 1-D): adapt one diagonal inv_mass shared by all chains
+    during warm-up (DESIGN §3.13).  Each window of mass_windows(burn) is a sink launch accumulating the chains' moments,
+    followed by hmcx_adapt_diag_mass, which pools them into the mass the next launch reads and restarts the dual averaging;
+    the last launch runs the rest of the warm-up and the sampling phase with the sink options above.  All on the current
+    stream, no host synchronisation.  ``result.inv_mass`` (D,), ``result.inv_mass_trace`` (K, D), ``result.mass_windows``.
+    ``mass_pool``: callable mapping each (C_local, ld) window sum to the (C, ld) sum of all chains in global order
+    (distributed.sample_chains_sharded passes an all-gather), so that every rank pools every chain into the same mass.
     """
     N.require_cuda()
     lib = N.load_library()
@@ -456,6 +516,11 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
             host_out, out = out, None
         else:
             host_samples = True                    # caller-provided pinned sample block: the kernel streams into it
+    if adapt_mass:
+        if not nuts:
+            raise RuntimeError('adapt_mass re-tunes the step size after each mass update: it needs NUTS (dual averaging)')
+        if nm.kind == N.MASS_FULL or host_out is not None:
+            raise NotImplementedError('adapt_mass: inv_mass None or 1-D, no windowed copy-engine delivery')
     use_sink = thin > 1 or moments or not keep_samples or host_samples
     keep = 1 + (S - burn - 1) // thin
     if not keep_samples:
@@ -503,7 +568,7 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
     if not torch.is_tensor(step_size):
         nuts_s.step_size_init = float(step_size)           # the double the reference divides in its split drifts
     if nuts:
-        table = nuts_table_device(burn, device)
+        table = nuts_table_restarted_device(burn, device) if adapt_mass else nuts_table_device(burn, device)
         h_bar = torch.zeros(Cn, dtype=torch.float64, device=device)
         eps_bar = torch.ones(Cn, dtype=torch.float64, device=device)
         nuts_s.enabled = 1
@@ -528,8 +593,16 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
             msum, msq, msum_lo, msq_lo = (torch.zeros((Cn, ld), dtype=torch.float32, device=device) for _ in range(4))
             sink.sum, sink.sumsq = msum.data_ptr(), msq.data_ptr()
             sink.sum_lo, sink.sumsq_lo = msum_lo.data_ptr(), msq_lo.data_ptr()
+    mass_out = None
     with torch.cuda.device(device):
-        if scheme is None:
+        if adapt_mass:
+            if sink is None:
+                sink = N.SinkStruct()
+                sink.thin = 1
+            mass_out = _adapted_launches(lib, nt, nm, rng, nuts_s, scheme, q_init, q_cur, eps, Cn, D, ld, L, S, burn,
+                                         samples, accepted, diverged, ham, num_rejected, int(tuning), sink, h_bar,
+                                         eps_bar, mass_pool, device, keep_alive)
+        elif scheme is None:
             ws_bytes = lib.hmcx_hmc_workspace_bytes(nt.ref(), nm.ref(), Cn, ld)
             ws = torch.empty(ws_bytes // 4, dtype=torch.float32, device=device) if ws_bytes else None
             if use_sink:
@@ -589,8 +662,89 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
     res.final_state = q_cur[:, :D]
     if nuts:
         res.eps_bar, res.h_bar = eps_bar, h_bar
+    if mass_out is not None:
+        res.inv_mass_trace, res.mass_windows = mass_out
+        res.inv_mass = res.inv_mass_trace[-1]
     res._keep_alive = keep_alive          # buffers the asynchronous kernel still reads
     return res
+
+
+def _window_rng(rng, it0, Cn, ld, num_splits):
+    """The random-stream struct of a launch starting at iteration it0: injected streams are indexed from the launch's first
+    iteration, so their pointers move to row it0."""
+    if rng.mode != N.RNG_INJECTED or it0 == 0:
+        return rng
+    r = N.RngStruct.from_buffer_copy(rng)
+    r.normals = rng.normals + it0 * Cn * ld * 4
+    r.log_uniforms = rng.log_uniforms + it0 * Cn * 4
+    if rng.perms:
+        r.perms = rng.perms + it0 * Cn * num_splits * 4
+    return r
+
+
+def _adapted_launches(lib, nt, nm, rng, nuts_s, scheme, q_init, q_cur, eps, Cn, D, ld, L, S, burn, samples, accepted,
+                      diverged, ham, num_rejected, tuning, sink, h_bar, eps_bar, mass_pool, device, keep_alive):
+    """hmc_run with adapt_mass: [0, a_1) and every window [a_k, b_k) of mass_windows(burn), each window followed by
+    hmcx_adapt_diag_mass, then [b_K, S) with the caller's sink.  Every launch is a sink launch (mu_chain and moments_all
+    are read by the sink forms only); the launches chain through q_cur, eps, the dual-averaging state and, for element-wise
+    targets, the log p workspace.  Returns (inv_mass_trace (K, D), windows)."""
+    windows = mass_windows(burn)
+    K = len(windows)
+    trace = torch.zeros((K, ld), dtype=torch.float32, device=device)          # row k: inv_mass after window k
+    factor = torch.zeros((K, ld), dtype=torch.float32, device=device)         # row k: its sqrt(1 / inv_mass)
+    acc = [torch.zeros((Cn, ld), dtype=torch.float32, device=device) for _ in range(4)]
+    mu_chain = torch.zeros(Cn, dtype=torch.float64, device=device)
+    wsink = N.SinkStruct()
+    wsink.thin = sink.thin
+    wsink.sum, wsink.sumsq, wsink.sum_lo, wsink.sumsq_lo = (t.data_ptr() for t in acc)
+    wsink.moments_all = 1
+    masses = []
+    for k in range(K):
+        m = N.MassStruct()
+        m.kind, m.inv_mass, m.mass_factor = N.MASS_DIAG, trace[k].data_ptr(), factor[k].data_ptr()
+        masses.append(m)
+    keep_alive += [trace, factor, mu_chain, wsink, masses] + acc
+    ws = None
+    if scheme is None:
+        ws_bytes = lib.hmcx_hmc_workspace_bytes(nt.ref(), nm.ref(), Cn, ld)
+        ws = torch.empty(ws_bytes // 4, dtype=torch.float32, device=device) if ws_bytes else None
+        keep_alive.append(ws)
+    stream = N.stream_ptr(device)
+
+    def launch(it0, it1, mass_ref, sink_s, per_chain_mu):
+        nuts_s.mu_chain = mu_chain.data_ptr() if per_chain_mu else None
+        r = _window_rng(rng, it0, Cn, ld, nt.num_splits)
+        keep_alive.append(r)
+        if scheme is None:
+            rc = lib.hmcx_hmc_run_sink(nt.ref(), mass_ref, C.byref(r), C.byref(nuts_s), N.ptr(q_init), N.ptr(q_cur),
+                                       N.ptr(eps), Cn, ld, L, S, burn, it0, it1, N.ptr(samples), N.ptr(accepted),
+                                       N.ptr(diverged), N.ptr(ham), N.ptr(num_rejected), tuning, N.ptr(ws),
+                                       C.byref(sink_s), stream)
+            N.check(rc, 'hmcx_hmc_run_sink')
+        else:
+            rc = lib.hmcx_split_run_sink(nt.ref(), mass_ref, C.byref(r), C.byref(nuts_s), int(scheme), N.ptr(q_init),
+                                         N.ptr(q_cur), N.ptr(eps), Cn, ld, L, S, burn, it0, it1, N.ptr(samples),
+                                         N.ptr(accepted), N.ptr(diverged), N.ptr(ham), N.ptr(num_rejected),
+                                         C.byref(sink_s), stream)
+            N.check(rc, 'hmcx_split_run_sink')
+
+    mass_ref = nm.ref()
+    launch(0, windows[0][0], mass_ref, sink, False)
+    for k, (a, b) in enumerate(windows):
+        launch(a, b, mass_ref, wsink, k > 0)
+        sums = acc if mass_pool is None else [mass_pool(t).contiguous() for t in acc]
+        if mass_pool is not None:
+            keep_alive.extend(sums)
+        rc = lib.hmcx_adapt_diag_mass(*(N.ptr(t) for t in sums), sums[0].shape[0], ld, D, b - a, N.ptr(eps), Cn,
+                                      N.ptr(trace[k]), N.ptr(factor[k]), N.ptr(mu_chain), N.ptr(h_bar), N.ptr(eps_bar),
+                                      stream)
+        N.check(rc, 'hmcx_adapt_diag_mass')
+        if mass_pool is not None:                  # the kernel zeroed the gathered copies; the next window starts from zero
+            for t in acc:
+                t.zero_()
+        mass_ref = C.byref(masses[k])
+    launch(windows[-1][1], S, mass_ref, sink, True)
+    return trace[:, :D], windows
 
 
 def grad_log_prob(target, q, split=-1, want_grad=True, want_log_prob=True, device=None):

@@ -324,7 +324,7 @@ def sample_chains(log_prob_func, params_init, num_samples=10, num_steps_per_samp
                   sampler=Sampler.HMC, integrator=Integrator.IMPLICIT, metric=Metric.HESSIAN,
                   desired_accept_rate=0.8, rng='philox', seed=0, chain_offset=0, normals=None, log_uniforms=None,
                   record_ham=False, out=None, perms=None, uniforms=None, thin=1, moments=False, keep_samples=True,
-                  store_on_GPU=True, host_windows=0):
+                  store_on_GPU=True, host_windows=0, adapt_mass=False, mass_pool=None):
     """The engine's native entry: C independent chains at once.  ``params_init`` is (C, D); every chain gets the
     reference's ``sample`` semantics.  Returns an ``engine.HMCResult`` whose ``.samples`` is (C, S-burn, D) on the
     GPU (row c = what ``sample`` would have returned for chain c, stacked).
@@ -345,11 +345,24 @@ def sample_chains(log_prob_func, params_init, num_samples=10, num_steps_per_samp
     ``out=<pinned host block>, host_windows=W`` (W >= 2) delivers into the caller's block through the copy engine instead:
     the run is cut into W windows of iterations and each window's sample slots go to the host on a second stream while the
     next window computes (costs a device staging block).
+
+    ``adapt_mass=True`` adapts one diagonal ``inv_mass`` shared by all chains during warm-up, with Stan's windowed
+    schedule (``engine.mass_windows(burn)``): the draws of every chain in a window are pooled into the variance estimate
+    of each dimension (regularised as Stan does), and the step-size dual averaging restarts after each update.  Needs
+    ``sampler=Sampler.HMC_NUTS`` and ``burn >= 20`` (``RuntimeError``) and a combination with a sample sink: GaussianIso /
+    GaussianDiag with D <= 4096, an MLPRegression, or a list of them with a SPLITTING integrator; ``inv_mass`` None or
+    1-D (the initial metric); no ``host_windows`` (``NotImplementedError`` otherwise).  ``thin`` / ``moments`` /
+    ``keep_samples`` / ``store_on_GPU`` apply to the sampling phase.  The result gains ``.inv_mass`` (D,) fp32 -- the
+    mass used after warm-up --, ``.inv_mass_trace`` (K, D), one row per window, and ``.mass_windows``, the K (a, b)
+    iteration ranges.  ``mass_pool`` (multi-GPU; ``distributed.sample_chains_sharded`` passes it) maps each (C_local, ld)
+    window sum to the sum of all chains in global order, so that every rank adapts the same mass.
     """
     if params_init.dim() != 2:
         raise RuntimeError('sample_chains: params_init must be (num_chains, D)')
     _check_sample_args(True, num_samples, burn, sampler)
     _require_target(log_prob_func)
+    if adapt_mass:
+        _check_adapt_mass(log_prob_func, sampler, integrator, inv_mass, burn, host_windows)
     return _run_chains(log_prob_func, params_init, num_samples, num_steps_per_sample, step_size, burn, jitter,
                        inv_mass, softabs_const, explicit_binding_const, fixed_point_threshold,
                        fixed_point_max_iterations, jitter_max_tries, sampler, integrator, metric,
@@ -357,7 +370,23 @@ def sample_chains(log_prob_func, params_init, num_samples=10, num_steps_per_samp
                        log_uniforms=log_uniforms, record_ham=record_ham, out=out, injected_perms=perms,
                        injected_uniforms=uniforms,
                        sink=dict(thin=thin, moments=moments, keep_samples=keep_samples, host_samples=not store_on_GPU,
-                                 host_windows=host_windows))
+                                 host_windows=host_windows, **(dict(adapt_mass=True, mass_pool=mass_pool)
+                                                               if adapt_mass else {})))
+
+
+def _check_adapt_mass(log_prob_func, sampler, integrator, inv_mass, burn, host_windows):
+    """sample_chains(adapt_mass=True) refusals, raised before any CUDA work."""
+    if not _sink_supported(log_prob_func, sampler, integrator, inv_mass) or \
+            (isinstance(log_prob_func, (T.GaussianIso, T.GaussianDiag)) and N.padded_ld(log_prob_func.dim) > 4096):
+        raise NotImplementedError('adapt_mass: GaussianIso / GaussianDiag with D <= 4096, an MLPRegression or a list of them '
+                                  'with a SPLITTING integrator, and inv_mass None or 1-D')
+    if sampler != Sampler.HMC_NUTS:
+        raise RuntimeError('adapt_mass needs sampler=Sampler.HMC_NUTS: the step size is re-tuned after each mass update')
+    if burn < 20:
+        raise RuntimeError('adapt_mass needs burn >= 20 (got %d)' % burn)
+    if int(host_windows) >= 2:
+        raise NotImplementedError('adapt_mass with host_windows: windowed copy-engine delivery is not combined with '
+                                  'mass adaptation')
 
 
 def _run_chains(log_prob_func, q0, num_samples, L, step_size, burn, jitter, inv_mass, softabs_const,

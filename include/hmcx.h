@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define HMCX_ABI_VERSION 10
+#define HMCX_ABI_VERSION 11
 
 #define HMCX_MLP_TC_AUTO 0
 #define HMCX_MLP_TC_OFF  1
@@ -152,6 +152,11 @@ typedef struct hmcx_nuts {
                                        while a chain's fp32 step size still equals (float)step_size_init the drift
                                        coefficient is (float)(step_size_init / K); an adapted step size is an fp32
                                        value in the reference too (:668) and is divided as such.                   */
+    const double* mu_chain;         /* optional [C] (ABI v11): per-chain mu replacing the scalar `mu`, written by
+                                       hmcx_adapt_diag_mass when the dual averaging restarts after a mass update.
+                                       Read by the sink forms only (hmcx_hmc_run_sink / hmcx_split_run_sink with a
+                                       sink; a thin = 1 sink without sums still selects the sink form when mu_chain is
+                                       set); hmcx_hmc_run and hmcx_split_run return HMCX_ERR_UNSUPPORTED for it   */
 } hmcx_nuts_t;
 
 int         hmcx_abi_version(void);
@@ -393,11 +398,15 @@ typedef struct hmcx_sink {
     float*  sumsq;
     float*  sum_lo;
     float*  sumsq_lo;
+    int32_t moments_all;            /* ABI v11: non-zero = accumulate sum / sumsq over EVERY iteration of the launch
+                                       (warm-up included) instead of n > burn only: the moments of a mass-adaptation
+                                       window (hmcx_adapt_diag_mass).  0 (a zero-initialised struct): as before   */
 } hmcx_sink_t;
 
-/* hmcx_hmc_run with a sample sink (sink == NULL or {1, NULL, NULL, NULL, NULL}: identical to hmcx_hmc_run).  Element-wise
- * targets (GAUSS_ISO / GAUSS_DIAG, mass none / diagonal, ld <= 4096); other combinations return HMCX_ERR_UNSUPPORTED
- * when the sink asks for thinning or moments. */
+/* hmcx_hmc_run with a sample sink (sink == NULL or {1, NULL, NULL, NULL, NULL} without nuts->mu_chain: identical to
+ * hmcx_hmc_run).  Element-wise targets (GAUSS_ISO / GAUSS_DIAG, mass none / diagonal, ld <= 4096); other combinations
+ * return HMCX_ERR_UNSUPPORTED when the sink asks for thinning or moments.  The workspace carries log p(q_cur) from one
+ * window of iterations to the next as in hmcx_hmc_run (ABI v11; the mass-adaptation windows rely on it). */
 int hmcx_hmc_run_sink(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmcx_rng_t* rng,
                       const hmcx_nuts_t* nuts,
                       const float* q_init, float* q_cur, float* eps,
@@ -419,6 +428,25 @@ int hmcx_split_run_sink(const hmcx_target_t* target, const hmcx_mass_t* mass, co
                         int32_t iter_begin, int32_t iter_end,
                         float* samples_out, uint8_t* accept_out, uint8_t* diverged_out, float* ham_out,
                         int32_t* num_rejected, const hmcx_sink_t* sink, void* stream);
+
+/*
+ * hmcx_adapt_diag_mass (ABI v11): the pooled diagonal mass estimate at the end of a warm-up window (Stan's windowed
+ * adaptation, regularised as Stan does) and the restart of the dual averaging that follows it.  One pass, fixed order, no
+ * atomics.  Inputs: the per-chain compensated sums of a window of n >= 2 draws, [C, ld] each, as a sink launch with
+ * moments_all leaves them (sum, sumsq, sum_lo, sumsq_lo; true sums hi + lo).  Per dimension d < D, in fp64:
+ *   m_c = S1_c / n,   v_c = (S2_c - S1_c * m_c) / (n - 1),   W = (sum_{c = 0..C-1} v_c, in that order) / C,   N = C * n,
+ *   var = (N / (N + 5)) * W + 1e-3 * (5 / (N + 5))
+ * inv_mass[d] = (float)var and mass_factor[d] = sqrtf(1 / inv_mass[d]) in IEEE fp32 (the hmcx_mass_t DIAG pair: bit-equal
+ * to what the Python binding builds from the same inv_mass on the device); lanes D..ld-1 of both are written as 0.  The four sums are
+ * zeroed (all ld lanes) for the next window.  For the C_chains chains whose step size adapts on this device:
+ *   mu_chain[c] = log(10 * eps[c]) (10 * eps in fp32, then the correctly rounded fp32 log), h_bar[c] = 0, eps_bar[c] = 1.
+ * C and C_chains differ when the sums were gathered from several devices (all chains, global order) and this device
+ * restarts its own chains only.  NULL pointers, C < 1, C_chains < 1, n < 2, D < 1, ld < D or ld % 4 != 0:
+ * HMCX_ERR_INVALID_ARG.
+ */
+int hmcx_adapt_diag_mass(float* sum, float* sumsq, float* sum_lo, float* sumsq_lo, int32_t C, int32_t ld, int32_t D,
+                         int32_t n, const float* eps, int32_t C_chains, float* inv_mass, float* mass_factor,
+                         double* mu_chain, double* h_bar, double* eps_bar, void* stream);
 
 /*
  * hmcx_copy_rows_async: `height` rows of `width` bytes from `src` (row pitch `spitch`) to `dst` (row pitch `dpitch`), either
