@@ -705,14 +705,28 @@ dense_kick_elem_kernel(const DenseArgs a, const float* __restrict__ Q, float* __
 // sample() loop with a full (2-D) inv_mass at D > 16 (samplers.py:199, :294, :812): every drift, the momentum
 // refresh and both kinetic energies are (chains x D) . (D x D) GEMMs on the tensor cores (dense_lin_kernel); a GaussianFull
 // target adds the gradient GEMM, GaussianIso / GaussianDiag kick element-wise.  2L+4 (L+3) GEMMs per iteration.
-// K / N padding to multiples of 32 (one K chunk); column-tile width = the widest of 128/64/32 that divides Dp and still
-// gives the GPU ~100 CTAs (each CTA re-streams its 128 chain rows)
-static void dense_geometry(DenseArgs& a) {
+// Column-tile width of the dense GEMMs over `mt` 128-row tiles and Dp (a multiple of 32) columns: the widest of 128/64/32
+// that divides Dp and still gives the GPU ~100 CTAs (each CTA re-streams its 128 chain rows).  HMCX_DENSE_BN (tests only)
+// forces the width so that every instantiation is reachable at small batches; it is read on every call, and a value that
+// is not 32/64/128 dividing Dp gives 0 (the run returns HMCX_ERR_INVALID_ARG rather than run a width nobody asked for).
+static int dense_tile_width(int Dp, int mt) {
+    if (const char* e = getenv("HMCX_DENSE_BN")) {
+        char* end = nullptr;
+        const long bn = strtol(e, &end, 10);
+        return (end != e && *end == '\0' && (bn == 32 || bn == 64 || bn == 128) && Dp % bn == 0) ? (int)bn : 0;
+    }
+    int bn = (Dp % 128 == 0) ? 128 : (Dp % 64 == 0) ? 64 : 32;
+    while (bn > 32 && mt * (Dp / bn) < 96) bn >>= 1;
+    return bn;
+}
+
+// K / N padding to multiples of 32 (one K chunk); false: HMCX_DENSE_BN forces a width that does not fit
+static bool dense_geometry(DenseArgs& a) {
     a.Dp = (a.D + 31) / 32 * 32;
-    const int mt = a.Cp / 128;
-    a.BN = (a.Dp % 128 == 0) ? 128 : (a.Dp % 64 == 0) ? 64 : 32;
-    while (a.BN > 32 && mt * (a.Dp / a.BN) < 96) a.BN >>= 1;
+    a.BN = dense_tile_width(a.Dp, a.Cp / 128);
+    if (!a.BN) return false;
     a.NT = a.Dp / a.BN;
+    return true;
 }
 
 static inline float mul_host(float x, float y) { volatile float r = x * y; return r; }
@@ -728,7 +742,7 @@ static int dense_fullmass_hmc_run(const hmcx_target_t* target, const hmcx_mass_t
     DenseArgs& a = r.a;
     a.C = C; a.D = D; a.Cp = (C + 127) / 128 * 128;
     a.log_norm = target->log_norm; a.mk = HMCX_MASS_FULL; a.tk = tk;
-    dense_geometry(a);
+    if (!dense_geometry(a)) return HMCX_ERR_INVALID_ARG;
     const size_t CD = (size_t)a.Cp * a.Dp, DD = (size_t)a.Dp * a.Dp;
     float* Q = ws;
     float* P = ws + CD;
@@ -855,12 +869,11 @@ int dense_hmc_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hm
                                       accept, diverged, ham, num_rejected, ws, st);
     DenseRun r = {};
     DenseArgs& a = r.a;
-    a.C = C; a.D = D; a.Cp = (C + 127) / 128 * 128; a.Dp = (D + 127) / 128 * 128; a.NT = a.Dp / 128;
+    a.C = C; a.D = D; a.Cp = (C + 127) / 128 * 128; a.Dp = (D + 127) / 128 * 128;
     a.log_norm = target->log_norm; a.mk = mk; a.tk = target->kind;
-    // column-tile width: the widest tile that still gives the GPU ~100 CTAs (each CTA re-streams its 128 chain rows)
     const int mt = a.Cp / 128;
-    a.BN = 128;
-    while (a.BN > 32 && mt * (a.Dp / a.BN) < 96) a.BN >>= 1;
+    a.BN = dense_tile_width(a.Dp, mt);
+    if (!a.BN) return HMCX_ERR_INVALID_ARG;
     a.NT = a.Dp / a.BN;
     // carve the workspace
     const size_t CD = (size_t)a.Cp * a.Dp, DD = (size_t)a.Dp * a.Dp;
@@ -1006,7 +1019,7 @@ int dense_rmhmc_run(const hmcx_target_t* target, const hmcx_rmhmc_t* cfg, const 
     DenseArgs& a = r.a;
     a.C = C; a.D = D; a.Cp = (C + 127) / 128 * 128;
     a.log_norm = target->log_norm; a.mk = HMCX_MASS_FULL; a.tk = tk;
-    dense_geometry(a);
+    if (!dense_geometry(a)) return HMCX_ERR_INVALID_ARG;
     const size_t CD = (size_t)a.Cp * a.Dp, DD = (size_t)a.Dp * a.Dp;
     float* Q = ws;           float* P = ws + CD;          float* Qc = ws + 2 * CD;      float* Pc = ws + 3 * CD;
     float* Qpack = ws + 4 * CD;  float* Ppack = ws + 6 * CD;  float* Qcpack = ws + 8 * CD;  float* Pcpack = ws + 10 * CD;

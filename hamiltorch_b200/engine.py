@@ -863,6 +863,11 @@ def rmhmc_run(target, params_init, num_samples, num_steps_per_sample, step_size,
     q_init = _as_rows(params_init, ld, device)
     Cn = q_init.shape[0]
     q_cur = q_init.clone()
+    if explicit and torch.is_tensor(step_size) and step_size.numel() > 1:
+        s = step_size.detach().reshape(-1)
+        if not bool((s == s[0]).all()):
+            # every kernel applies ONE binding rotation c, s = cos/sin(2 * omega * step_size) (:435-436) to all chains
+            raise NotImplementedError('the explicit RMHMC integrator takes one step size for all chains')
     eps = _eps_vector(step_size, Cn, device)
     samples = torch.empty((Cn, S - burn, ld), dtype=torch.float32, device=device)
     accepted = torch.empty((Cn, S), dtype=torch.uint8, device=device)

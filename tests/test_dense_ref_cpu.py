@@ -1,0 +1,134 @@
+"""CPU: the fp64 per-iteration replay of the dense paths (tests/dense_ref.py), which the wide-tile GPU tests
+(tests/test_dense_tiles_gpu.py) hold the kernels to, is itself checked here.
+
+* It accepts the unmodified reference's chains (the committed fixtures) as if they were kernel output: identical
+  decisions, states and Hamiltonians within FIXTURE_BOUND.
+* It accepts the fp32 oracle's chains at D = 250 (a full target with a full and with a diagonal mass) within
+  ORACLE_BOUND.
+* It rejects the same oracle runs made with one 64-column block of the precision or of inv_mass off by a relative 1e-4
+  (of the order of one missing lo term of a 3xTF32 product, an estimate): the harness catches a one-tile error.
+"""
+import copy
+import os
+
+import numpy as np
+import pytest
+import torch
+
+from hamiltorch_b200 import targets as T
+from oracle import cases as K, hmc_oracle as O, rmhmc_oracle as R
+from tests import dense_ref
+
+GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
+# 2x the largest scaled error max|a - d| / (1 + |d|) measured on the CPU: fixtures 1.2e-6 (the explicit RMHMC states),
+# oracle at D = 250 4.9e-7.  The perturbed runs below measure 1.9e-6 (inv_mass block) and 5.1e-6 (precision block).
+FIXTURE_BOUND = 2.5e-6
+ORACLE_BOUND = 1e-6
+
+
+def _load(name):
+    f = np.load(os.path.join(GOLDEN, name + '.npz'))
+    C = len(f['seeds'])
+    t = lambda k: torch.from_numpy(np.stack([f['%s_%d' % (k, c)] for c in range(C)]))
+    ham = torch.stack([t('ham_old'), t('ham_new')], -1)
+    return f, C, t, ham
+
+
+def _run(model, init, acc, samples, z, logu, ham, eps, L, burn, tag, bound):
+    rep = dense_ref.replay(model, init, acc, samples, z, eps, L, burn)
+    return dense_ref.check(tag, rep, init, samples, acc, ham, logu, burn, ceiling=bound)
+
+
+@pytest.mark.parametrize('name', ['full48_dense', 'full40_fullmass', 'iso40_fullmass_nuts', 'iso40_blockmass'])
+def test_replay_accepts_the_reference_hmc_chains(name):
+    case = K.plain_cases()[name]
+    kw = case['kw']
+    f, C, t, ham = _load(name)
+    S, L, burn = kw['num_samples'], kw['num_steps_per_sample'], kw['burn']
+    init = t('init')
+    z, logu = t('z').transpose(0, 1), t('logu').t()
+    if kw.get('nuts'):
+        eps = t('step_sizes').t().float()                    # teacher-forced: the step size each iteration used
+        # the dual averaging restated in fp64 proposes the reference's next step sizes (eps_bar at n = burn)
+        prop = dense_ref.dual_averaging(ham, burn, kw['step_size'], kw['desired_accept_rate'])
+        np.testing.assert_allclose(prop.numpy(), eps[1:burn + 2].t().numpy(), rtol=2e-6)
+    else:
+        eps = torch.full((C,), kw['step_size'])
+    model = dense_ref.HMC(case['target'], kw.get('inv_mass'))
+    flips = _run(model, init, t('accepted'), t('samples'), z, logu, ham, eps, L, burn, 'cpu_replay/' + name,
+                 FIXTURE_BOUND)
+    assert flips == 0
+
+
+@pytest.mark.parametrize('name', ['rmhmc_exp_hess_full24', 'rmhmc_imp_softabs_diag20'])
+def test_replay_accepts_the_reference_constant_metric_rmhmc_chains(name):
+    case = K.rmhmc_cases()[name]
+    f, C, t, ham = _load(name)
+    D = case['target'].dim
+    init = torch.tensor(case['init'], dtype=torch.float32).expand(C, D).contiguous()
+    model = dense_ref.RMHMC(case['target'], case['metric'] == 'SOFTABS', case['softabs_const'],
+                            explicit=case['integrator'] == 'EXPLICIT', omega=case.get('explicit_binding_const', 100))
+    eps = torch.full((C,), case['step_size'])
+    flips = _run(model, init, t('accepted'), t('samples'), t('z').transpose(0, 1), t('logu').t(), ham, eps,
+                 case['num_steps_per_sample'], case['burn'], 'cpu_replay/' + name, FIXTURE_BOUND)
+    assert flips == 0
+
+
+# ---- the fp32 oracle at D = 250, a shape of the wide-tile GPU tests ------------------------------------------------
+D250, C3, S6, L5 = 250, 3, 6, 5
+EPS3 = torch.tensor([0.22, 0.25, 0.28])          # one step size per chain, as in the GPU tests
+
+
+def _target(D, seed):
+    g = torch.Generator().manual_seed(seed)
+    A = torch.randn(D, D, generator=g, dtype=torch.float64) / D ** 0.5
+    return T.GaussianFull(torch.randn(D, generator=g), cov=A @ A.t() + 0.5 * torch.eye(D, dtype=torch.float64))
+
+
+def _mass(kind, D):
+    g = torch.Generator().manual_seed(7)
+    if kind == 'diag':
+        return 0.5 + torch.rand(D, generator=g)
+    A = torch.randn(D, D, generator=g, dtype=torch.float64) / D ** 0.5
+    return (A @ A.t() + 0.7 * torch.eye(D, dtype=torch.float64)).float()
+
+
+def _oracle(tgt, im):
+    D = tgt.dim
+    outs, inits, zs, lus = [], [], [], []
+    for c in range(C3):
+        init, z, logu, _ = O.reference_stream(300 + c, D, S6, prior=lambda: tgt.mean + 0.3 * torch.randn(D))
+        outs.append(O.sample_hmc(tgt, init, num_samples=S6, num_steps_per_sample=L5, step_size=float(EPS3[c]),
+                                 inv_mass=im, normals=z, log_uniforms=logu))
+        inits.append(init), zs.append(z), lus.append(logu)
+    acc = torch.tensor([o['accepted'] for o in outs])
+    samples = torch.stack([torch.stack(o['samples']) for o in outs])
+    ham = torch.tensor([[o['ham_old'], o['ham_new']] for o in outs], dtype=torch.float64).transpose(1, 2)
+    return torch.stack(inits), acc, samples, torch.stack(zs, 1), torch.stack(lus, 1), ham
+
+
+@pytest.mark.parametrize('mass', ['full', 'diag'])
+def test_replay_accepts_the_oracle_at_d250(mass):
+    tgt, im = _target(D250, 5), _mass(mass, D250)
+    init, acc, samples, z, logu, ham = _oracle(tgt, im)
+    assert 0 < int(acc.sum()) < acc.numel() + 1
+    flips = _run(dense_ref.HMC(tgt, im), init, acc, samples, z, logu, ham, EPS3, L5, 0, 'cpu_replay/d250_' + mass,
+                 ORACLE_BOUND)
+    assert flips == 0
+
+
+@pytest.mark.parametrize('mass,operand', [('full', 'prec'), ('full', 'inv_mass'), ('diag', 'prec')])
+def test_replay_rejects_one_perturbed_64_column_block(mass, operand):
+    tgt, im = _target(D250, 5), _mass(mass, D250)
+    bad_tgt, bad_im = tgt, im
+    if operand == 'prec':
+        bad_tgt = copy.copy(tgt)                 # same log_norm: only the contraction is off
+        bad_tgt.prec = tgt.prec.clone()
+        bad_tgt.prec[:, 64:128] *= 1 + 1e-4
+    else:
+        bad_im = im.clone()
+        bad_im[:, 64:128] *= 1 + 1e-4
+    init, acc, samples, z, logu, ham = _oracle(bad_tgt, bad_im)
+    with pytest.raises(AssertionError, match='tolerance'):
+        _run(dense_ref.HMC(tgt, im), init, acc, samples, z, logu, ham, EPS3, L5, 0,
+             'cpu_replay/d250_%s_bad_%s' % (mass, operand), ORACLE_BOUND)
