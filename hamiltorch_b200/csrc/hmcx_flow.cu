@@ -484,26 +484,45 @@ __global__ void __launch_bounds__(256, 1) flow_small_kernel(const FlowArgs a) {
     }
 }
 
-static int flow_threads_and_grid(int C, int D, size_t matrix_bytes, int& R, int& threads, int& grid) {
-    int sms = 132;
-    int dev = 0;
-    if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+// A test switch (HMCX_FLOW_R / HMCX_FLOW_W): -1 when unset, the value when it is a whole decimal number in [lo, hi], else 0
+static int flow_env(const char* name, long lo, long hi) {
+    const char* e = getenv(name);
+    if (!e) return -1;
+    char* end = nullptr;
+    const long v = strtol(e, &end, 10);
+    return (end != e && *end == '\0' && v >= lo && v <= hi) ? (int)v : 0;
+}
+
+// Launch geometry: R chains per warp, w = threads / 32 warps per CTA, `grid` CTAs and `smem` bytes of dynamic shared memory
+// (the nmat transposed K4 x DP matrices, then two staging rows of DP floats per chain of every warp).  HMCX_FLOW_R = 1|2|4
+// forces R and HMCX_FLOW_W = 1..8 caps w (tests and tuning: every instantiation reachable at any batch); both are read on
+// every call.  Any other value of either, or a geometry whose shared memory exceeds the device's opt-in limit, is
+// HMCX_ERR_INVALID_ARG: the run never launches a geometry nobody asked for, nor one that cannot launch.
+// tests/test_flow_geometry_cpu.py restates this rule and checks it against the constants below.
+static int flow_geometry(int C, int nmat, int K4, int DP, int& R, int& threads, int& grid, size_t& smem) {
+    int dev = 0, sms = 0, optin = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+        cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev) != cudaSuccess) {
+        cudaGetLastError();
+        return HMCX_ERR_CUDA;
+    }
+    const int fr = flow_env("HMCX_FLOW_R", 1, 4), fw = flow_env("HMCX_FLOW_W", 1, 8);
+    if (fr == 0 || fr == 3 || fw == 0) return HMCX_ERR_INVALID_ARG;
     // chains per warp: every warp-matvec streams the whole matrix from shared memory once, so more chains per warp = less
     // shared-memory traffic per chain, fewer chains per warp = more warps (SMs) working on a small batch
-    const char* fr = getenv("HMCX_FLOW_R");
-    if (fr && (atoi(fr) == 1 || atoi(fr) == 2 || atoi(fr) == 4)) R = atoi(fr);
-    else R = (C <= 4 * sms) ? 1 : (C <= 12 * sms) ? 2 : 4;
+    R = fr > 0 ? fr : (C <= 4 * sms) ? 1 : (C <= 12 * sms) ? 2 : 4;
     const int warps = (C + R - 1) / R;
     int w = (warps + sms - 1) / sms;
     // big batches: when two CTAs' matrices fit one SM, CTAs of 4 warps (finer waves, the same warps per SM); D = 128 with
     // three matrices fills the SM with one CTA of 8
-    const int wmax = (const char*)getenv("HMCX_FLOW_W") ? atoi(getenv("HMCX_FLOW_W")) : (matrix_bytes <= 100 * 1024 ? 4 : 8);
+    const size_t matrix_bytes = (size_t)nmat * K4 * DP * sizeof(float);
+    const int wmax = fw > 0 ? fw : (matrix_bytes <= 100 * 1024 ? 4 : 8);
     if (w > wmax) w = wmax;
     if (w < 1) w = 1;
     threads = 32 * w;
     grid = (warps + w - 1) / w;
-    (void)D;
-    return 0;
+    smem = ((size_t)nmat * K4 * DP + (size_t)w * 2 * R * DP) * sizeof(float);
+    return smem <= (size_t)optin ? HMCX_OK : HMCX_ERR_INVALID_ARG;
 }
 
 template <int NJ>
@@ -524,9 +543,9 @@ static int flow_launch_nj(const FlowArgs& a, int R, int threads, int grid, size_
 static int flow_launch(const FlowArgs& a, cudaStream_t st) {
     const int NJ = (a.D + 31) / 32, DP = NJ * 32, K4 = (a.D + 3) & ~3;
     int R, threads, grid;
+    size_t smem;
     const int nmat = (a.tk == HMCX_TARGET_GAUSS_FULL ? 1 : 0) + (a.mk == HMCX_MASS_FULL ? 2 : 0);
-    flow_threads_and_grid(a.C, a.D, (size_t)nmat * K4 * DP * sizeof(float), R, threads, grid);
-    const size_t smem = ((size_t)nmat * K4 * DP + (size_t)(threads / 32) * 2 * R * DP) * sizeof(float);
+    if (const int rc = flow_geometry(a.C, nmat, K4, DP, R, threads, grid, smem)) return rc;
     switch (NJ) {
         case 1: return flow_launch_nj<1>(a, R, threads, grid, smem, st);
         case 2: return flow_launch_nj<2>(a, R, threads, grid, smem, st);
