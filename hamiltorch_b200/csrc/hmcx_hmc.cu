@@ -58,6 +58,12 @@ __device__ __forceinline__ float grad1(float q, float mean, float ivar) {
     if (TK == HMCX_TARGET_GAUSS_ISO) return -q;
     return -mul(ivar, sub(q, mean));
 }
+// -grad1, exactly
+template <int TK>
+__device__ __forceinline__ float neg_grad1(float q, float mean, float ivar) {
+    if (TK == HMCX_TARGET_GAUSS_ISO) return q;
+    return mul(ivar, sub(q, mean));
+}
 // summand of -2*(log p - log_norm)
 template <int TK>
 __device__ __forceinline__ float uterm1(float q, float mean, float ivar) {
@@ -148,10 +154,12 @@ __device__ __forceinline__ void trajectory_groups(float (*q)[E], float (*p)[E], 
 #pragma unroll 1
     for (; l + 2 <= L; l += 2) { one_step(); one_step(); }
     if (l < L) one_step();
+    // p - half*g as p + half*(-g): half*(-g) == -(half*g) and p - (-y) == p + y in round-to-nearest, bit for bit.  With
+    // -g the compiler materialised the negation of every element where the odd and even step counts join (8 FADDs).
 #pragma unroll
     for (int g = 0; g < NG; ++g)
 #pragma unroll
-        for (int j = 0; j < E; ++j) p[g][j] = sub(p[g][j], mul(half, grad1<TK>(q[g][j], c[g].mean[j], c[g].ivar[j])));
+        for (int j = 0; j < E; ++j) p[g][j] = add(p[g][j], mul(half, neg_grad1<TK>(q[g][j], c[g].mean[j], c[g].ivar[j])));
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -461,12 +469,10 @@ __device__ __forceinline__ void hmc_produce(const RunArgs& a, int pt, int G, uin
         }
 #pragma unroll
         for (int u = 0; u < NT; ++u) {
-            const int tt = pt + 32 * PW * u;
-            if (tt < G) {
-                r.p[0][tt] = pv[u][0];
-                r.p[1][tt] = pv[u][1];
-                if ((lane & 15) == 0) r.kin[(tt >> 5) + (lane >> 4) * nwarp] = kin[u][0];
-            }
+            const int tt = pt + 32 * PW * u;            // < 32 * PW * NT = MAXT = G: every mirrored thread exists
+            r.p[0][tt] = pv[u][0];
+            r.p[1][tt] = pv[u][1];
+            if ((lane & 15) == 0) r.kin[(tt >> 5) + (lane >> 4) * nwarp] = kin[u][0];
         }
         if (pt == 0) r.logu = logu;
         bar_arrive(BAR_SLOT_FULL, nthr);
@@ -506,7 +512,9 @@ hmc_run_kernel(const RunArgs a) {
     __shared__ float s_eps[2];
     __shared__ MomentumSlot s_slot;                        // PW > 0 only (unreferenced, and dropped, otherwise)
 
-    const int c = blockIdx.x / CS, rank = blockIdx.x % CS, G = blockDim.x - 32 * PW;
+    // the producer form always runs MAXT compute threads (elem_hmc_run): a compile-time G makes its barrier counts, warp
+    // count and slot offsets immediates instead of values re-derived from blockDim on every iteration
+    const int c = blockIdx.x / CS, rank = blockIdx.x % CS, G = PW > 0 ? MAXT : blockDim.x - 32 * PW;
     const int tid = threadIdx.x, gt = rank * G + tid;       // thread index within the CTA / within the chain
     const bool lead = tid == 0 && rank == 0;                // writes the chain's scalar outputs
     const bool nuts = NUTS && a.nuts;
@@ -1305,7 +1313,7 @@ int elem_hmc_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmc
     const bool pair = tuning == 0 && K == 2 && G <= 128 && pair_ok;
     // the producer form's CTAs have 1.5x the threads and ~1.5x the registers per thread: it runs while every chain's CTA
     // finds an SM beside at most one other, and the plain paired form above that (measured at 512 chains, DESIGN §3.1)
-    const bool producers = pair && C <= 2 * sm_count();
+    const bool producers = pair && G == 128 && C <= 2 * sm_count();     // G is 128 whenever 768 < ld <= 1024
 #define CALL(TK, MK)                                                                                    \
     if (producers) hmc_run_kernel<TK, MK, 4, 2, 128, false, true, 1, false, 2><<<C, G + 64, 0, st>>>(a);  \
     else if (pair) hmc_run_kernel<TK, MK, 4, 2, 128, false, true, 1, false><<<C, G, 0, st>>>(a);        \
