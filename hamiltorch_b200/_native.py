@@ -15,7 +15,7 @@ LIB_PATH = os.path.join(_HERE, 'lib', 'libhmcx.so')
 OK, ERR_INVALID_ARG, ERR_UNSUPPORTED, ERR_CUDA = 0, -1, -2, -3
 MASS_NONE, MASS_DIAG, MASS_FULL = 0, 1, 2
 RNG_INJECTED, RNG_PHILOX = 0, 1
-ABI_VERSION = 11
+ABI_VERSION = 12
 
 
 class NativeError(RuntimeError):
@@ -144,6 +144,11 @@ _PROTOS = {
                                        C.c_void_p, C.c_void_p]),
     'hmcx_rank_indicator': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                       C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
+    'hmcx_mlp_pointwise_ll': (C.c_int, [C.POINTER(TargetStruct), C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32,
+                                        C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
+    'hmcx_loo_workspace_bytes': (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
+    'hmcx_loo_pass': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
 DIAG_LAG_BLOCK = 32                     # HMCX_DIAG_LAG_BLOCK: lags per hmcx_diag_acov pass

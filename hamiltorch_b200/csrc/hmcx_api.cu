@@ -1,4 +1,5 @@
 // hmcx_api.cu -- the extern "C" surface declared in include/hmcx.h; validates and dispatches on target kind.
+#include <cfloat>
 #include <cstdlib>
 #include "hmcx_common.cuh"
 
@@ -51,6 +52,11 @@ int rank_indicator(const float*, long long, long long, int, int, int, const doub
                    cudaStream_t);
 int adapt_diag_mass(float*, float*, float*, float*, int, int, int, int, const float*, int, float*, float*, double*, double*,
                     double*, cudaStream_t);
+int mlp_pointwise_ll(const hmcx_target_t*, const float*, long long, long long, int, int, int, int, float*, long long,
+                     long long, cudaStream_t);
+size_t loo_workspace_bytes(int, int, int);
+int loo_pass(const float*, long long, long long, int, int, int, int, int, double, double*, int*, int*, void*,
+             cudaStream_t);
 }  // namespace hmcx
 
 static inline bool has_mu_chain(const hmcx_nuts_t* nuts) { return nuts && nuts->enabled && nuts->mu_chain; }
@@ -324,6 +330,35 @@ int hmcx_rank_indicator(const float* x, int64_t chain_stride, int64_t draw_strid
         return HMCX_ERR_INVALID_ARG;
     return hmcx::rank_indicator(x, chain_stride, draw_stride, C, n, D, thr, out, out_chain_stride, out_draw_stride,
                                 (cudaStream_t)stream);
+}
+
+int hmcx_mlp_pointwise_ll(const hmcx_target_t* target, const float* samples, int64_t chain_stride, int64_t draw_stride,
+                          int32_t C, int32_t n, int32_t row_begin, int32_t row_end, float* ll_out,
+                          int64_t ll_chain_stride, int64_t ll_draw_stride, void* stream) {
+    if (!target) return HMCX_ERR_INVALID_ARG;
+    if (target->kind != HMCX_TARGET_MLP) return HMCX_ERR_UNSUPPORTED;
+    return hmcx::mlp_pointwise_ll(target, samples, chain_stride, draw_stride, C, n, row_begin, row_end, ll_out,
+                                  ll_chain_stride, ll_draw_stride, (cudaStream_t)stream);
+}
+
+static inline bool loo_shape_ok(int32_t C, int32_t n) {
+    return C >= 1 && n >= 1 && (int64_t)C * n >= 2 && (int64_t)C * n <= HMCX_RANK_MAX_DRAWS;
+}
+
+size_t hmcx_loo_workspace_bytes(int32_t C, int32_t n, int32_t k) {
+    if (!loo_shape_ok(C, n) || !rank_slab_ok(k)) return 0;
+    return hmcx::loo_workspace_bytes(C, n, k);
+}
+
+int hmcx_loo_pass(const float* ll, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t N,
+                  int32_t i0, int32_t k, double r_eff, double* pointwise, int32_t* tail_size, int32_t* nonfinite,
+                  void* workspace, size_t workspace_bytes, void* stream) {
+    if (!ll || !pointwise || !tail_size || !nonfinite || !workspace || chain_stride < 0 || draw_stride < 0 ||
+        !loo_shape_ok(C, n) || N < 1 || i0 < 0 || !rank_slab_ok(k) || (int64_t)i0 + k > N || !(r_eff > 0.0) ||
+        !(r_eff <= DBL_MAX) || workspace_bytes < hmcx::loo_workspace_bytes(C, n, k))
+        return HMCX_ERR_INVALID_ARG;
+    return hmcx::loo_pass(ll, chain_stride, draw_stride, C, n, N, i0, k, r_eff, pointwise, tail_size, nonfinite,
+                          workspace, (cudaStream_t)stream);
 }
 
 int hmcx_adapt_diag_mass(float* sum, float* sumsq, float* sum_lo, float* sumsq_lo, int32_t C, int32_t ld, int32_t D,

@@ -1,0 +1,188 @@
+// hmcx_loo.cu -- Pareto-smoothed importance-sampling leave-one-out (PSIS-LOO, Vehtari, Gelman & Gabry 2017; Vehtari,
+// Simpson, Gelman, Yao & Gabry 2024) and WAIC per data point, from a pointwise log-likelihood block.
+// hamiltorch_b200/loo.py drives it; tests/loo_oracle.py is the numpy definition.
+//
+// The block is fp32 ll[c, s, i] at ll + c*chain_stride + s*draw_stride + i: C chains of n draws, S = C*n pooled draws per
+// data point i.  A call handles a slab of k points [i0, i0 + k):
+//   1-2. the key build and segmented radix sort of hmcx_rank.cu (rank_sort), segments = points: every point's S draws in
+//        ascending ll order, i.e. descending r = -ll;
+//   3.   one CTA per point, in fp64: the tail cut, the Zhang & Stephens (2009) generalised-Pareto fit, the smoothed
+//        log-ratios and the LOO / WAIC terms.  Every draw-sum is a thread-strided loop over the sorted draws followed by a
+//        fixed shuffle tree and a fixed in-order sum over warps; there are no atomics, so the outputs depend on the block
+//        alone (not on k or the launch geometry) and the same block gives the same bits.
+// The smoothed tail needs no draw index: each term of every sum is a function of the sorted position only.
+#include <cfloat>
+#include "hmcx_common.cuh"
+
+namespace hmcx {
+
+size_t rank_sort_workspace_bytes(int C, int n, int k);
+int rank_sort(const float* x, long long cs, long long ds, int C, int n, int d0, int k, int* nonfinite, void* ws,
+              const uint32_t** sorted_keys, cudaStream_t st);
+
+namespace {
+
+constexpr int LT = 256;                     // threads per point
+constexpr int LW = LT / 32;
+
+__device__ __forceinline__ double ll_of_key(uint32_t k) {
+    return (double)__uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+
+// Fixed-order CTA sum / max of one double per thread; every thread gets the result.  The xor tree leaves the same bits
+// in every lane (each level adds the same two operands), the warp partials are summed in warp order.
+__device__ __forceinline__ double cta_sum(double v, double* sh) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
+    __syncthreads();
+    double s = sh[0];
+#pragma unroll
+    for (int w = 1; w < LW; ++w) s += sh[w];
+    __syncthreads();
+    return s;
+}
+
+__device__ __forceinline__ double cta_max(double v, double* sh) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
+    if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
+    __syncthreads();
+    double s = sh[0];
+#pragma unroll
+    for (int w = 1; w < LW; ++w) s = fmax(s, sh[w]);
+    __syncthreads();
+    return s;
+}
+
+// One point per CTA.  keys: the slab's sorted keys, S per point.  M = ceil(min(0.2 S, 3 sqrt(S / r_eff))) (host).
+// out[row * N + i], rows: 0 elpd_loo, 1 p_loo, 2 pareto_k, 3 lppd, 4 p_waic, 5 elpd_waic; tail[i] = M'.
+// Dynamic shared memory: 30 + floor(sqrt(M)) doubles (the L_j of the fit).
+__global__ void __launch_bounds__(LT) loo_point_kernel(const uint32_t* __restrict__ keys, int S, int M, int N, int i0,
+                                                       const int* __restrict__ nonfinite, double* __restrict__ out,
+                                                       int* __restrict__ tail) {
+    extern __shared__ double sL[];
+    __shared__ double sh[LW];
+    const int j = blockIdx.x, i = i0 + j, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint32_t* kp = keys + (long long)j * S;
+    if (nonfinite[i]) {
+        if (tid == 0) {
+            const double nan = __longlong_as_double(0x7ff8000000000000LL);
+            for (int r = 0; r < 6; ++r) out[(long long)r * N + i] = nan;
+            tail[i] = 0;
+        }
+        return;
+    }
+    auto llv = [&](int p) { return ll_of_key(kp[p]); };
+    const double rmax = -llv(0);
+    auto rr = [&](int p) { return -llv(p) - rmax; };           // shifted log-ratio, non-increasing in p, rr(0) = 0
+    // 3-4. cutoff = the (M+1)-th largest r, floored; the tail is {r > cutoff} = sorted positions [0, Mt)
+    const double c = fmax(rr(M), log(DBL_MIN));
+    int lo = 0, hi = M;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (rr(mid) > c) lo = mid + 1; else hi = mid;
+    }
+    const int Mt = lo;
+    const double ec = exp(c);
+    auto xt = [&](int t) { return exp(rr(Mt - t)) - ec; };     // ascending exceedances, t = 1..Mt
+    // 5. generalised-Pareto fit (Zhang & Stephens 2009, with the weakly informative prior of Vehtari et al.)
+    double khat = __longlong_as_double(0x7ff0000000000000LL), sigma = 0.0;
+    if (Mt > 4) {
+        const int m = 30 + (int)floor(sqrt((double)Mt));
+        const double x_max = xt(Mt), x_q = xt((int)floor(Mt / 4.0 + 0.5));
+        auto b_of = [&](int jj) { return 1.0 / x_max + (1.0 - sqrt(m / (jj - 0.5))) / (3.0 * x_q); };
+        for (int jj = 1 + warp; jj <= m; jj += LW) {            // a warp per j: lane-strided sum, xor tree
+            const double b = b_of(jj);
+            double s = 0.0;
+            for (int t = 1 + lane; t <= Mt; t += 32) s += log1p(-b * xt(t));
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+            const double k = s / Mt;
+            if (lane == 0) sL[jj - 1] = Mt * (log(-b / k) - k - 1.0);
+        }
+        __syncthreads();
+        double wsum = 0.0, wbsum = 0.0;
+        for (int jj = 1 + tid; jj <= m; jj += LT) {
+            const double Lj = sL[jj - 1];
+            double d = 0.0;
+            for (int l = 0; l < m; ++l) d += exp(sL[l] - Lj);
+            const double w = 1.0 / d;
+            if (w >= 10.0 * DBL_EPSILON) { wsum += w; wbsum += w * b_of(jj); }
+        }
+        const double bbar = cta_sum(wbsum, sh) / cta_sum(wsum, sh);
+        double s = 0.0;
+        for (int t = 1 + tid; t <= Mt; t += LT) s += log1p(-bbar * xt(t));
+        const double xi = cta_sum(s, sh) / Mt;
+        sigma = -xi / bbar;
+        khat = (Mt * xi + 5.0) / (Mt + 10.0);
+    }
+    const bool smooth = Mt > 4 && isfinite(khat);
+    // 6. log-ratios: the tail (ascending z = Mt - p) replaced by the GPD quantiles, then capped at 0 (the largest raw one)
+    auto lw = [&](int p) {
+        double v;
+        if (smooth && p < Mt) {
+            const double pz = (Mt - p - 0.5) / Mt;
+            const double q = khat == 0.0 ? -sigma * log1p(-pz) : sigma * expm1(-khat * log1p(-pz)) / khat;
+            v = log(q + ec);
+        } else {
+            v = rr(p);
+        }
+        return v > 0.0 ? 0.0 : v;
+    };
+    double mx = -DBL_MAX;
+    for (int p = tid; p < S; p += LT) mx = fmax(mx, lw(p));
+    mx = cta_max(mx, sh);
+    double s = 0.0;
+    for (int p = tid; p < S; p += LT) s += exp(lw(p) - mx);
+    const double lse_w = mx + log(cta_sum(s, sh));
+    // 7. elpd_loo = logsumexp(lw + ll), lw normalised
+    mx = -DBL_MAX;
+    for (int p = tid; p < S; p += LT) mx = fmax(mx, (lw(p) - lse_w) + llv(p));
+    mx = cta_max(mx, sh);
+    s = 0.0;
+    for (int p = tid; p < S; p += LT) s += exp(((lw(p) - lse_w) + llv(p)) - mx);
+    const double elpd = mx + log(cta_sum(s, sh));
+    // lppd = logsumexp(ll) - log S (the largest ll is the last sorted draw); p_waic = var(ll), ddof 1
+    const double llmax = llv(S - 1);
+    double se = 0.0, sm = 0.0;
+    for (int p = tid; p < S; p += LT) { const double v = llv(p); se += exp(v - llmax); sm += v; }
+    const double lppd = (llmax + log(cta_sum(se, sh))) - log((double)S);
+    const double mean = cta_sum(sm, sh) / S;
+    double sv = 0.0;
+    for (int p = tid; p < S; p += LT) { const double d = llv(p) - mean; sv += d * d; }
+    const double pw = cta_sum(sv, sh) / (S - 1);
+    if (tid == 0) {
+        out[i] = elpd;
+        out[(long long)N + i] = lppd - elpd;
+        out[2LL * N + i] = khat;
+        out[3LL * N + i] = lppd;
+        out[4LL * N + i] = pw;
+        out[5LL * N + i] = lppd - pw;
+        tail[i] = Mt;
+    }
+}
+
+}  // namespace
+
+int loo_tail_cap(int S, double r_eff) {
+    return (int)ceil(fmin(0.2 * S, 3.0 * sqrt(S / r_eff)));
+}
+
+size_t loo_workspace_bytes(int C, int n, int k) { return rank_sort_workspace_bytes(C, n, k); }
+
+int loo_pass(const float* ll, long long cs, long long ds, int C, int n, int N, int i0, int k, double r_eff, double* out,
+             int* tail, int* nonfinite, void* ws, cudaStream_t st) {
+    const int S = C * n;
+    const uint32_t* keys = nullptr;
+    int rc = rank_sort(ll, cs, ds, C, n, i0, k, nonfinite, ws, &keys, st);
+    if (rc != HMCX_OK) return rc;
+    const int M = loo_tail_cap(S, r_eff);
+    const size_t smem = (size_t)(30 + (int)floor(sqrt((double)M))) * sizeof(double);
+    if (cudaFuncSetAttribute(loo_point_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+        return HMCX_ERR_CUDA;
+    loo_point_kernel<<<k, LT, smem, st>>>(keys, S, M, N, i0, nonfinite, out, tail);
+    return cudaGetLastError() == cudaSuccess ? HMCX_OK : HMCX_ERR_CUDA;
+}
+
+}  // namespace hmcx

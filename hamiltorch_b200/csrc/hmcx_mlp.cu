@@ -1513,6 +1513,89 @@ mlp_predict_kernel(const MlpDev m, const float* __restrict__ samples, int ld, fl
     if (threadIdx.x == 0 && lpout) lpout[blockIdx.x] = lp;
 }
 
+// Pointwise log-likelihood of the rows [r_begin, r_end) of a forwarded tile (rows r0 .. r0 + cnt - 1), one thread per row:
+//   regression   ll_const + c_ll * sum_o (f_o - y_o)^2       (c_ll = -0.5 tau_out, ll_const = 0.5 O log(tau_out / 2 pi))
+//   binary       -sum_o BCEWithLogits(f_o, y_o) in torch's stable form
+//   multi-class  log_softmax(f)[y];  LogSoftmax output: f[y], the same value of the logits
+// tau_out tempers the classification likelihoods during sampling only; it does not enter these densities.
+__device__ __forceinline__ void mlp_ll_rows(const MlpDev& m, const float* out, const float* ytile, int r0, int cnt,
+                                            int r_begin, int r_end, float ll_const, float* llrow) {
+    const int nL = m.n[m.L];
+    for (int r = threadIdx.x; r < cnt; r += MLP_THREADS) {
+        const int i = r0 + r;
+        if (i < r_begin || i >= r_end) continue;
+        const float* z = out + r * nL;
+        float v = 0.0f;
+        if (m.loss == HMCX_LOSS_REGRESSION || m.loss == HMCX_LOSS_BINARY) {
+            for (int o = 0; o < nL; ++o) {
+                const float yv = ytile ? ytile[r * nL + o] : __ldg(m.y + (size_t)i * nL + o), f = z[o];
+                if (m.loss == HMCX_LOSS_REGRESSION) {
+                    const float d = f - yv;
+                    v += d * d;
+                } else {
+                    v -= (1.0f - yv) * f + fmaxf(-f, 0.0f) + log1pf(expf(-fabsf(f)));
+                }
+            }
+            if (m.loss == HMCX_LOSS_REGRESSION) v = ll_const + (-0.5f * m.tau_out) * v;
+        } else {
+            // both multi-class losses: the tile holds the logits (a LogSoftmax output layer is applied here, as in the
+            // loss stage), so f[y] of a LogSoftmax network is log_softmax(logits)[y]
+            int label = (int)(ytile ? ytile[r] : __ldg(m.y + i));
+            label = label < 0 ? 0 : (label >= nL ? nL - 1 : label);
+            float mx = z[0];
+            for (int k = 1; k < nL; ++k) mx = fmaxf(mx, z[k]);
+            float se = 0.0f;
+            for (int k = 0; k < nL; ++k) se += expf(z[k] - mx);
+            v = (z[label] - mx) - logf(se);
+        }
+        llrow[i] = v;
+    }
+}
+
+// ll[c, s, i - r_begin] = log p(y_i | theta_{c,s}) for the rows [r_begin, r_end): one CTA per draw, the tiles of the
+// target's own data (x, y and the packed tensor-core operands) read in place; tiles that straddle the slab's edges are
+// forwarded whole and only their rows inside it written.  The network outputs never leave shared memory.
+__global__ void __launch_bounds__(MLP_THREADS, 1)
+mlp_ll_kernel(const MlpDev m, const float* __restrict__ samples, long long cs, long long ds, int n, int r_begin,
+              int r_end, float ll_const, float* __restrict__ ll, long long lcs, long long lds) {
+    extern __shared__ __align__(128) float sm[];
+    __shared__ __align__(8) uint64_t s_bars[3];
+    float* q = sm;
+    float* tile = sm + m.tile_base;
+    const int c = blockIdx.x / n, s = blockIdx.x - c * n;
+    const float* qin = samples + (long long)c * cs + (long long)s * ds;
+    for (int i = threadIdx.x; i < m.Dp; i += MLP_THREADS) q[i] = i < m.D ? qin[i] : 0.0f;
+    __syncthreads();
+    float* llrow = ll + (long long)c * lcs + (long long)s * lds - r_begin;
+    TcCtx tc = {};
+    TcEpi te;
+    if (m.tc) {
+        tc_init(tc, s_bars);
+        tc_epi_begin(m, q, te);
+        fence_async_smem();
+        __syncthreads();
+    }
+    for (int sp = 0; sp < m.M; ++sp) {
+        if (m.sb[sp + 1] <= r_begin || m.sb[sp] >= r_end) continue;
+        int ti = 0;
+        for (int r0 = m.sb[sp]; r0 < m.sb[sp + 1] && r0 < r_end; r0 += m.T, ++ti) {
+            if (r0 + m.T <= r_begin) continue;
+            const int cnt = min(m.T, m.sb[sp + 1] - r0);
+            if (m.tc) {
+                float act[16];
+                tc_prefetch_fwd(m, tile, tc, m.tb[sp] + ti, 0);
+                tc_prefetch_y(m, tile, r0, cnt);
+                tc_forward_tile(m, q, tile, tc, te, act, 0);
+            } else {
+                mlp_forward_tile(m, q, tile, r0, cnt);
+            }
+            mlp_ll_rows(m, tile + m.aoff[m.L], m.tc ? tile + m.tc_yraw : nullptr, r0, cnt, r_begin, r_end, ll_const,
+                        llrow);
+            __syncthreads();
+        }
+    }
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------
@@ -1746,6 +1829,24 @@ int mlp_predict(const hmcx_target_t* target, const float* samples, int S, int ld
     rc = prepare_smem(mlp_predict_kernel, smem);
     if (rc != HMCX_OK) return rc;
     mlp_predict_kernel<<<S, MLP_THREADS, smem, st>>>(m, samples, ld, pred_out, log_prob_out);
+    return cuda_status();
+}
+
+int mlp_pointwise_ll(const hmcx_target_t* target, const float* samples, long long cs, long long ds, int C, int n,
+                     int r_begin, int r_end, float* ll, long long lcs, long long lds, cudaStream_t st) {
+    MlpDev m = {};
+    int rc = fill_mlp(target, m);
+    if (rc != HMCX_OK) return rc;
+    if (!samples || !ll || C < 1 || n < 1 || (long long)C * n > 0x7fffffffLL || cs < 0 || ds < 0 || lcs < 0 || lds < 0 ||
+        !m.has_data || r_begin < 0 || r_end > m.N || r_begin >= r_end)
+        return HMCX_ERR_INVALID_ARG;
+    if (!mlp_pick_tile(m, 1, target->mlp->tensor_cores != HMCX_MLP_TC_OFF)) return HMCX_ERR_UNSUPPORTED;
+    const size_t smem = (size_t)(m.tile_base + m.tile_floats) * sizeof(float);
+    rc = prepare_smem(mlp_ll_kernel, smem);
+    if (rc != HMCX_OK) return rc;
+    const double tau = (double)target->mlp->tau_out;
+    const float ll_const = (float)(0.5 * m.n[m.L] * log(tau / (2.0 * 3.14159265358979323846)));
+    mlp_ll_kernel<<<C * n, MLP_THREADS, smem, st>>>(m, samples, cs, ds, n, r_begin, r_end, ll_const, ll, lcs, lds);
     return cuda_status();
 }
 

@@ -393,6 +393,26 @@ RankWs carve(void* base, int L, int k) {
     return RankWs{(uint32_t*)p[0], (uint32_t*)p[1], (uint32_t*)p[5], (int*)p[2], (int*)p[3], (int*)p[4], (int*)p[6]};
 }
 
+// Stages 1-2 on a slab of k segments: nonfinite[d0, d0 + k) cleared then flagged, the keys built into (ka, ia) and
+// sorted by four LSD passes that ping-pong through (kb, ib); the sorted keys and flat indices end back in (ka, ia).
+int sort_slab(const float* x, long long cs, long long ds, int n, int L, int d0, int k, int* nonfinite, uint32_t* ka,
+              uint32_t* kb, int* ia, int* ib, uint32_t* cnt, cudaStream_t st) {
+    const int nt = (L + TILE - 1) / TILE;
+    if (cudaMemsetAsync(nonfinite + d0, 0, (size_t)k * sizeof(int), st) != cudaSuccess) return HMCX_ERR_CUDA;
+    rank_keys_kernel<<<dim3((L + 31) / 32, (k + 31) / 32), dim3(32, 8), 0, st>>>(x, cs, ds, n, L, d0, k, ka, ia,
+                                                                                 nonfinite);
+    uint32_t *ki = ka, *ko = kb;
+    int *ii = ia, *io = ib;
+    for (int shift = 0; shift < 32; shift += 8) {
+        radix_hist_kernel<<<dim3(nt, k), RT, 0, st>>>(ki, L, nt, shift, cnt);
+        seg_scan_kernel<<<k, SCAN_T, 0, st>>>(cnt, 256 * nt);
+        radix_scatter_kernel<<<dim3(nt, k), RT, 0, st>>>(ki, ii, ko, io, L, nt, shift, cnt);
+        uint32_t* tk = ki; ki = ko; ko = tk;
+        int* ti = ii; ii = io; io = ti;
+    }
+    return HMCX_OK;
+}
+
 }  // namespace
 
 size_t rank_workspace_bytes(int C, int n, int k) {
@@ -402,23 +422,40 @@ size_t rank_workspace_bytes(int C, int n, int k) {
     return b;
 }
 
+// The sort alone (stages 1-2) for the PSIS pass of hmcx_loo.cu: keys and indices twice plus the digit counts -- the
+// pieces 0-3 and 5 of ws_sizes, carved in that order.
+size_t rank_sort_workspace_bytes(int C, int n, int k) {
+    size_t sz[7];
+    ws_sizes(C * n, k, sz);
+    return sz[0] + sz[1] + sz[2] + sz[3] + sz[5];
+}
+
+int rank_sort(const float* x, long long cs, long long ds, int C, int n, int d0, int k, int* nonfinite, void* ws,
+              const uint32_t** sorted_keys, cudaStream_t st) {
+    const int L = C * n;
+    size_t sz[7];
+    ws_sizes(L, k, sz);
+    char* p = (char*)ws;
+    uint32_t* ka = (uint32_t*)p;
+    uint32_t* kb = (uint32_t*)(p += sz[0]);
+    int* ia = (int*)(p += sz[1]);
+    int* ib = (int*)(p += sz[2]);
+    uint32_t* cnt = (uint32_t*)(p += sz[3]);
+    *sorted_keys = ka;
+    const int rc = sort_slab(x, cs, ds, n, L, d0, k, nonfinite, ka, kb, ia, ib, cnt, st);
+    if (rc != HMCX_OK) return rc;
+    return cudaGetLastError() == cudaSuccess ? HMCX_OK : HMCX_ERR_CUDA;
+}
+
 int rank_pass(const float* x, long long cs, long long ds, int C, int n, int D, int d0, int k, float* bz, long long bcs,
               long long bds, float* fz, long long fcs, long long fds, double* q, int* nonfinite, void* ws,
               cudaStream_t st) {
     const int L = C * n, nt = (L + TILE - 1) / TILE;
     const RankWs w = carve(ws, L, k);
-    if (cudaMemsetAsync(nonfinite + d0, 0, (size_t)k * sizeof(int), st) != cudaSuccess) return HMCX_ERR_CUDA;
-    rank_keys_kernel<<<dim3((L + 31) / 32, (k + 31) / 32), dim3(32, 8), 0, st>>>(x, cs, ds, n, L, d0, k, w.ka, w.ia,
-                                                                                 nonfinite);
-    uint32_t *ki = w.ka, *ko = w.kb;
-    int *ii = w.ia, *io = w.ib;
-    for (int shift = 0; shift < 32; shift += 8) {
-        radix_hist_kernel<<<dim3(nt, k), RT, 0, st>>>(ki, L, nt, shift, w.cnt);
-        seg_scan_kernel<<<k, SCAN_T, 0, st>>>(w.cnt, 256 * nt);
-        radix_scatter_kernel<<<dim3(nt, k), RT, 0, st>>>(ki, ii, ko, io, L, nt, shift, w.cnt);
-        uint32_t* tk = ki; ki = ko; ko = tk;
-        int* ti = ii; ii = io; io = ti;
-    }
+    const int rc = sort_slab(x, cs, ds, n, L, d0, k, nonfinite, w.ka, w.kb, w.ia, w.ib, w.cnt, st);
+    if (rc != HMCX_OK) return rc;
+    uint32_t* ki = w.ka;
+    int* ii = w.ia;
     // four passes: the sorted keys and indices are back in (ka, ia)
     kept_count_kernel<<<dim3(nt, k), RT, 0, st>>>(ii, L, n, nt, w.cnt);
     seg_scan_kernel<<<k, SCAN_T, 0, st>>>(w.cnt, nt);

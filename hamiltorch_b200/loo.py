@@ -1,0 +1,291 @@
+"""Model comparison for Bayesian NNs on the GPU: Pareto-smoothed importance-sampling leave-one-out cross-validation
+(PSIS-LOO; Vehtari, Gelman & Gabry 2017, Vehtari, Simpson, Gelman, Yao & Gabry 2024) and WAIC -- what Stan's ``loo``,
+ArviZ's ``az.loo`` / ``az.waic`` and PyMC report, restated in numpy fp64 by tests/loo_oracle.py.
+
+    ll = hamiltorch_b200.loo.pointwise_log_lik(res, target)     # (C, n, N) fp32: log p(y_i | theta_{c,s})
+    lo = hamiltorch_b200.loo.psis_loo(res, target)              # or psis_loo(ll)
+    lo.elpd_loo, lo.se, lo.pareto_k.max(), lo.num_bad_k
+    hamiltorch_b200.loo.compare(lo_a, lo_b)                     # elpd differences to the best model
+
+``target`` is the ``MLPTarget`` of ``define_model_log_prob`` or the list ``define_split_model_log_prob`` returns (data
+points in split order).  Two CUDA passes:
+  * hmcx_mlp_pointwise_ll: one CTA per draw runs the network over the target's own device data (the SIMT tiles, or the
+    3xTF32 tensor-core forward of n0 -> 128 -> nL stacks) and writes one log-likelihood per data row; the network outputs
+    never reach device memory.  Regression: the normalised Gaussian density with noise precision ``tau_out``.
+    Classification: the categorical / Bernoulli density of the network's logits -- ``tau_out`` tempers these
+    likelihoods while sampling but is NOT part of the predictive density LOO and WAIC score.
+  * hmcx_loo_pass: per data point, the segmented radix sort of rank_summary over the S = C*n pooled draws, then one fp64
+    pass: tail cut, Zhang & Stephens generalised-Pareto fit, smoothed importance weights, LOO and WAIC terms.
+Samples plus a target are processed in slabs of data points, so the (S, N) log-likelihood block is never held whole:
+each slab's block and sort workspace fit in ``diagnostics.RANK_WORKSPACE_BUDGET`` bytes (at least one point per slab).
+"""
+import ctypes as C
+import math
+
+import torch
+
+from . import _native as N
+from . import diagnostics as _diag
+from . import targets as T
+
+_slab_points_override = None            # tests: force this many data points per slab
+_ROW_TILE = 128                         # slab boundaries of the likelihood pass: whole tiles of the packed data operand
+_ROWS = ('elpd_loo', 'p_loo', 'pareto_k', 'lppd', 'p_waic', 'elpd_waic')
+
+
+class LooResult:
+    """``psis_loo``: per point (N,) fp64 on the block's device -- ``pointwise`` (elpd_loo_i), ``p_loo_i``,
+    ``pareto_k``, ``lppd``, ``tail_size`` (int32, M'); totals (Python floats) ``elpd_loo``, ``se``, ``p_loo``,
+    ``p_loo_se``, ``looic`` = -2 elpd_loo, ``looic_se``; ``k_threshold`` = min(1 - 1/log10 S, 0.7), ``num_bad_k``
+    (points with pareto_k above it), ``num_nonfinite`` (points with a non-finite draw: NaN outputs, and NaN totals),
+    ``num_points``, ``num_draws``, ``r_eff``."""
+
+    kind = 'loo'
+
+    def __repr__(self):
+        return ('LooResult(elpd_loo=%.3f, se=%.3f, p_loo=%.3f, N=%d, S=%d, bad k-hat=%d, nonfinite=%d)'
+                % (self.elpd_loo, self.se, self.p_loo, self.num_points, self.num_draws, self.num_bad_k,
+                   self.num_nonfinite))
+
+
+class WaicResult:
+    """``waic``: per point (N,) fp64 -- ``pointwise`` (elpd_waic_i), ``p_waic``, ``lppd``; totals ``elpd_waic``,
+    ``se``, ``p_waic_total``, ``p_waic_se``, ``waic`` = -2 elpd_waic, ``waic_se``; ``num_p_waic_warn`` (points with
+    p_waic_i > 0.4), ``num_nonfinite``, ``num_points``, ``num_draws``."""
+
+    kind = 'waic'
+
+    def __repr__(self):
+        return ('WaicResult(elpd_waic=%.3f, se=%.3f, p_waic=%.3f, N=%d, S=%d, p_waic > 0.4: %d, nonfinite=%d)'
+                % (self.elpd_waic, self.se, self.p_waic_total, self.num_points, self.num_draws, self.num_p_waic_warn,
+                   self.num_nonfinite))
+
+
+class Comparison:
+    """``compare``: ``elpd`` per model (input order), ``elpd_diff`` = elpd - elpd of the best model (<= 0, 0 for the
+    best), ``se_diff`` = sqrt(N) sd(pointwise difference to the best, ddof 1) (0 for the best), ``order`` = model
+    indices from best to worst."""
+
+    def __init__(self, elpd, elpd_diff, se_diff, order):
+        self.elpd, self.elpd_diff, self.se_diff, self.order = elpd, elpd_diff, se_diff, order
+
+    def __repr__(self):
+        rows = ['  model %d: elpd %.3f, elpd_diff %.3f, se_diff %.3f' % (i, self.elpd[i], self.elpd_diff[i],
+                                                                         self.se_diff[i]) for i in self.order]
+        return 'Comparison(\n%s)' % '\n'.join(rows)
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# Inputs
+# ------------------------------------------------------------------------------------------------------------------
+def _mlp_target(target):
+    items = target if isinstance(target, list) else [target]
+    if not items or not all(isinstance(t, T.MLPTarget) for t in items):
+        raise TypeError('loo: the target must be an MLPTarget (define_model_log_prob) or the list '
+                        'define_split_model_log_prob returns, got %s' % type(target).__name__)
+    if any(t.x is None for t in items):
+        raise RuntimeError('loo: the target has no data (x is None): there are no points to leave out')
+    return items[0]
+
+
+def _check_r_eff(r_eff):
+    r = float(r_eff)
+    if not (r > 0.0 and math.isfinite(r)):
+        raise ValueError('loo: r_eff must be a finite positive number, got %r' % (r_eff,))
+    return r
+
+
+def _samples_block(samples, target):
+    first = _mlp_target(target)
+    if torch.is_tensor(samples) and samples.dim() in (2, 3) and samples.shape[-1] != first.dim:
+        raise RuntimeError('loo: the samples have %d parameters per draw, the target has %d'
+                           % (samples.shape[-1], first.dim))
+    x = _diag.as_block(samples)
+    if x.shape[2] != first.dim:
+        raise RuntimeError('loo: the samples have %d parameters per draw, the target has %d'
+                           % (x.shape[2], first.dim))
+    return x
+
+
+def _native_target(target, device):
+    from .engine import native_target
+    return native_target(target, device)
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# Pointwise log-likelihood
+# ------------------------------------------------------------------------------------------------------------------
+def _ll_rows(lib, nt, x, r0, r1, out):
+    """out[c, s, :] = ll of rows [r0, r1) (out a (C, n, r1 - r0) view with unit stride along its last dimension)."""
+    C_, n = int(x.shape[0]), int(x.shape[1])
+    rc = lib.hmcx_mlp_pointwise_ll(nt.ref(), N.ptr(x), x.stride(0), x.stride(1), C_, n, r0, r1, N.ptr(out),
+                                   out.stride(0), out.stride(1), N.stream_ptr(x.device))
+    N.check(rc, 'hmcx_mlp_pointwise_ll')
+
+
+def pointwise_log_lik(samples, target):
+    """The (C, n, N) fp32 CUDA tensor ll[c, s, i] = log p(y_i | theta_{c,s}) of every draw and data point.
+
+    ``samples``: what ``diagnostics.summary`` accepts (an ``HMCResult``, a (C, n, D) / (n, D) CUDA fp32 tensor, the list
+    ``sample`` returns), refused in the same cases.  ``target``: an ``MLPTarget`` with data, or the list of split
+    descriptors (points in split order).  Per point, with f the network output (O values) and tau = tau_out:
+    regression sum_o -0.5 tau (f_o - y_o)^2 + 0.5 O log(tau / 2 pi); binary sum_o -BCEWithLogits(f_o, y_o);
+    multi-class log_softmax(f)[y]; LogSoftmax output f[y].  tau_out does not enter the classification densities."""
+    x = _samples_block(samples, target)
+    N.require_cuda()
+    lib = N.load_library()
+    nt = _native_target(target, x.device)
+    Np = int(nt.mlp_struct.num_rows)
+    out = torch.empty((x.shape[0], x.shape[1], Np), dtype=torch.float32, device=x.device)
+    with torch.cuda.device(x.device):
+        _ll_rows(lib, nt, x, 0, Np, out)
+    return out
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# PSIS / WAIC pass
+# ------------------------------------------------------------------------------------------------------------------
+def _slab_points(lib, C_, n, Np, extra_per_point=0):
+    """Points per slab: the sort workspace (and, from samples, the slab's fp32 likelihood block) within the budget."""
+    if _slab_points_override is not None:
+        return max(1, min(Np, N.RANK_MAX_SLAB, int(_slab_points_override)))
+    budget = _diag.RANK_WORKSPACE_BUDGET
+    cost = lambda k: lib.hmcx_loo_workspace_bytes(C_, n, k) + k * extra_per_point
+    k = max(1, min(Np, N.RANK_MAX_SLAB, budget // cost(1)))
+    while k > 1 and cost(k) > budget:
+        k -= 1
+    if extra_per_point and _ROW_TILE <= k < Np:
+        k -= k % _ROW_TILE
+    return k
+
+
+def _pointwise_pass(x, target, r_eff):
+    """(C, n, N) draws -> (pw (6, N) fp64, tail (N,) int32, flag (N,) int32, S, N)."""
+    N.require_cuda()
+    lib = N.load_library()
+    dev = x.device
+    C_, n = int(x.shape[0]), int(x.shape[1])
+    S = C_ * n
+    if S > N.RANK_MAX_DRAWS:
+        raise RuntimeError('loo: %d chains x %d draws exceed the %d draws per point the sort indexes'
+                           % (C_, n, N.RANK_MAX_DRAWS))
+    if target is None:
+        Np = int(x.shape[2])
+        k = _slab_points(lib, C_, n, Np)
+        nt = None
+    else:
+        nt = _native_target(target, dev)
+        Np = int(nt.mlp_struct.num_rows)
+        k = _slab_points(lib, C_, n, Np, extra_per_point=4 * S)
+    pw = torch.empty((6, Np), dtype=torch.float64, device=dev)
+    tail = torch.empty(Np, dtype=torch.int32, device=dev)
+    flag = torch.empty(Np, dtype=torch.int32, device=dev)
+    ws_bytes = lib.hmcx_loo_workspace_bytes(C_, n, k)
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        st = N.stream_ptr(dev)
+        blk = None if nt is None else torch.empty((C_, n, k), dtype=torch.float32, device=dev)
+        for i0 in range(0, Np, k):
+            kk = min(k, Np - i0)
+            if nt is None:
+                src, base = x, N.ptr(x)
+            else:
+                _ll_rows(lib, nt, x, i0, i0 + kk, blk)
+                # the pass reads point i at column i of the block: the slab's block holds columns [i0, i0 + kk)
+                src, base = blk, C.c_void_p(blk.data_ptr() - 4 * i0)
+            rc = lib.hmcx_loo_pass(base, src.stride(0), src.stride(1), C_, n, Np, i0, kk, float(r_eff), N.ptr(pw),
+                                   N.ptr(tail), N.ptr(flag), N.ptr(ws), ws_bytes, st)
+            N.check(rc, 'hmcx_loo_pass')
+        del ws
+    return pw, tail, flag, S, Np
+
+
+def _total(v):
+    """(sum, sqrt(N) * sd(v, ddof 1)) of a per-point fp64 tensor, as Python floats."""
+    n = v.numel()
+    s = float(v.sum())
+    se = float(math.sqrt(n) * v.std(unbiased=True)) if n > 1 else float('nan')
+    return s, se
+
+
+def _prepare(x, target, r_eff=None):
+    if r_eff is not None:
+        r_eff = _check_r_eff(r_eff)
+    if target is None:
+        blk = _diag.as_block(x)
+    else:
+        blk = _samples_block(x, target)
+    return blk, r_eff
+
+
+def psis_loo(x, target=None, r_eff=1.0):
+    """PSIS-LOO of a Bayesian NN on the GPU.
+
+    ``x``: a log-likelihood block ll[c, s, i] -- a (C, n, N) or (n, N) CUDA fp32 tensor, e.g. ``pointwise_log_lik``'s
+    -- or, with ``target``, the samples (read like ``diagnostics.summary`` reads them) whose likelihood is computed slab
+    by slab.  ``r_eff``: the relative efficiency of the draws' importance ratios (1 for independent draws), which sets
+    the tail length M = ceil(min(0.2 S, 3 sqrt(S / r_eff))).  Per point i over its S = C*n pooled draws (fp64):
+    r = -ll shifted to max 0; the tail is the draws with r above the (M+1)-th largest r (ties at the cutoff stay out);
+    with more than 4 tail draws a generalised Pareto distribution is fitted to their exceedances (Zhang & Stephens 2009,
+    with Vehtari et al.'s prior: pareto_k = (M' xi + 5)/(M' + 10)) and their log-ratios replaced by its quantiles,
+    otherwise pareto_k = inf; the log-ratios are capped at 0 and normalised (lw); elpd_loo_i = logsumexp(lw + ll),
+    p_loo_i = lppd_i - elpd_loo_i.  Totals are sums over points, se = sqrt(N) sd(pointwise).  A point with a non-finite
+    draw gets NaN outputs (so the totals are NaN) and is counted in ``num_nonfinite``.  The same block gives the same
+    bits on every call, whatever the slab size.  Returns a ``LooResult``."""
+    blk, r_eff = _prepare(x, target, r_eff)
+    pw, tail, flag, S, Np = _pointwise_pass(blk, target, r_eff)
+    r = LooResult()
+    r.pointwise, r.p_loo_i, r.pareto_k, r.lppd, r.tail_size = pw[0], pw[1], pw[2], pw[3], tail
+    r.elpd_loo, r.se = _total(pw[0])
+    r.p_loo, r.p_loo_se = _total(pw[1])
+    r.looic, r.looic_se = -2.0 * r.elpd_loo, 2.0 * r.se
+    r.k_threshold = min(1.0 - 1.0 / math.log10(S), 0.7)
+    r.num_bad_k = int((pw[2] > r.k_threshold).sum())
+    r.num_nonfinite = int((flag != 0).sum())
+    r.num_points, r.num_draws, r.r_eff = Np, S, r_eff
+    return r
+
+
+def waic(x, target=None):
+    """WAIC of a Bayesian NN on the GPU (Watanabe 2010, in the elpd scale of Vehtari et al. 2017): per point
+    lppd_i = logsumexp(ll) - log S, p_waic_i = var(ll) over the S pooled draws (ddof 1), elpd_waic_i = lppd_i - p_waic_i;
+    totals are sums, se = sqrt(N) sd(pointwise), waic = -2 elpd_waic.  ``x`` / ``target`` as ``psis_loo``.
+    ``num_p_waic_warn`` counts points with p_waic_i > 0.4, where WAIC is known to be unreliable (prefer PSIS-LOO).
+    Returns a ``WaicResult``."""
+    blk, _ = _prepare(x, target)
+    pw, _, flag, S, Np = _pointwise_pass(blk, target, 1.0)
+    r = WaicResult()
+    r.pointwise, r.p_waic, r.lppd = pw[5], pw[4], pw[3]
+    r.elpd_waic, r.se = _total(pw[5])
+    r.p_waic_total, r.p_waic_se = _total(pw[4])
+    r.waic, r.waic_se = -2.0 * r.elpd_waic, 2.0 * r.se
+    r.num_p_waic_warn = int((pw[4] > 0.4).sum())
+    r.num_nonfinite = int((flag != 0).sum())
+    r.num_points, r.num_draws = Np, S
+    return r
+
+
+def compare(*results):
+    """Compare models fitted to the same N data points by their ``psis_loo`` (or ``waic``) results: the elpd
+    differences to the best model and se_diff = sqrt(N) sd(diff_i) of the pointwise differences (ddof 1).  Refuses
+    results of different kinds or different N.  Returns a ``Comparison``."""
+    if len(results) == 1 and isinstance(results[0], (list, tuple)):
+        results = tuple(results[0])
+    if len(results) < 2:
+        raise ValueError('compare: need at least two results')
+    kinds = {getattr(r, 'kind', None) for r in results}
+    if len(kinds) != 1 or kinds.pop() not in ('loo', 'waic'):
+        raise TypeError('compare: pass psis_loo results only or waic results only')
+    n0 = results[0].num_points
+    if any(r.num_points != n0 for r in results):
+        raise RuntimeError('compare: the results score different numbers of data points (%s); models are compared '
+                           'on the same data' % ', '.join(str(r.num_points) for r in results))
+    elpd = [r.elpd_loo if r.kind == 'loo' else r.elpd_waic for r in results]
+    order = sorted(range(len(results)), key=lambda i: -elpd[i])
+    best = results[order[0]].pointwise
+    diff, se = [], []
+    for i, r in enumerate(results):
+        d = r.pointwise - best.to(r.pointwise.device)
+        diff.append(elpd[i] - elpd[order[0]])
+        se.append(0.0 if i == order[0] else _total(d)[1])
+    return Comparison(elpd, diff, se, order)

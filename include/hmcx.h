@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define HMCX_ABI_VERSION 11
+#define HMCX_ABI_VERSION 12
 
 #define HMCX_MLP_TC_AUTO 0
 #define HMCX_MLP_TC_OFF  1
@@ -510,6 +510,44 @@ int hmcx_rank_pass(const float* x, int64_t chain_stride, int64_t draw_stride, in
                    int32_t* nonfinite, void* workspace, size_t workspace_bytes, void* stream);
 int hmcx_rank_indicator(const float* x, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t D,
                         const double* thr, float* out, int64_t out_chain_stride, int64_t out_draw_stride, void* stream);
+
+/*
+ * Model comparison for Bayesian NNs (ABI v12): PSIS-LOO and WAIC (Vehtari, Gelman & Gabry 2017; hamiltorch_b200/loo.py).
+ *   hmcx_mlp_pointwise_ll  ll_out[c, s, i - row_begin] = log p(y_i | theta_{c,s}) for the data rows [row_begin, row_end)
+ *                    of an HMCX_TARGET_MLP target (split targets: rows in split order), draw theta_{c,s} at samples +
+ *                    c*chain_stride + s*draw_stride (unit stride along D).  One CTA per draw runs the forward pass of
+ *                    hmcx_mlp_predict (SIMT tiles, or the tensor-core form when x_packed is set) over the target's own
+ *                    x / y / x_packed in place; the network outputs stay in shared memory.  Per row, f = network output:
+ *                      REGRESSION      sum_o -0.5 tau_out (f_o - y_o)^2 + 0.5 O log(tau_out / 2 pi)
+ *                      BINARY          sum_o -BCEWithLogits(f_o, y_o)
+ *                      MULTICLASS      log_softmax(f)[y]
+ *                      .._LOGSOFTMAX   f[y]
+ *                    tau_out (a tempering of the classification likelihoods while sampling) is not part of the last three.
+ *                    NULL pointers, C < 1, n < 1, C*n > INT32_MAX, negative strides, a target without data or a row range
+ *                    outside [0, num_rows) or empty: HMCX_ERR_INVALID_ARG; other target kinds: HMCX_ERR_UNSUPPORTED.
+ *   hmcx_loo_workspace_bytes  sort workspace a slab of k points needs (0 for invalid arguments).
+ *   hmcx_loo_pass    for the points i in [i0, i0 + k) of an fp32 block ll[c, s, i] (strides as the v9 entries, N points,
+ *                    S = C*n >= 2 pooled draws per point): the segmented radix sort of hmcx_rank_pass, then per point in fp64
+ *                    r = -ll - max(-ll); M = ceil(min(0.2 S, 3 sqrt(S / r_eff))); cutoff = max(the (M+1)-th largest r,
+ *                    log DBL_MIN); tail = {r > cutoff}, M' = its size (tail_size[i]); for M' > 4 the Zhang-Stephens GPD fit
+ *                    of the exceedances exp(r) - exp(cutoff) gives k-hat and sigma, and the tail's log-ratios become
+ *                    log(q_z + exp(cutoff)), q_z the GPD quantile at (z - 1/2)/M'; M' <= 4: k-hat = +inf, no smoothing.
+ *                    Log-ratios capped at 0 and normalised: lw.  pointwise [6, N] fp64, rows:
+ *                      0 elpd_loo = logsumexp(lw + ll)       1 p_loo = lppd - elpd_loo      2 pareto_k = k-hat
+ *                      3 lppd = logsumexp(ll) - log S        4 p_waic = var(ll) (ddof 1)    5 elpd_waic = lppd - p_waic
+ *                    nonfinite [N] int32: 1 where the point has a non-finite draw (its six outputs are NaN).  Fixed-order
+ *                    sums, no atomics: the outputs depend on the block only, not on the slab.  NULL pointers, C < 1,
+ *                    n < 1, S < 2 or > HMCX_RANK_MAX_DRAWS, negative strides, a slab outside [0, N), k >
+ *                    HMCX_RANK_MAX_SLAB, r_eff not in (0, inf) or a workspace smaller than hmcx_loo_workspace_bytes(C, n,
+ *                    k): HMCX_ERR_INVALID_ARG.
+ */
+int hmcx_mlp_pointwise_ll(const hmcx_target_t* target, const float* samples, int64_t chain_stride, int64_t draw_stride,
+                          int32_t C, int32_t n, int32_t row_begin, int32_t row_end, float* ll_out,
+                          int64_t ll_chain_stride, int64_t ll_draw_stride, void* stream);
+size_t hmcx_loo_workspace_bytes(int32_t C, int32_t n, int32_t k);
+int hmcx_loo_pass(const float* ll, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t N,
+                  int32_t i0, int32_t k, double r_eff, double* pointwise, int32_t* tail_size, int32_t* nonfinite,
+                  void* workspace, size_t workspace_bytes, void* stream);
 
 #ifdef __cplusplus
 }
