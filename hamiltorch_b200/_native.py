@@ -68,6 +68,15 @@ class SinkStruct(C.Structure):
                 ('sumsq_lo', C.c_void_p), ('moments_all', C.c_int32)]
 
 
+HYPER_GROUPS = 2 * MLP_MAX_LAYERS + 1
+
+
+class HyperStruct(C.Structure):
+    _fields_ = [('sampled', C.c_int32 * HYPER_GROUPS), ('a', C.c_double * HYPER_GROUPS), ('b', C.c_double * HYPER_GROUPS),
+                ('tau', C.c_void_p), ('tau_out', C.c_void_p), ('tau_trace', C.c_void_p), ('tau_out_trace', C.c_void_p),
+                ('gammas', C.c_void_p)]
+
+
 class NutsStruct(C.Structure):
     _fields_ = [('enabled', C.c_int32), ('desired_accept_rate', C.c_double), ('mu', C.c_double),
                 ('table', C.c_void_p), ('h_bar', C.c_void_p), ('eps_bar', C.c_void_p),
@@ -120,6 +129,13 @@ _PROTOS = {
                                       C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.POINTER(SinkStruct), C.c_void_p]),
+    'hmcx_split_run_hyper': (C.c_int, [C.POINTER(TargetStruct), C.POINTER(MassStruct), C.POINTER(RngStruct),
+                                       C.POINTER(NutsStruct), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.POINTER(SinkStruct), C.POINTER(HyperStruct), C.c_void_p]),
+    'hmcx_hyper_gamma_draws': (C.c_int, [C.c_uint64, C.c_uint64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                         C.POINTER(C.c_double), C.c_void_p, C.c_void_p]),
     'hmcx_gemm_nt_tf32x3': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),
     'hmcx_copy_rows_async': (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p]),
     'hmcx_grad_log_prob': (C.c_int, [C.POINTER(TargetStruct), C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
@@ -146,6 +162,9 @@ _PROTOS = {
                                       C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
     'hmcx_mlp_pointwise_ll': (C.c_int, [C.POINTER(TargetStruct), C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32,
                                         C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
+    'hmcx_mlp_pointwise_ll_tau': (C.c_int, [C.POINTER(TargetStruct), C.c_void_p, C.c_int64, C.c_int64, C.c_int32,
+                                            C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.c_int64,
+                                            C.c_void_p, C.c_int64, C.c_int64, C.c_void_p]),
     'hmcx_loo_workspace_bytes': (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
     'hmcx_loo_pass': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                 C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

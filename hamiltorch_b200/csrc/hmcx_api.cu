@@ -22,7 +22,8 @@ int dense_rmhmc_run(const hmcx_target_t*, const hmcx_rmhmc_t*, const hmcx_const_
                     float*, int32_t*, float*, cudaStream_t);
 int mlp_split_run(const hmcx_target_t*, const hmcx_mass_t*, const hmcx_rng_t*, const hmcx_nuts_t*, int, const float*,
                   float*, float*, int, int, int, int, int, int, int, float*, uint8_t*, uint8_t*, float*, int32_t*,
-                  cudaStream_t, const float*, float*, float*, const hmcx_sink_t*);
+                  cudaStream_t, const float*, float*, float*, const hmcx_sink_t*, const hmcx_hyper_t*);
+int hyper_gamma_draws(uint64_t, uint64_t, int, int, int, int, const double*, double*, cudaStream_t);
 int mlp_leapfrog(const hmcx_target_t*, const hmcx_mass_t*, const hmcx_rng_t*, int, double, const float*, const float*, float*,
                  int, int, int, float*, float*, cudaStream_t);
 int mlp_grad_log_prob(const hmcx_target_t*, const float*, int, int, int, float*, float*, cudaStream_t);
@@ -53,7 +54,7 @@ int rank_indicator(const float*, long long, long long, int, int, int, const doub
 int adapt_diag_mass(float*, float*, float*, float*, int, int, int, int, const float*, int, float*, float*, double*, double*,
                     double*, cudaStream_t);
 int mlp_pointwise_ll(const hmcx_target_t*, const float*, long long, long long, int, int, int, int, float*, long long,
-                     long long, cudaStream_t);
+                     long long, cudaStream_t, const float*, long long, long long);
 size_t loo_workspace_bytes(int, int, int);
 int loo_pass(const float*, long long, long long, int, int, int, int, int, double, double*, int*, int*, void*,
              cudaStream_t);
@@ -153,7 +154,7 @@ int hmcx_hmc_run_sink(const hmcx_target_t* target, const hmcx_mass_t* mass, cons
     if (target->kind == HMCX_TARGET_MLP)      // un-split Bayesian NN == sample_model (samplers.py:1261)
         return hmcx::mlp_split_run(target, mass, rng, nuts, HMCX_SCHEME_PLAIN, q_init, q_cur, eps, C, ld, L,
                                    num_samples, burn, iter_begin, iter_end, samples_out, accept_out, diverged_out,
-                                   ham_out, num_rejected, (cudaStream_t)stream, nullptr, nullptr, nullptr, nullptr);
+                                   ham_out, num_rejected, (cudaStream_t)stream, nullptr, nullptr, nullptr, nullptr, nullptr);
     return HMCX_ERR_UNSUPPORTED;
 }
 
@@ -173,14 +174,30 @@ int hmcx_split_run_sink(const hmcx_target_t* target, const hmcx_mass_t* mass, co
                         int32_t C, int32_t ld, int32_t L, int32_t num_samples, int32_t burn, int32_t iter_begin,
                         int32_t iter_end, float* samples_out, uint8_t* accept_out, uint8_t* diverged_out,
                         float* ham_out, int32_t* num_rejected, const hmcx_sink_t* sink, void* stream) {
+    return hmcx_split_run_hyper(target, mass, rng, nuts, scheme, q_init, q_cur, eps, C, ld, L, num_samples, burn, iter_begin,
+                                iter_end, samples_out, accept_out, diverged_out, ham_out, num_rejected, sink, nullptr,
+                                stream);
+}
+
+int hmcx_split_run_hyper(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmcx_rng_t* rng,
+                         const hmcx_nuts_t* nuts, int32_t scheme, const float* q_init, float* q_cur, float* eps,
+                         int32_t C, int32_t ld, int32_t L, int32_t num_samples, int32_t burn, int32_t iter_begin,
+                         int32_t iter_end, float* samples_out, uint8_t* accept_out, uint8_t* diverged_out,
+                         float* ham_out, int32_t* num_rejected, const hmcx_sink_t* sink, const hmcx_hyper_t* hyper,
+                         void* stream) {
     if (!target) return HMCX_ERR_INVALID_ARG;
     if (sink && (sink->thin < 1 || (sink->sum_lo && !sink->sum) || (sink->sumsq_lo && !sink->sumsq)))
         return HMCX_ERR_INVALID_ARG;
     if (target->kind != HMCX_TARGET_MLP) return HMCX_ERR_UNSUPPORTED;
-    if (!sink && has_mu_chain(nuts)) return HMCX_ERR_UNSUPPORTED;
+    if (!sink && !hyper && has_mu_chain(nuts)) return HMCX_ERR_UNSUPPORTED;
     return hmcx::mlp_split_run(target, mass, rng, nuts, scheme, q_init, q_cur, eps, C, ld, L, num_samples, burn,
                                iter_begin, iter_end, samples_out, accept_out, diverged_out, ham_out, num_rejected,
-                               (cudaStream_t)stream, nullptr, nullptr, nullptr, sink);
+                               (cudaStream_t)stream, nullptr, nullptr, nullptr, sink, hyper);
+}
+
+int hmcx_hyper_gamma_draws(uint64_t seed, uint64_t chain_offset, int32_t C, int32_t iter_begin, int32_t iter_end,
+                           int32_t K, const double* shapes, double* out, void* stream) {
+    return hmcx::hyper_gamma_draws(seed, chain_offset, C, iter_begin, iter_end, K, shapes, out, (cudaStream_t)stream);
 }
 
 int hmcx_split_leapfrog(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmcx_rng_t* rng, int32_t scheme,
@@ -338,7 +355,18 @@ int hmcx_mlp_pointwise_ll(const hmcx_target_t* target, const float* samples, int
     if (!target) return HMCX_ERR_INVALID_ARG;
     if (target->kind != HMCX_TARGET_MLP) return HMCX_ERR_UNSUPPORTED;
     return hmcx::mlp_pointwise_ll(target, samples, chain_stride, draw_stride, C, n, row_begin, row_end, ll_out,
-                                  ll_chain_stride, ll_draw_stride, (cudaStream_t)stream);
+                                  ll_chain_stride, ll_draw_stride, (cudaStream_t)stream, nullptr, 0, 0);
+}
+
+int hmcx_mlp_pointwise_ll_tau(const hmcx_target_t* target, const float* samples, int64_t chain_stride,
+                              int64_t draw_stride, int32_t C, int32_t n, int32_t row_begin, int32_t row_end,
+                              const float* tau_out, int64_t tau_chain_stride, int64_t tau_draw_stride, float* ll_out,
+                              int64_t ll_chain_stride, int64_t ll_draw_stride, void* stream) {
+    if (!target) return HMCX_ERR_INVALID_ARG;
+    if (target->kind != HMCX_TARGET_MLP) return HMCX_ERR_UNSUPPORTED;
+    return hmcx::mlp_pointwise_ll(target, samples, chain_stride, draw_stride, C, n, row_begin, row_end, ll_out,
+                                  ll_chain_stride, ll_draw_stride, (cudaStream_t)stream, tau_out, tau_chain_stride,
+                                  tau_draw_stride);
 }
 
 static inline bool loo_shape_ok(int32_t C, int32_t n) {

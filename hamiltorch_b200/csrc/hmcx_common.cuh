@@ -45,7 +45,7 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
     return c;
 }
 
-enum { STREAM_MOMENTUM = 0, STREAM_ACCEPT = 1, STREAM_JITTER = 2, STREAM_PERM = 3 };
+enum { STREAM_MOMENTUM = 0, STREAM_ACCEPT = 1, STREAM_JITTER = 2, STREAM_PERM = 3, STREAM_HYPER = 4 };
 
 // The key schedule k_r = k_0 + r*(W0, W1) depends on (seed, chain) only: a persistent kernel that owns one chain computes it
 // once and keeps the 20 words in registers (the asm makes them opaque, otherwise the compiler re-derives each with an
@@ -189,6 +189,34 @@ __device__ __forceinline__ void philox_jitter4(uint64_t seed, uint64_t chain, ui
     u[1] = (float)(r.y >> 8) * 5.9604645e-8f;
     u[2] = (float)(r.z >> 8) * 5.9604645e-8f;
     u[3] = (float)(r.w >> 8) * 5.9604645e-8f;
+}
+
+// Standard Gamma(alpha) draw of the hyperprior Gibbs step (Marsaglia & Tsang 2000), in fp64.  Attempt t of group k reads
+// the Philox block (seed, chain, iter, k << 16 | t) of STREAM_HYPER: a 53-bit uniform from words x, y and a 32-bit one from
+// z give the normal (Box-Muller), w the acceptance uniform.  Shapes below 1 draw G(alpha + 1) U^(1/alpha), U from the block
+// k << 16 | 0xFFFF.  The counters depend on (seed, global chain, iteration, group) only, never on the launch geometry.
+__device__ __forceinline__ double u01_53(uint32_t hi, uint32_t lo) {          // (0, 1)
+    return ((double)(((uint64_t)hi << 21) | (lo >> 11)) + 0.5) * 1.1102230246251565e-16;
+}
+static __device__ __noinline__ double philox_std_gamma(uint64_t seed, uint64_t chain, uint64_t iter, uint32_t group, double alpha) {
+    const bool boost = alpha < 1.0;
+    const double d = (boost ? alpha + 1.0 : alpha) - 1.0 / 3.0, c = 1.0 / sqrt(9.0 * d);
+    double g = 0.0;
+    for (uint32_t t = 0; t < 0xFFFFu; ++t) {
+        const uint4 r = philox_draw(seed, chain, iter, (group << 16) | t, STREAM_HYPER);
+        const double u1 = u01_53(r.x, r.y), u2 = ((double)r.z + 0.5) * 2.3283064365386963e-10;
+        const double u3 = ((double)r.w + 0.5) * 2.3283064365386963e-10;
+        const double z = sqrt(-2.0 * log(u1)) * cospi(2.0 * u2);
+        double v = 1.0 + c * z;
+        if (v <= 0.0) continue;
+        v = v * v * v;
+        if (log(u3) < 0.5 * z * z + d - d * v + d * log(v)) { g = d * v; break; }
+    }
+    if (boost) {
+        const uint4 r = philox_draw(seed, chain, iter, (group << 16) | 0xFFFFu, STREAM_HYPER);
+        g *= pow(u01_53(r.x, r.y), 1.0 / alpha);
+    }
+    return g;
 }
 
 // ---------------------------------------------------------------------------------------------------------

@@ -19,6 +19,7 @@
 #include "hmcx_common.cuh"
 #include "hmcx_wgmma.cuh"
 #include <cooperative_groups.h>
+#include <cfloat>
 
 namespace cg = cooperative_groups;
 
@@ -946,11 +947,14 @@ __device__ __forceinline__ float mlp_log_prior(const MlpDev& m, const float* q, 
 }
 
 // log p(q) = sum over splits of (ll_m + l_prior/prior_scale)  (hamiltonian's split loop, samplers.py:787-796);
-// with s >= 0 only that split.  Optionally writes the network outputs (predict_model).
+// with s >= 0 only that split.  Optionally writes the network outputs (predict_model) and, to every thread's *sse_out, the
+// loss sums of the splits added in fp64 in split order (the regression SSE the tau_out Gibbs step needs).
 template <int CS>
 __device__ __forceinline__ float mlp_log_prob(const MlpDev& m, const float* q, float* tile, float* sred, int s,
-                                              float* pred_out, ClusterCtx cc, float* xslot, TcCtx& tc) {
+                                              float* pred_out, ClusterCtx cc, float* xslot, TcCtx& tc,
+                                              double* sse_out = nullptr) {
     const float prior_term = __fdiv_rn(mlp_log_prior(m, q, sred), m.prior_scale);
+    if (sse_out) *sse_out = 0.0;
     if (!m.has_data) return prior_term;
     TcEpi te;
     if (m.tc) {
@@ -988,6 +992,7 @@ __device__ __forceinline__ float mlp_log_prob(const MlpDev& m, const float* q, f
         block_sum<1>(sse, sred);
         __syncthreads();
         sse[0] = cluster_sum_scalar<CS>(sse[0], xslot);
+        if (sse_out) *sse_out += (double)sse[0];
         const float ll = mlp_ll_from_sum(m, sse[0], m.sb[sp + 1] - m.sb[sp]);
         lp = (sp == s0) ? add(ll, prior_term) : add(lp, add(ll, prior_term));
     }
@@ -997,6 +1002,70 @@ __device__ __forceinline__ float mlp_log_prob(const MlpDev& m, const float* q, f
 // ---------------------------------------------------------------------------------------------------------
 // persistent sample() kernel for the BNN path
 // ---------------------------------------------------------------------------------------------------------
+constexpr int HYPER_GROUPS = 2 * HMCX_MLP_MAX_LAYERS + 1;     // the parameter tensors, then tau_out
+
+// Gamma hyperpriors on the precisions (hmcx_hyper_t), read by the HYPER instantiations only.  Group k < 2L is parameter
+// tensor k (tau_list order), group 2L the regression likelihood's tau_out.
+struct MlpHyperDev {
+    int sampled;                  // bit k: group k is Gibbs-updated
+    double a[HYPER_GROUPS], b[HYPER_GROUPS];
+    double n_obs;                 // N * O, the Gaussian likelihood's observation count
+    float* tau;                   // [C, 2L] in/out
+    float* tau_out;               // [C] in/out
+    float* tau_trace;             // [C, keep, 2L] or NULL
+    float* tau_out_trace;         // [C, keep] or NULL
+    const double* gammas;         // INJECTED: standard-gamma draws [it1 - it0, C, 2L + 1]
+};
+
+// A HYPER kernel reads the model descriptor from a shared-memory copy whose prior constants and c_ll follow the chain's
+// current precisions (the constant bank holds the launch-wide ones).
+struct HyperSm {
+    MlpDev m;
+    double red[MLP_THREADS / 32];
+    double ssq[2 * HMCX_MLP_MAX_LAYERS];
+    float tau[2 * HMCX_MLP_MAX_LAYERS];
+    float tau_out;
+};
+__device__ __forceinline__ HyperSm& hyper_sm() {
+    __shared__ HyperSm s;
+    return s;
+}
+template <bool HYPER>
+__device__ __forceinline__ const MlpDev& run_model(const MlpDev& m) {
+    if constexpr (HYPER) return hyper_sm().m;
+    else return m;
+}
+
+// The prior constants of the sampled tensors and c_ll from the precisions, in fp32 with the host's operation order
+// (targets.MLPTarget.__init__: scale = tau ** -0.5, two_var = 2 * scale ** 2, log_scale = log(scale),
+// grad_coef = (1 / prior_scale) / two_var; c_ll = fp32(-0.5 * tau_out)).  Unsampled groups keep the host's constants.
+__device__ __forceinline__ void hyper_constants(MlpDev& m, const float* tau, float tau_out, int sampled) {
+    for (int t = 0; t < 2 * m.L; ++t) {
+        if (!((sampled >> t) & 1)) continue;
+        const float sc = __fdiv_rn(1.0f, __fsqrt_rn(tau[t]));
+        const float tv = mul(2.0f, mul(sc, sc));
+        m.two_var[t] = tv;
+        m.log_scale[t] = logf(sc);
+        m.gcoef[t] = __fdiv_rn(__fdiv_rn(1.0f, m.prior_scale), tv);
+    }
+    if ((sampled >> (2 * m.L)) & 1) {
+        m.tau_out = tau_out;
+        m.c_ll = (float)(-0.5 * (double)tau_out);
+    }
+}
+
+// sum over the CTA in fp64, in a fixed order (xor butterflies, then the warps in order): every thread returns the same bits
+__device__ __forceinline__ double block_sum_d(double v, double* red) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    double s = 0.0;
+    for (int w = 0; w < MLP_THREADS / 32; ++w) s += red[w];
+    __syncthreads();
+    return s;
+}
+
 struct MlpRunArgs {
     MlpDev m;
     int scheme, mk, C, ld;
@@ -1037,6 +1106,7 @@ struct MlpRunArgs {
     // mass adaptation (ABI v11), SINK only: moments over every iteration of the launch; per-chain mu (may be null)
     int moments_all;
     const double* mu_chain;
+    MlpHyperDev hy;               // HYPER instantiations only
 };
 
 // One sink accumulator [C, ld] (sum, or sum of squares when `squares`) += the float4 x at element offset `off`, read and
@@ -1065,8 +1135,9 @@ __device__ __forceinline__ void sink_accumulate(float* hi, float* lo, size_t off
 }
 
 // SINK = false: the plain sample() loop (rank 0 stores every post-burn row); SINK = true adds the sample sink, its row
-// work divided over the cluster's ranks (see sink_row below)
-template <int CS, bool SINK>
+// work divided over the cluster's ranks (see sink_row below).  HYPER (with SINK only) adds the Gibbs updates of the Gamma
+// hyperpriors on the precisions after every MH step (DESIGN.md 3.15).
+template <int CS, bool SINK, bool HYPER = false>
 __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArgs a) {
     extern __shared__ __align__(128) float sm[];
     __shared__ float sred[64];
@@ -1075,7 +1146,19 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
     __shared__ int s_perm[HMCX_MLP_MAX_SPLITS];
     __shared__ __align__(8) uint64_t s_bars[3];
 
-    const MlpDev& m = a.m;
+    static_assert(SINK || !HYPER, "the hyperprior form is a sink form");
+    if constexpr (HYPER) {                                     // this chain's precisions and the constants they give
+        HyperSm& hs = hyper_sm();
+        if (threadIdx.x == 0) {
+            const int c0 = blockIdx.x / CS, K = 2 * a.m.L;
+            hs.m = a.m;
+            for (int k = 0; k < K; ++k) hs.tau[k] = a.hy.tau[(size_t)c0 * K + k];
+            hs.tau_out = a.hy.tau_out[c0];
+            hyper_constants(hs.m, hs.tau, hs.tau_out, a.hy.sampled);
+        }
+        __syncthreads();
+    }
+    const MlpDev& m = run_model<HYPER>(a.m);
     ClusterCtx cc = {0, 1};
     if (CS > 1) { cc.rank = (int)cg::this_cluster().block_rank(); cc.size = CS; }
     const bool lead = cc.rank == 0;                            // rank 0 owns every global-memory output but the sink rows
@@ -1091,7 +1174,9 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
 
     for (int i = tid; i < m.Dp; i += MLP_THREADS) { q[i] = i < D ? a.q_cur[row + i] : 0.0f; p[i] = 0.0f; g[i] = 0.0f; }
     __syncthreads();
-    float lp_cur = a.p_given ? 0.0f : mlp_log_prob<CS>(m, q, tile, sred, -1, nullptr, cc, &s_xchg, tc);
+    double sse_cur = 0.0, sse_new = 0.0;                      // HYPER: the loss sum at q_cur / at the proposal
+    float lp_cur = a.p_given ? 0.0f : mlp_log_prob<CS>(m, q, tile, sred, -1, nullptr, cc, &s_xchg, tc,
+                                                       HYPER ? &sse_cur : nullptr);
 
     float eps = a.eps[c];
     double h_bar = 0.0, eps_bar = 1.0;
@@ -1121,6 +1206,19 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
         if constexpr (SINK) sink_row(my_samples, false);
         else for (int i = tid; i < a.ld; i += MLP_THREADS) my_samples[i] = i < D ? q[i] : 0.0f;
     }
+    // HYPER: the precisions of retained slot j (the slots of samples_out, thinned alike); slot 0 = the initial values
+    auto hyper_store = [&](int slot) {
+        if constexpr (HYPER) {
+            if (tid == 0 && lead) {
+                const HyperSm& hs = hyper_sm();
+                const int K = 2 * m.L;
+                if (a.hy.tau_trace)
+                    for (int k = 0; k < K; ++k) a.hy.tau_trace[((size_t)c * keep + slot) * K + k] = hs.tau[k];
+                if (a.hy.tau_out_trace) a.hy.tau_out_trace[(size_t)c * keep + slot] = hs.tau_out;
+            }
+        }
+    };
+    if (a.it0 == 0) hyper_store(0);
 
     auto kinetic = [&]() {                                    // 2*K: p.p or p.(im*p)   (samplers.py:801, :814)
         float s[1] = {0.0f};
@@ -1394,7 +1492,7 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
         }
         if (a.p_given) break;                                             // stand-alone leapfrog: no Hamiltonian, no MH
         // ---- Hamiltonians + MH ----
-        const float lp_new = mlp_log_prob<CS>(m, q, tile, sred, -1, nullptr, cc, &s_xchg, tc);
+        const float lp_new = mlp_log_prob<CS>(m, q, tile, sred, -1, nullptr, cc, &s_xchg, tc, HYPER ? &sse_new : nullptr);
         const float kin1 = kinetic();
         const float h_old = add(-lp_cur, mul(0.5f, kin0));
         const float h_new = add(-lp_new, mul(0.5f, kin1));
@@ -1409,6 +1507,7 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
         const bool acc = !bad && (rho >= logu);
         if (acc) {
             lp_cur = lp_new;
+            if constexpr (HYPER) sse_cur = sse_new;
             if (lead) for (int i = tid; i < D; i += MLP_THREADS) a.q_cur[row + i] = q[i];
         } else {
             ++rejected;
@@ -1417,11 +1516,48 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
             for (int i = tid; i < D; i += MLP_THREADS) q[i] = src[row + i];
             __syncthreads();
             if (n == a.burn + 1) {
-                lp_cur = mlp_log_prob<CS>(m, q, tile, sred, -1, nullptr, cc, &s_xchg, tc);
+                lp_cur = mlp_log_prob<CS>(m, q, tile, sred, -1, nullptr, cc, &s_xchg, tc, HYPER ? &sse_cur : nullptr);
                 if (lead) for (int i = tid; i < D; i += MLP_THREADS) a.q_cur[row + i] = q[i];
             }
         }
         if (CS > 1) cg::this_cluster().sync();                 // q_cur is stable before any rank re-reads it
+        if constexpr (HYPER) {
+            // Gibbs step of the precisions given q_n: tau_k ~ Gamma(a_k + n_k/2, b_k + |w_k|^2/2), tau_out ~ Gamma(a_o + N O/2,
+            // b_o + SSE(q_n)/2).  |w_k|^2 is a fixed-order fp64 sum over every rank's identical replica of q, SSE the cluster
+            // sum of the MH evaluation at q_cur, so every rank draws the same precisions.
+            HyperSm& hs = hyper_sm();
+            const int K = 2 * m.L;
+            __syncthreads();                                   // nobody reads the constants thread 0 rewrites below
+            for (int t = 0; t < K; ++t) {
+                if (!((a.hy.sampled >> t) & 1)) continue;
+                const int l = t >> 1, off = (t & 1) ? m.boff[l] : m.woff[l];
+                const int cnt = (t & 1) ? m.n[l + 1] : m.n[l] * m.n[l + 1];
+                double ss = 0.0;
+                for (int i = tid; i < cnt; i += MLP_THREADS) { const double w = (double)q[off + i]; ss = fma(w, w, ss); }
+                ss = block_sum_d(ss, hs.red);
+                if (tid == 0) hs.ssq[t] = ss;
+            }
+            if (tid == 0) {
+                for (int k = 0; k <= K; ++k) {
+                    if (!((a.hy.sampled >> k) & 1)) continue;
+                    const int l = k >> 1;
+                    const double nk = k < K ? (double)((k & 1) ? m.n[l + 1] : m.n[l] * m.n[l + 1]) : a.hy.n_obs;
+                    const double shape = a.hy.a[k] + 0.5 * nk, rate = a.hy.b[k] + 0.5 * (k < K ? hs.ssq[k] : sse_cur);
+                    const double g = a.rng_mode == HMCX_RNG_INJECTED
+                                         ? a.hy.gammas[((size_t)(n - a.it0) * a.C + c) * (K + 1) + k]
+                                         : philox_std_gamma(a.seed, chain_id, (uint64_t)n, (uint32_t)k, shape);
+                    const float tau = (float)(g / rate);
+                    if (k < K) hs.tau[k] = tau;
+                    else hs.tau_out = tau;
+                }
+                hyper_constants(hs.m, hs.tau, hs.tau_out, a.hy.sampled);
+            }
+            __syncthreads();
+            // log p(q_cur) and any carried gradient belong to the old precisions: re-evaluate the former, drop the latter
+            lp_cur = mlp_log_prob<CS>(m, q, tile, sred, -1, nullptr, cc, &s_xchg, tc);
+            g_fresh = false;
+            if (n > a.burn && (n - a.burn) % a.thin == 0) hyper_store((n - a.burn) / a.thin);
+        }
         if constexpr (SINK) {
             if (n > a.burn)
                 sink_row((my_samples && (n - a.burn) % a.thin == 0) ? my_samples + (size_t)((n - a.burn) / a.thin) * a.ld
@@ -1460,6 +1596,13 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
             a.eps_trace[(size_t)c * a.S + n] = eps;
         }
         __syncthreads();
+    }
+    if constexpr (HYPER) {
+        if (tid == 0 && lead) {
+            const HyperSm& hs = hyper_sm();
+            for (int k = 0; k < 2 * m.L; ++k) a.hy.tau[(size_t)c * 2 * m.L + k] = hs.tau[k];
+            a.hy.tau_out[c] = hs.tau_out;
+        }
     }
     if (tid == 0 && lead && !a.p_given) {
         a.eps[c] = eps;
@@ -1596,6 +1739,89 @@ mlp_ll_kernel(const MlpDev m, const float* __restrict__ samples, long long cs, l
     }
 }
 
+// mlp_ll_rows / mlp_ll_kernel with one tau_out per draw (the draws of a run with a tau_out hyperprior, DESIGN.md 3.15):
+// draw (c, s) reads tau[c * tcs + s * tds] and evaluates its constant 0.5 O log(tau / 2 pi) as the host does for the
+// target's tau_out (fp64 log, then the fp32 rounding).  A separate kernel, so that mlp_ll_kernel's code stays as it is.
+__device__ __forceinline__ void mlp_ll_rows_tau(const MlpDev& m, const float* out, const float* ytile, int r0, int cnt,
+                                            int r_begin, int r_end, float ll_const, float tau_out,
+                                                float* llrow) {
+    const int nL = m.n[m.L];
+    for (int r = threadIdx.x; r < cnt; r += MLP_THREADS) {
+        const int i = r0 + r;
+        if (i < r_begin || i >= r_end) continue;
+        const float* z = out + r * nL;
+        float v = 0.0f;
+        if (m.loss == HMCX_LOSS_REGRESSION || m.loss == HMCX_LOSS_BINARY) {
+            for (int o = 0; o < nL; ++o) {
+                const float yv = ytile ? ytile[r * nL + o] : __ldg(m.y + (size_t)i * nL + o), f = z[o];
+                if (m.loss == HMCX_LOSS_REGRESSION) {
+                    const float d = f - yv;
+                    v += d * d;
+                } else {
+                    v -= (1.0f - yv) * f + fmaxf(-f, 0.0f) + log1pf(expf(-fabsf(f)));
+                }
+            }
+            if (m.loss == HMCX_LOSS_REGRESSION) v = ll_const + (-0.5f * tau_out) * v;
+        } else {
+            // both multi-class losses: the tile holds the logits (a LogSoftmax output layer is applied here, as in the
+            // loss stage), so f[y] of a LogSoftmax network is log_softmax(logits)[y]
+            int label = (int)(ytile ? ytile[r] : __ldg(m.y + i));
+            label = label < 0 ? 0 : (label >= nL ? nL - 1 : label);
+            float mx = z[0];
+            for (int k = 1; k < nL; ++k) mx = fmaxf(mx, z[k]);
+            float se = 0.0f;
+            for (int k = 0; k < nL; ++k) se += expf(z[k] - mx);
+            v = (z[label] - mx) - logf(se);
+        }
+        llrow[i] = v;
+    }
+}
+
+
+__global__ void __launch_bounds__(MLP_THREADS, 1)
+mlp_ll_tau_kernel(const MlpDev m, const float* __restrict__ samples, long long cs, long long ds, int n, int r_begin,
+                  int r_end, float* __restrict__ ll, long long lcs, long long lds, const float* __restrict__ tau,
+                  long long tcs, long long tds) {
+    extern __shared__ __align__(128) float sm[];
+    __shared__ __align__(8) uint64_t s_bars[3];
+    float* q = sm;
+    float* tile = sm + m.tile_base;
+    const int c = blockIdx.x / n, s = blockIdx.x - c * n;
+    const float* qin = samples + (long long)c * cs + (long long)s * ds;
+    for (int i = threadIdx.x; i < m.Dp; i += MLP_THREADS) q[i] = i < m.D ? qin[i] : 0.0f;
+    const float tau_out = tau[(long long)c * tcs + (long long)s * tds];
+    const float ll_const = (float)(0.5 * m.n[m.L] * log((double)tau_out / (2.0 * 3.14159265358979323846)));
+    __syncthreads();
+    float* llrow = ll + (long long)c * lcs + (long long)s * lds - r_begin;
+    TcCtx tc = {};
+    TcEpi te;
+    if (m.tc) {
+        tc_init(tc, s_bars);
+        tc_epi_begin(m, q, te);
+        fence_async_smem();
+        __syncthreads();
+    }
+    for (int sp = 0; sp < m.M; ++sp) {
+        if (m.sb[sp + 1] <= r_begin || m.sb[sp] >= r_end) continue;
+        int ti = 0;
+        for (int r0 = m.sb[sp]; r0 < m.sb[sp + 1] && r0 < r_end; r0 += m.T, ++ti) {
+            if (r0 + m.T <= r_begin) continue;
+            const int cnt = min(m.T, m.sb[sp + 1] - r0);
+            if (m.tc) {
+                float act[16];
+                tc_prefetch_fwd(m, tile, tc, m.tb[sp] + ti, 0);
+                tc_prefetch_y(m, tile, r0, cnt);
+                tc_forward_tile(m, q, tile, tc, te, act, 0);
+            } else {
+                mlp_forward_tile(m, q, tile, r0, cnt);
+            }
+            mlp_ll_rows_tau(m, tile + m.aoff[m.L], m.tc ? tile + m.tc_yraw : nullptr, r0, cnt, r_begin, r_end, ll_const,
+                            tau_out, llrow);
+            __syncthreads();
+        }
+    }
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------
@@ -1616,8 +1842,9 @@ static bool mlp_tc_shape(const MlpDev& m) {
     return m.L == 2 && m.n[1] == TC_H && m.n[0] >= 16 && m.n[0] <= 64 && (m.n[0] & 15) == 0 && m.n[2] <= TC_NLMAX && m.has_data;
 }
 
-// tensor-core layout of the tile area (one-hidden-layer stacks n0 -> 128 -> nL, see the tensor-core section above)
-static bool mlp_layout_tc(MlpDev& m, int state_vectors) {
+// tensor-core layout of the tile area (one-hidden-layer stacks n0 -> 128 -> nL, see the tensor-core section above);
+// `reserve`: static shared memory a kernel form holds beyond the common headroom (HyperSm for the HYPER forms)
+static bool mlp_layout_tc(MlpDev& m, int state_vectors, size_t reserve) {
     if (!mlp_tc_shape(m) || !m.xp) return false;
     const int n0 = m.n[0];
     int off = 0;
@@ -1633,17 +1860,17 @@ static bool mlp_layout_tc(MlpDev& m, int state_vectors) {
     m.tile_base = (state_vectors * m.Dp + 31) / 32 * 32;      // 128-byte aligned operand buffers
     m.T = TC_TR;
     m.tc = 1;
-    return (size_t)(m.tile_base + m.tile_floats) * sizeof(float) <= 227 * 1024 - 2048;
+    return (size_t)(m.tile_base + m.tile_floats) * sizeof(float) + reserve <= 227 * 1024 - 2048;
 }
 
 // pick the largest tile height whose buffers fit next to `state_vectors` copies of the parameter vector
-static bool mlp_pick_tile(MlpDev& m, int state_vectors, bool allow_tc = false) {
-    if (allow_tc && mlp_layout_tc(m, state_vectors)) return true;
+static bool mlp_pick_tile(MlpDev& m, int state_vectors, bool allow_tc = false, size_t reserve = 0) {
+    if (allow_tc && mlp_layout_tc(m, state_vectors, reserve)) return true;
     m.tc = 0;
     m.tile_base = state_vectors * m.Dp;
     for (int T = MLP_T_MAX; T >= 8; T >>= 1) {
         mlp_layout_tiles(m, T);
-        if ((size_t)(state_vectors * m.Dp + m.tile_floats) * sizeof(float) <= 227 * 1024 - 4096) return true;
+        if ((size_t)(state_vectors * m.Dp + m.tile_floats) * sizeof(float) + reserve <= 227 * 1024 - 4096) return true;
     }
     return false;
 }
@@ -1728,8 +1955,10 @@ int mlp_split_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hm
                   int scheme, const float* q_init, float* q_cur, float* eps, int C, int ld, int L, int S, int burn,
                   int it0, int it1, float* samples, uint8_t* accept, uint8_t* diverged, float* ham,
                   int32_t* num_rejected, cudaStream_t st, const float* p_given, float* q_traj, float* p_traj,
-                  const hmcx_sink_t* sink) {
+                  const hmcx_sink_t* sink, const hmcx_hyper_t* hyper) {
     MlpRunArgs a = {};
+    hmcx_sink_t thin1 = {};
+    if (hyper && !sink) { thin1.thin = 1; sink = &thin1; }      // the hyperprior form is a sink form
     a.p_given = p_given; a.q_traj = q_traj; a.p_traj = p_traj;
     if (sink) {
         a.thin = sink->thin; a.msum = sink->sum; a.msumsq = sink->sumsq;
@@ -1753,6 +1982,24 @@ int mlp_split_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hm
     } else if (rng->mode != HMCX_RNG_PHILOX) {
         return HMCX_ERR_INVALID_ARG;
     }
+    if (hyper) {
+        const int K = 2 * a.m.L;
+        if (!hyper->tau || !hyper->tau_out || p_given) return HMCX_ERR_INVALID_ARG;
+        if (rng->mode == HMCX_RNG_INJECTED && !hyper->gammas) return HMCX_ERR_INVALID_ARG;
+        for (int k = 0; k < HMCX_HYPER_GROUPS; ++k) {
+            if (!hyper->sampled[k]) continue;
+            if (k > K || !(hyper->a[k] > 0.0) || !(hyper->b[k] > 0.0) || !(hyper->a[k] <= DBL_MAX) || !(hyper->b[k] <= DBL_MAX))
+                return HMCX_ERR_INVALID_ARG;
+            a.hy.sampled |= 1 << k;
+            a.hy.a[k] = hyper->a[k]; a.hy.b[k] = hyper->b[k];
+        }
+        if (hyper->sampled[K] && !a.m.has_data) return HMCX_ERR_INVALID_ARG;
+        if (hyper->sampled[K] && a.m.loss != HMCX_LOSS_REGRESSION) return HMCX_ERR_UNSUPPORTED;
+        a.hy.n_obs = (double)a.m.N * (double)a.m.n[a.m.L];
+        a.hy.tau = hyper->tau; a.hy.tau_out = hyper->tau_out;
+        a.hy.tau_trace = hyper->tau_trace; a.hy.tau_out_trace = hyper->tau_out_trace;
+        a.hy.gammas = hyper->gammas;
+    }
     a.scheme = scheme; a.mk = mk; a.C = C; a.ld = ld;
     a.im = mass ? mass->inv_mass : nullptr; a.sd = mass ? mass->mass_factor : nullptr;
     a.rng_mode = rng->mode; a.seed = rng->seed; a.chain_offset = rng->chain_offset;
@@ -1767,7 +2014,7 @@ int mlp_split_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hm
     }
     a.q_init = q_init; a.q_cur = q_cur; a.eps = eps; a.L = L; a.S = S; a.burn = burn; a.it0 = it0; a.it1 = it1;
     a.samples = samples; a.accept = accept; a.diverged = diverged; a.ham = ham; a.num_rejected = num_rejected;
-    if (!mlp_pick_tile(a.m, 3, target->mlp->tensor_cores != HMCX_MLP_TC_OFF))
+    if (!mlp_pick_tile(a.m, 3, target->mlp->tensor_cores != HMCX_MLP_TC_OFF, hyper ? sizeof(HyperSm) : 0))
         return HMCX_ERR_UNSUPPORTED;                            // q, p, g do not fit one SM's shared memory
     const size_t smem = (size_t)(a.m.tile_base + a.m.tile_floats) * sizeof(float);
     // CTAs per chain (thread-block cluster size): at most the tiles of the smallest split, at most 4, and -- unless the
@@ -1794,7 +2041,8 @@ int mlp_split_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hm
     attr[0].val.clusterDim.x = cs; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
     void (*kern)(MlpRunArgs);
-    if (cs == 4) kern = sink ? mlp_run_kernel<4, true> : mlp_run_kernel<4, false>;
+    if (hyper) kern = cs == 4 ? mlp_run_kernel<4, true, true> : cs == 2 ? mlp_run_kernel<2, true, true> : mlp_run_kernel<1, true, true>;
+    else if (cs == 4) kern = sink ? mlp_run_kernel<4, true> : mlp_run_kernel<4, false>;
     else if (cs == 2) kern = sink ? mlp_run_kernel<2, true> : mlp_run_kernel<2, false>;
     else kern = sink ? mlp_run_kernel<1, true> : mlp_run_kernel<1, false>;
     rc = prepare_smem(kern, smem);
@@ -1833,19 +2081,27 @@ int mlp_predict(const hmcx_target_t* target, const float* samples, int S, int ld
 }
 
 int mlp_pointwise_ll(const hmcx_target_t* target, const float* samples, long long cs, long long ds, int C, int n,
-                     int r_begin, int r_end, float* ll, long long lcs, long long lds, cudaStream_t st) {
+                     int r_begin, int r_end, float* ll, long long lcs, long long lds, cudaStream_t st,
+                     const float* tau, long long tcs, long long tds) {
     MlpDev m = {};
     int rc = fill_mlp(target, m);
     if (rc != HMCX_OK) return rc;
     if (!samples || !ll || C < 1 || n < 1 || (long long)C * n > 0x7fffffffLL || cs < 0 || ds < 0 || lcs < 0 || lds < 0 ||
-        !m.has_data || r_begin < 0 || r_end > m.N || r_begin >= r_end)
+        !m.has_data || r_begin < 0 || r_end > m.N || r_begin >= r_end || tcs < 0 || tds < 0)
         return HMCX_ERR_INVALID_ARG;
     if (!mlp_pick_tile(m, 1, target->mlp->tensor_cores != HMCX_MLP_TC_OFF)) return HMCX_ERR_UNSUPPORTED;
     const size_t smem = (size_t)(m.tile_base + m.tile_floats) * sizeof(float);
+    if (tau) {
+        rc = prepare_smem(mlp_ll_tau_kernel, smem);
+        if (rc != HMCX_OK) return rc;
+        mlp_ll_tau_kernel<<<C * n, MLP_THREADS, smem, st>>>(m, samples, cs, ds, n, r_begin, r_end, ll, lcs, lds, tau, tcs,
+                                                            tds);
+        return cuda_status();
+    }
     rc = prepare_smem(mlp_ll_kernel, smem);
     if (rc != HMCX_OK) return rc;
-    const double tau = (double)target->mlp->tau_out;
-    const float ll_const = (float)(0.5 * m.n[m.L] * log(tau / (2.0 * 3.14159265358979323846)));
+    const double tau_t = (double)target->mlp->tau_out;
+    const float ll_const = (float)(0.5 * m.n[m.L] * log(tau_t / (2.0 * 3.14159265358979323846)));
     mlp_ll_kernel<<<C * n, MLP_THREADS, smem, st>>>(m, samples, cs, ds, n, r_begin, r_end, ll_const, ll, lcs, lds);
     return cuda_status();
 }
@@ -1859,7 +2115,30 @@ int mlp_leapfrog(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmc
     hmcx_nuts_t no_nuts = {};
     no_nuts.step_size_init = step_size;                        // the Python double the drifts divide (:513, :558)
     return mlp_split_run(target, mass, rng, &no_nuts, scheme, q_in, const_cast<float*>(q_in), eps, C, ld, L, 1, 0, 0, 1,
-                         nullptr, nullptr, nullptr, nullptr, nullptr, st, p_in, q_traj, p_traj, nullptr);
+                         nullptr, nullptr, nullptr, nullptr, nullptr, st, p_in, q_traj, p_traj, nullptr, nullptr);
+}
+
+// hmcx_hyper_gamma_draws: one thread per (iteration, chain, group), the device function of the HYPER kernels
+struct GammaShapes { double v[HYPER_GROUPS]; };
+__global__ void __launch_bounds__(256) hyper_gamma_kernel(uint64_t seed, uint64_t chain_offset, int C, int it0, int n_it,
+                                                          int K, const GammaShapes shapes, double* __restrict__ out) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (long long)n_it * C * K) return;
+    const int k = (int)(i % K), c = (int)((i / K) % C), n = it0 + (int)(i / ((long long)K * C));
+    out[i] = philox_std_gamma(seed, chain_offset + (uint64_t)c, (uint64_t)n, (uint32_t)k, shapes.v[k]);
+}
+
+int hyper_gamma_draws(uint64_t seed, uint64_t chain_offset, int C, int it0, int it1, int K, const double* shapes,
+                      double* out, cudaStream_t st) {
+    if (C < 1 || it0 < 0 || it1 <= it0 || K < 1 || K > HYPER_GROUPS || !shapes || !out) return HMCX_ERR_INVALID_ARG;
+    GammaShapes sh = {};
+    for (int k = 0; k < K; ++k) {
+        if (!(shapes[k] > 0.0) || !(shapes[k] <= DBL_MAX)) return HMCX_ERR_INVALID_ARG;
+        sh.v[k] = shapes[k];
+    }
+    const long long total = (long long)(it1 - it0) * C * K;
+    hyper_gamma_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(seed, chain_offset, C, it0, it1 - it0, K, sh, out);
+    return cuda_status();
 }
 
 // packed X operands of the tensor-core path (hmcx_mlp_t.x_packed): size in floats (0: the stack does not use it) / build

@@ -104,6 +104,8 @@ def sample_chains_sharded(log_prob_func, params_init, gather_samples=False, runn
     (``all_gather_rows``, one (C, ld) gather per sum) before the pooled estimate, so every rank adapts the same mass from
     all C chains -- with Philox keyed by the global chain id the samples do not depend on the sharding.  ``inv_mass``
     then holds the adapted (D,) mass.
+    With hyperpriors (``tau_prior`` / ``tau_out_prior``, passed through) and ``gather_samples``, ``tau_list_trace``
+    (C, keep, 2L) and ``tau_out_trace`` (C, keep) are gathered alongside the samples.
     ``runner`` replaces ``samplers.sample_chains`` and ``diagnostics_partials`` the diagnostics' CUDA stages (used by
     the CPU tests of this host logic).
     """
@@ -115,7 +117,7 @@ def sample_chains_sharded(log_prob_func, params_init, gather_samples=False, runn
     if hi == lo:
         raise RuntimeError('sample_chains_sharded: rank %d of %d would own no chain (C=%d < world); use fewer ranks'
                            % (rank, world, C))
-    for name in ('normals', 'log_uniforms', 'perms', 'uniforms'):          # every injected stream is (S, C, ...)
+    for name in ('normals', 'log_uniforms', 'perms', 'uniforms', 'gammas'):     # every injected stream is (S, C, ...)
         if kw.get(name) is not None:
             if kw[name].shape[1] != C:
                 raise RuntimeError('%s must be (S, C=%d, ...), got %s' % (name, C, tuple(kw[name].shape)))
@@ -136,6 +138,9 @@ def sample_chains_sharded(log_prob_func, params_init, gather_samples=False, runn
             raise RuntimeError('gather_samples with store_on_GPU=False: the samples live in pinned host memory, which '
                                'NCCL cannot gather -- keep them on the GPU or gather on the host')
         out['samples'] = all_gather_rows(blk, C)[..., :local.dim]
+        if getattr(local, 'tau_list_trace', None) is not None:         # hyperpriors: the precisions of the same slots
+            out['tau_list_trace'] = all_gather_rows(local.tau_list_trace, C)
+            out['tau_out_trace'] = all_gather_rows(local.tau_out_trace, C)
     if getattr(local, 'moment_sum', None) is not None:          # sink moments requested: pool them over all ranks
         out['posterior_mean'], out['posterior_var'], out['posterior_n'] = pooled_moments(
             local.moment_sum, local.moment_sumsq, local.moment_count)

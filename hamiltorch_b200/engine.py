@@ -460,7 +460,7 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
             nuts=False, desired_accept_rate=0.8, seed=0, chain_offset=0, normals=None, log_uniforms=None,
             record_ham=False, out=None, device=None, tuning=0, eps_schedule=None, record_eps=False, scheme=None,
             perms=None, thin=1, moments=False, keep_samples=True, host_samples=False, host_windows=0, adapt_mass=False,
-            mass_pool=None):
+            mass_pool=None, hyper=None, gammas=None):
     """The reference's sample() loop for sampler in {HMC, HMC_NUTS} as one persistent kernel over C chains.
 
     params_init (C, D) | (D,).  Randomness: in-kernel Philox keyed by (seed, chain_offset+c, iteration), or -- when
@@ -485,6 +485,12 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
     stream, no host synchronisation.  ``result.inv_mass`` (D,), ``result.inv_mass_trace`` (K, D), ``result.mass_windows``.
     ``mass_pool``: callable mapping each (C_local, ld) window sum to the (C, ld) sum of all chains in global order
     (distributed.sample_chains_sharded passes an all-gather), so that every rank pools every chain into the same mass.
+    ``hyper`` (Bayesian-NN targets with a ``scheme``): Gamma hyperpriors on the precisions, a list of 2L + 1 entries --
+    the parameter tensors in tau_list order, then tau_out -- each None (fixed) or (a, b) (shape, rate), Gibbs-updated
+    inside the kernel after every MH step (include/hmcx.h hmcx_hyper_t, DESIGN §3.15).  Injected mode takes ``gammas``
+    (S, C, 2L + 1) fp64 standard-gamma draws.  The result gains ``tau_list_trace`` (C, keep, 2L), ``tau_out_trace``
+    (C, keep) -- on the device whatever ``host_samples`` says -- and the final state ``tau_list_final`` (C, 2L),
+    ``tau_out_final`` (C,).
     """
     N.require_cuda()
     lib = N.load_library()
@@ -593,6 +599,32 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
             msum, msq, msum_lo, msq_lo = (torch.zeros((Cn, ld), dtype=torch.float32, device=device) for _ in range(4))
             sink.sum, sink.sumsq = msum.data_ptr(), msq.data_ptr()
             sink.sum_lo, sink.sumsq_lo = msum_lo.data_ptr(), msq_lo.data_ptr()
+    hyper_s = None
+    if hyper is not None:
+        if scheme is None:
+            raise NotImplementedError('hyperpriors: Bayesian-NN targets only')
+        desc = nt.mlp_desc
+        K = 2 * desc.num_layers
+        if len(hyper) != K + 1:
+            raise RuntimeError('hyper needs %d entries (the parameter tensors, then tau_out)' % (K + 1))
+        hyper_s = N.HyperStruct()
+        for k, ab in enumerate(hyper):
+            if ab is not None:
+                hyper_s.sampled[k] = 1
+                hyper_s.a[k], hyper_s.b[k] = float(ab[0]), float(ab[1])
+        tau = torch.tensor([float(t) for t in desc.tau_list], dtype=torch.float32).to(device).repeat(Cn, 1).contiguous()
+        tau_out = torch.full((Cn,), desc.tau_out, dtype=torch.float32, device=device)
+        tau_trace = torch.zeros((Cn, keep, K), dtype=torch.float32, device=device)
+        tau_out_trace = torch.zeros((Cn, keep), dtype=torch.float32, device=device)
+        hyper_s.tau, hyper_s.tau_out = tau.data_ptr(), tau_out.data_ptr()
+        hyper_s.tau_trace, hyper_s.tau_out_trace = tau_trace.data_ptr(), tau_out_trace.data_ptr()
+        keep_alive += [tau, tau_out, tau_trace, tau_out_trace]
+        if rng.mode == N.RNG_INJECTED:
+            if gammas is None or tuple(gammas.shape) != (S, Cn, K + 1):
+                raise RuntimeError('injected hyperpriors need gammas (S, C, 2L + 1) = (%d, %d, %d)' % (S, Cn, K + 1))
+            gm = gammas.detach().to(device=device, dtype=torch.float64).contiguous()
+            hyper_s.gammas = gm.data_ptr()
+            keep_alive.append(gm)
     mass_out = None
     with torch.cuda.device(device):
         if adapt_mass:
@@ -601,7 +633,7 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
                 sink.thin = 1
             mass_out = _adapted_launches(lib, nt, nm, rng, nuts_s, scheme, q_init, q_cur, eps, Cn, D, ld, L, S, burn,
                                          samples, accepted, diverged, ham, num_rejected, int(tuning), sink, h_bar,
-                                         eps_bar, mass_pool, device, keep_alive)
+                                         eps_bar, mass_pool, device, keep_alive, hyper_s)
         elif scheme is None:
             ws_bytes = lib.hmcx_hmc_workspace_bytes(nt.ref(), nm.ref(), Cn, ld)
             ws = torch.empty(ws_bytes // 4, dtype=torch.float32, device=device) if ws_bytes else None
@@ -646,6 +678,12 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
                                       N.ptr(diverged), N.ptr(ham), N.ptr(num_rejected), int(tuning), N.ptr(ws),
                                       N.stream_ptr(device))
                 N.check(rc, 'hmcx_hmc_run')
+        elif hyper_s is not None:
+            rc = lib.hmcx_split_run_hyper(nt.ref(), nm.ref(), C.byref(rng), C.byref(nuts_s), int(scheme), N.ptr(q_init),
+                                          N.ptr(q_cur), N.ptr(eps), Cn, ld, L, S, burn, 0, S, N.ptr(samples),
+                                          N.ptr(accepted), N.ptr(diverged), N.ptr(ham), N.ptr(num_rejected),
+                                          None if sink is None else C.byref(sink), C.byref(hyper_s), N.stream_ptr(device))
+            N.check(rc, 'hmcx_split_run_hyper')
         else:
             rc = lib.hmcx_split_run_sink(nt.ref(), nm.ref(), C.byref(rng), C.byref(nuts_s), int(scheme), N.ptr(q_init),
                                          N.ptr(q_cur), N.ptr(eps), Cn, ld, L, S, burn, 0, S, N.ptr(samples),
@@ -665,8 +703,21 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
     if mass_out is not None:
         res.inv_mass_trace, res.mass_windows = mass_out
         res.inv_mass = res.inv_mass_trace[-1]
+    if hyper_s is not None:
+        res.tau_list_trace, res.tau_out_trace = tau_trace, tau_out_trace
+        res.tau_list_final, res.tau_out_final = tau, tau_out
     res._keep_alive = keep_alive          # buffers the asynchronous kernel still reads
     return res
+
+
+def _window_hyper(hyper_s, it0, Cn, groups):
+    """The hyperprior struct of a launch starting at iteration it0: the injected gamma draws (rows of Cn * groups fp64)
+    move to row it0."""
+    if hyper_s is None or not hyper_s.gammas or it0 == 0:
+        return hyper_s
+    h = N.HyperStruct.from_buffer_copy(hyper_s)
+    h.gammas = hyper_s.gammas + it0 * Cn * groups * 8
+    return h
 
 
 def _window_rng(rng, it0, Cn, ld, num_splits):
@@ -683,9 +734,10 @@ def _window_rng(rng, it0, Cn, ld, num_splits):
 
 
 def _adapted_launches(lib, nt, nm, rng, nuts_s, scheme, q_init, q_cur, eps, Cn, D, ld, L, S, burn, samples, accepted,
-                      diverged, ham, num_rejected, tuning, sink, h_bar, eps_bar, mass_pool, device, keep_alive):
+                      diverged, ham, num_rejected, tuning, sink, h_bar, eps_bar, mass_pool, device, keep_alive,
+                      hyper_s=None):
     """hmc_run with adapt_mass: [0, a_1) and every window [a_k, b_k) of mass_windows(burn), each window followed by
-    hmcx_adapt_diag_mass, then [b_K, S) with the caller's sink.  Every launch is a sink launch (mu_chain and moments_all
+    hmcx_adapt_diag_mass, then [b_K, S) with the caller's sink (and the hyperprior state ``hyper_s``, if any).  Every launch is a sink launch (mu_chain and moments_all
     are read by the sink forms only); the launches chain through q_cur, eps, the dual-averaging state and, for element-wise
     targets, the log p workspace.  Returns (inv_mass_trace (K, D), windows)."""
     windows = mass_windows(burn)
@@ -722,11 +774,13 @@ def _adapted_launches(lib, nt, nm, rng, nuts_s, scheme, q_init, q_cur, eps, Cn, 
                                        C.byref(sink_s), stream)
             N.check(rc, 'hmcx_hmc_run_sink')
         else:
-            rc = lib.hmcx_split_run_sink(nt.ref(), mass_ref, C.byref(r), C.byref(nuts_s), int(scheme), N.ptr(q_init),
-                                         N.ptr(q_cur), N.ptr(eps), Cn, ld, L, S, burn, it0, it1, N.ptr(samples),
-                                         N.ptr(accepted), N.ptr(diverged), N.ptr(ham), N.ptr(num_rejected),
-                                         C.byref(sink_s), stream)
-            N.check(rc, 'hmcx_split_run_sink')
+            h = _window_hyper(hyper_s, it0, Cn, 2 * nt.mlp_desc.num_layers + 1)
+            keep_alive.append(h)
+            rc = lib.hmcx_split_run_hyper(nt.ref(), mass_ref, C.byref(r), C.byref(nuts_s), int(scheme), N.ptr(q_init),
+                                          N.ptr(q_cur), N.ptr(eps), Cn, ld, L, S, burn, it0, it1, N.ptr(samples),
+                                          N.ptr(accepted), N.ptr(diverged), N.ptr(ham), N.ptr(num_rejected),
+                                          C.byref(sink_s), None if h is None else C.byref(h), stream)
+            N.check(rc, 'hmcx_split_run_hyper')
 
     mass_ref = nm.ref()
     launch(0, windows[0][0], mass_ref, sink, False)
@@ -745,6 +799,23 @@ def _adapted_launches(lib, nt, nm, rng, nuts_s, scheme, q_init, q_cur, eps, Cn, 
         mass_ref = C.byref(masses[k])
     launch(windows[-1][1], S, mass_ref, sink, True)
     return trace[:, :D], windows
+
+
+def hyper_gamma_draws(seed, num_chains, iter_begin, iter_end, shapes, chain_offset=0, device='cuda'):
+    """The Philox-mode standard-gamma draws of the hyperprior kernels (hmcx_hyper_gamma_draws): (iter_end - iter_begin,
+    num_chains, K) fp64, entry [n, c, k] the Gamma(shapes[k], 1) draw of group k for chain chain_offset + c at
+    iteration iter_begin + n."""
+    N.require_cuda()
+    lib = N.load_library()
+    device = torch.device(device)
+    K = len(shapes)
+    sh = (C.c_double * max(K, 1))(*[float(v) for v in shapes])
+    out = torch.empty((int(iter_end) - int(iter_begin), int(num_chains), K), dtype=torch.float64, device=device)
+    with torch.cuda.device(device):
+        rc = lib.hmcx_hyper_gamma_draws(int(seed), int(chain_offset), int(num_chains), int(iter_begin), int(iter_end), K,
+                                        sh, N.ptr(out), N.stream_ptr(device))
+    N.check(rc, 'hmcx_hyper_gamma_draws')
+    return out
 
 
 def grad_log_prob(target, q, split=-1, want_grad=True, want_log_prob=True, device=None):

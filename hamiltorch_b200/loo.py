@@ -107,6 +107,25 @@ def _samples_block(samples, target):
     return x
 
 
+def _tau_block(samples, x, tau_out):
+    """The per-draw tau_out of the (C, n, D) block x as a (C, n) fp32 tensor on its device, or None (the target's).
+    Explicit ``tau_out``: (C, n), or (n,) for an (n, D) block / a single chain; otherwise an ``HMCResult`` of a run with
+    tau_out_prior brings its ``tau_out_trace`` (the same slots as its samples)."""
+    if tau_out is None:
+        tau_out = getattr(samples, 'tau_out_trace', None)
+        if tau_out is None:
+            return None
+    t = torch.as_tensor(tau_out).detach().to(device=x.device, dtype=torch.float32)
+    if t.dim() == 1 and x.shape[0] == 1:
+        t = t[None]
+    if tuple(t.shape) != (x.shape[0], x.shape[1]):
+        raise RuntimeError('loo: tau_out must hold one value per draw, (C, n) = (%d, %d), got %s'
+                           % (x.shape[0], x.shape[1], tuple(t.shape)))
+    if not bool((t > 0).all()) or not bool(torch.isfinite(t).all()):
+        raise ValueError('loo: tau_out must be positive and finite')
+    return t
+
+
 def _native_target(target, device):
     from .engine import native_target
     return native_target(target, device)
@@ -115,30 +134,40 @@ def _native_target(target, device):
 # ------------------------------------------------------------------------------------------------------------------
 # Pointwise log-likelihood
 # ------------------------------------------------------------------------------------------------------------------
-def _ll_rows(lib, nt, x, r0, r1, out):
-    """out[c, s, :] = ll of rows [r0, r1) (out a (C, n, r1 - r0) view with unit stride along its last dimension)."""
+def _ll_rows(lib, nt, x, r0, r1, out, tau=None):
+    """out[c, s, :] = ll of rows [r0, r1) (out a (C, n, r1 - r0) view with unit stride along its last dimension);
+    tau: the (C, n) per-draw tau_out, or None for the target's."""
     C_, n = int(x.shape[0]), int(x.shape[1])
-    rc = lib.hmcx_mlp_pointwise_ll(nt.ref(), N.ptr(x), x.stride(0), x.stride(1), C_, n, r0, r1, N.ptr(out),
-                                   out.stride(0), out.stride(1), N.stream_ptr(x.device))
-    N.check(rc, 'hmcx_mlp_pointwise_ll')
+    if tau is None:
+        rc = lib.hmcx_mlp_pointwise_ll(nt.ref(), N.ptr(x), x.stride(0), x.stride(1), C_, n, r0, r1, N.ptr(out),
+                                       out.stride(0), out.stride(1), N.stream_ptr(x.device))
+        N.check(rc, 'hmcx_mlp_pointwise_ll')
+        return
+    rc = lib.hmcx_mlp_pointwise_ll_tau(nt.ref(), N.ptr(x), x.stride(0), x.stride(1), C_, n, r0, r1, N.ptr(tau),
+                                       tau.stride(0), tau.stride(1), N.ptr(out), out.stride(0), out.stride(1),
+                                       N.stream_ptr(x.device))
+    N.check(rc, 'hmcx_mlp_pointwise_ll_tau')
 
 
-def pointwise_log_lik(samples, target):
+def pointwise_log_lik(samples, target, tau_out=None):
     """The (C, n, N) fp32 CUDA tensor ll[c, s, i] = log p(y_i | theta_{c,s}) of every draw and data point.
 
     ``samples``: what ``diagnostics.summary`` accepts (an ``HMCResult``, a (C, n, D) / (n, D) CUDA fp32 tensor, the list
     ``sample`` returns), refused in the same cases.  ``target``: an ``MLPTarget`` with data, or the list of split
     descriptors (points in split order).  Per point, with f the network output (O values) and tau = tau_out:
     regression sum_o -0.5 tau (f_o - y_o)^2 + 0.5 O log(tau / 2 pi); binary sum_o -BCEWithLogits(f_o, y_o);
-    multi-class log_softmax(f)[y]; LogSoftmax output f[y].  tau_out does not enter the classification densities."""
+    multi-class log_softmax(f)[y]; LogSoftmax output f[y].  tau_out does not enter the classification densities.
+    ``tau_out``: one noise precision per draw, (C, n) (or (n,) for one chain), for draws of a run with a tau_out
+    hyperprior; an ``HMCResult`` of such a run brings its ``tau_out_trace`` without it.  None: the target's tau_out."""
     x = _samples_block(samples, target)
+    tau = _tau_block(samples, x, tau_out)
     N.require_cuda()
     lib = N.load_library()
     nt = _native_target(target, x.device)
     Np = int(nt.mlp_struct.num_rows)
     out = torch.empty((x.shape[0], x.shape[1], Np), dtype=torch.float32, device=x.device)
     with torch.cuda.device(x.device):
-        _ll_rows(lib, nt, x, 0, Np, out)
+        _ll_rows(lib, nt, x, 0, Np, out, tau)
     return out
 
 
@@ -159,7 +188,7 @@ def _slab_points(lib, C_, n, Np, extra_per_point=0):
     return k
 
 
-def _pointwise_pass(x, target, r_eff):
+def _pointwise_pass(x, target, r_eff, tau=None):
     """(C, n, N) draws -> (pw (6, N) fp64, tail (N,) int32, flag (N,) int32, S, N)."""
     N.require_cuda()
     lib = N.load_library()
@@ -190,7 +219,7 @@ def _pointwise_pass(x, target, r_eff):
             if nt is None:
                 src, base = x, N.ptr(x)
             else:
-                _ll_rows(lib, nt, x, i0, i0 + kk, blk)
+                _ll_rows(lib, nt, x, i0, i0 + kk, blk, tau)
                 # the pass reads point i at column i of the block: the slab's block holds columns [i0, i0 + kk)
                 src, base = blk, C.c_void_p(blk.data_ptr() - 4 * i0)
             rc = lib.hmcx_loo_pass(base, src.stride(0), src.stride(1), C_, n, Np, i0, kk, float(r_eff), N.ptr(pw),
@@ -208,17 +237,18 @@ def _total(v):
     return s, se
 
 
-def _prepare(x, target, r_eff=None):
+def _prepare(x, target, r_eff=None, tau_out=None):
     if r_eff is not None:
         r_eff = _check_r_eff(r_eff)
     if target is None:
-        blk = _diag.as_block(x)
-    else:
-        blk = _samples_block(x, target)
-    return blk, r_eff
+        if tau_out is not None:
+            raise RuntimeError('loo: tau_out applies to samples with a target, not to a log-likelihood block')
+        return _diag.as_block(x), r_eff, None
+    blk = _samples_block(x, target)
+    return blk, r_eff, _tau_block(x, blk, tau_out)
 
 
-def psis_loo(x, target=None, r_eff=1.0):
+def psis_loo(x, target=None, r_eff=1.0, tau_out=None):
     """PSIS-LOO of a Bayesian NN on the GPU.
 
     ``x``: a log-likelihood block ll[c, s, i] -- a (C, n, N) or (n, N) CUDA fp32 tensor, e.g. ``pointwise_log_lik``'s
@@ -231,9 +261,11 @@ def psis_loo(x, target=None, r_eff=1.0):
     otherwise pareto_k = inf; the log-ratios are capped at 0 and normalised (lw); elpd_loo_i = logsumexp(lw + ll),
     p_loo_i = lppd_i - elpd_loo_i.  Totals are sums over points, se = sqrt(N) sd(pointwise).  A point with a non-finite
     draw gets NaN outputs (so the totals are NaN) and is counted in ``num_nonfinite``.  The same block gives the same
-    bits on every call, whatever the slab size.  Returns a ``LooResult``."""
-    blk, r_eff = _prepare(x, target, r_eff)
-    pw, tail, flag, S, Np = _pointwise_pass(blk, target, r_eff)
+    bits on every call, whatever the slab size.  ``tau_out``: per-draw noise precisions of samples from a run with a
+    tau_out hyperprior, as ``pointwise_log_lik`` takes them (an ``HMCResult`` brings its own trace).
+    Returns a ``LooResult``."""
+    blk, r_eff, tau = _prepare(x, target, r_eff, tau_out)
+    pw, tail, flag, S, Np = _pointwise_pass(blk, target, r_eff, tau)
     r = LooResult()
     r.pointwise, r.p_loo_i, r.pareto_k, r.lppd, r.tail_size = pw[0], pw[1], pw[2], pw[3], tail
     r.elpd_loo, r.se = _total(pw[0])
@@ -246,14 +278,14 @@ def psis_loo(x, target=None, r_eff=1.0):
     return r
 
 
-def waic(x, target=None):
+def waic(x, target=None, tau_out=None):
     """WAIC of a Bayesian NN on the GPU (Watanabe 2010, in the elpd scale of Vehtari et al. 2017): per point
     lppd_i = logsumexp(ll) - log S, p_waic_i = var(ll) over the S pooled draws (ddof 1), elpd_waic_i = lppd_i - p_waic_i;
     totals are sums, se = sqrt(N) sd(pointwise), waic = -2 elpd_waic.  ``x`` / ``target`` as ``psis_loo``.
     ``num_p_waic_warn`` counts points with p_waic_i > 0.4, where WAIC is known to be unreliable (prefer PSIS-LOO).
-    Returns a ``WaicResult``."""
-    blk, _ = _prepare(x, target)
-    pw, _, flag, S, Np = _pointwise_pass(blk, target, 1.0)
+    ``tau_out`` as ``psis_loo``.  Returns a ``WaicResult``."""
+    blk, _, tau = _prepare(x, target, tau_out=tau_out)
+    pw, _, flag, S, Np = _pointwise_pass(blk, target, 1.0, tau)
     r = WaicResult()
     r.pointwise, r.p_waic, r.lppd = pw[5], pw[4], pw[3]
     r.elpd_waic, r.se = _total(pw[5])

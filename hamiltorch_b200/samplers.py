@@ -14,6 +14,7 @@ What differs by design
     many-chains entry (the engine's native shape), ``sample`` is the one-chain drop-in.
 """
 from enum import Enum
+import math
 
 import torch
 
@@ -245,14 +246,21 @@ def _check_sample_args(params_init_dim_ok, num_samples, burn, sampler):
         raise RuntimeError('burn must be greater than 0 for NUTS.')             # :933-934
 
 
-def _draw_reference_stream(dim, num_samples, device, num_perm=0, blocks=None):
+def _draw_reference_stream(dim, num_samples, device, num_perm=0, blocks=None, gamma_shapes=None):
     """Pre-draw one chain's randoms from torch's GLOBAL generators in exactly the order the reference consumes
     them (SURVEY.md section 8c fact 3): per iteration the momentum normals -- ``Normal(zeros_like(params),
     ones_like(params)).sample()`` (:186, :202), i.e. the generator of params' device -- then ``torch.rand(1)`` on
-    the CPU generator (:1004).  Valid while no LogProbError occurs (that skips the iteration's rand(1))."""
+    the CPU generator (:1004).  Valid while no LogProbError occurs (that skips the iteration's rand(1)).
+    ``gamma_shapes`` (hyperpriors, (K,) fp64 with 0 for a fixed group): after the iteration's rand(1), ONE
+    ``torch._standard_gamma`` call on the CPU generator over the sampled groups' posterior shapes in group order; the
+    draws come back as the last element, (S, K) fp64 with 0 at the fixed groups."""
     z = torch.empty((num_samples, dim), dtype=torch.float32, device=device)
     logu = torch.empty(num_samples, dtype=torch.float32)
     perms = torch.empty((num_samples, num_perm), dtype=torch.int32) if num_perm else None
+    gam = None
+    if gamma_shapes is not None:
+        gam = torch.zeros((num_samples, gamma_shapes.numel()), dtype=torch.float64)
+        live = gamma_shapes > 0
     for n in range(num_samples):
         if blocks:                                          # block-list mass: one draw per block (:188-197)
             z[n] = torch.cat([torch.randn(b, dtype=torch.float32, device=device) for b in blocks])
@@ -261,16 +269,18 @@ def _draw_reference_stream(dim, num_samples, device, num_perm=0, blocks=None):
         if num_perm:
             perms[n] = torch.randperm(num_perm)             # SPLITTING_RAND: once per trajectory (:550)
         logu[n] = torch.log(torch.rand(1))[0]
-    if num_perm:
-        return z, logu, perms
-    return z, logu
+        if gam is not None:
+            gam[n, live] = torch._standard_gamma(gamma_shapes[live])
+    out = (z, logu) + ((perms,) if num_perm else ())
+    return out + ((gam,) if gam is not None else ())
 
 
 def sample(log_prob_func, params_init, num_samples=10, num_steps_per_sample=10, step_size=0.1, burn=0, jitter=None,
            inv_mass=None, normalizing_const=1., softabs_const=None, explicit_binding_const=100,
            fixed_point_threshold=1e-5, fixed_point_max_iterations=1000, jitter_max_tries=10, sampler=Sampler.HMC,
            integrator=Integrator.IMPLICIT, metric=Metric.HESSIAN, debug=False, desired_accept_rate=0.8,
-           store_on_GPU=True, pass_grad=None, verbose=True, *, rng='reference', seed=None):
+           store_on_GPU=True, pass_grad=None, verbose=True, *, rng='reference', seed=None, tau_prior=None,
+           tau_out_prior=None):
     """Drop-in for ``hamiltorch.sample`` (samplers.py:850-1091): ONE chain, same arguments, same return value --
     a list of ``num_samples - burn`` detached (D,) tensors whose element 0 is ``params_init`` (:959), plus the
     adapted step size (NUTS) or the acceptance rate when ``debug == 2`` (:1086-1089).
@@ -278,6 +288,11 @@ def sample(log_prob_func, params_init, num_samples=10, num_steps_per_sample=10, 
     rng='reference' (default): the chain consumes torch's global random stream exactly like the reference, so
         after ``set_random_seed(s)`` the returned samples equal the reference's (to fp32 summation order in the
         Hamiltonian).  rng='philox': in-kernel counter RNG keyed by ``seed`` (default: drawn from torch's RNG).
+    ``tau_prior`` / ``tau_out_prior``: Gamma hyperpriors on the precisions of a Bayesian-NN target (see
+    ``sample_chains``).  The call then returns ``(samples, hyper)`` -- ``hyper`` a dict of the retained slots'
+    ``'tau_list'`` (S-burn, 2L) and ``'tau_out'`` (S-burn,) -- and ``(samples, hyper, value)`` with ``debug == 2``.
+    With rng='reference' the gamma draws come from torch's CPU generator after each iteration's rand(1)
+    (``_draw_reference_stream``), so ``set_random_seed`` makes the call reproducible.
     """
     _check_sample_args(params_init.dim() == 1, num_samples, burn, sampler)
     _require_target(log_prob_func)
@@ -292,7 +307,8 @@ def sample(log_prob_func, params_init, num_samples=10, num_steps_per_sample=10, 
                       fixed_point_max_iterations, jitter_max_tries, sampler, integrator, metric,
                       desired_accept_rate, rng=rng, seed=seed, record_ham=(debug == 1),
                       sink=dict(host_samples=True) if (
-                          not store_on_GPU and _sink_supported(log_prob_func, sampler, integrator, inv_mass)) else None)
+                          not store_on_GPU and _sink_supported(log_prob_func, sampler, integrator, inv_mass)) else None,
+                      hyper=_hyper_groups(log_prob_func, sampler, tau_prior, tau_out_prior))
     if not res.samples_padded.is_cuda:
         torch.cuda.current_stream().synchronize()       # the kernel wrote the samples into pinned host memory
     nuts = sampler == Sampler.HMC_NUTS
@@ -311,11 +327,14 @@ def sample(log_prob_func, params_init, num_samples=10, num_steps_per_sample=10, 
         print('Final Adapted Step Size: ', final_eps)                                              # :1035
     if verbose:
         print('Acceptance Rate {:.2f}'.format(1 - num_rejected / num_samples))                     # :1085
+    extra = ()
+    if getattr(res, 'tau_list_trace', None) is not None:
+        extra = ({'tau_list': res.tau_list_trace[0], 'tau_out': res.tau_out_trace[0]},)
     if nuts and debug == 2:
-        return ret, final_eps
+        return (ret,) + extra + (final_eps,)
     elif debug == 2:
-        return ret, 1 - num_rejected / num_samples
-    return ret
+        return (ret,) + extra + (1 - num_rejected / num_samples,)
+    return (ret,) + extra if extra else ret
 
 
 def sample_chains(log_prob_func, params_init, num_samples=10, num_steps_per_sample=10, step_size=0.1, burn=0,
@@ -324,7 +343,8 @@ def sample_chains(log_prob_func, params_init, num_samples=10, num_steps_per_samp
                   sampler=Sampler.HMC, integrator=Integrator.IMPLICIT, metric=Metric.HESSIAN,
                   desired_accept_rate=0.8, rng='philox', seed=0, chain_offset=0, normals=None, log_uniforms=None,
                   record_ham=False, out=None, perms=None, uniforms=None, thin=1, moments=False, keep_samples=True,
-                  store_on_GPU=True, host_windows=0, adapt_mass=False, mass_pool=None):
+                  store_on_GPU=True, host_windows=0, adapt_mass=False, mass_pool=None, tau_prior=None,
+                  tau_out_prior=None, gammas=None):
     """The engine's native entry: C independent chains at once.  ``params_init`` is (C, D); every chain gets the
     reference's ``sample`` semantics.  Returns an ``engine.HMCResult`` whose ``.samples`` is (C, S-burn, D) on the
     GPU (row c = what ``sample`` would have returned for chain c, stacked).
@@ -356,6 +376,16 @@ def sample_chains(log_prob_func, params_init, num_samples=10, num_steps_per_samp
     mass used after warm-up --, ``.inv_mass_trace`` (K, D), one row per window, and ``.mass_windows``, the K (a, b)
     iteration ranges.  ``mass_pool`` (multi-GPU; ``distributed.sample_chains_sharded`` passes it) maps each (C_local, ld)
     window sum to the sum of all chains in global order, so that every rank adapts the same mass.
+
+    Hyperpriors (an ``MLPRegression`` or a split list of them, HMC / HMC_NUTS; DESIGN §3.15): ``tau_prior`` is ``(a, b)``
+    for every parameter tensor or a list of 2L entries in tau_list order, each ``(a, b)`` or ``None`` (fixed at its
+    tau_list value); ``tau_out_prior`` is ``(a, b)`` for the regression noise precision.  Gamma(shape a, rate b); every
+    iteration, after the MH step, each precision is drawn from its Gamma conditional given the weights (and, for tau_out,
+    the sum of squared errors over all data rows) inside the kernel, and the next iteration samples with the new values.
+    They start from tau_list / tau_out.  ``rng='injected'`` also takes ``gammas`` (S, C, 2L + 1) fp64: the
+    standard-gamma draw of every group (tensors, then tau_out).  The result gains ``.tau_list_trace`` (C, keep, 2L) and
+    ``.tau_out_trace`` (C, keep) for the retained sample slots (slot 0 = the initial values; on the device even with
+    ``store_on_GPU=False``) and the final state ``.tau_list_final`` / ``.tau_out_final``.
     """
     if params_init.dim() != 2:
         raise RuntimeError('sample_chains: params_init must be (num_chains, D)')
@@ -363,6 +393,7 @@ def sample_chains(log_prob_func, params_init, num_samples=10, num_steps_per_samp
     _require_target(log_prob_func)
     if adapt_mass:
         _check_adapt_mass(log_prob_func, sampler, integrator, inv_mass, burn, host_windows)
+    hyper = _hyper_groups(log_prob_func, sampler, tau_prior, tau_out_prior)
     return _run_chains(log_prob_func, params_init, num_samples, num_steps_per_sample, step_size, burn, jitter,
                        inv_mass, softabs_const, explicit_binding_const, fixed_point_threshold,
                        fixed_point_max_iterations, jitter_max_tries, sampler, integrator, metric,
@@ -371,7 +402,58 @@ def sample_chains(log_prob_func, params_init, num_samples=10, num_steps_per_samp
                        injected_uniforms=uniforms,
                        sink=dict(thin=thin, moments=moments, keep_samples=keep_samples, host_samples=not store_on_GPU,
                                  host_windows=host_windows, **(dict(adapt_mass=True, mass_pool=mass_pool)
-                                                               if adapt_mass else {})))
+                                                               if adapt_mass else {})),
+                       hyper=hyper, gammas=gammas)
+
+
+def _check_gamma(ab, what):
+    try:
+        a, b = (float(v) for v in ab)
+    except (TypeError, ValueError):
+        raise ValueError('%s must be a pair (a, b), got %r' % (what, ab))
+    if not (0 < a < math.inf and 0 < b < math.inf):
+        raise ValueError('%s: Gamma(a, b) needs finite a > 0 and b > 0, got (%r, %r)' % (what, a, b))
+    return a, b
+
+
+def _hyper_groups(log_prob_func, sampler, tau_prior, tau_out_prior):
+    """tau_prior / tau_out_prior -> the 2L + 1 entries of engine.hmc_run's ``hyper`` (None: no hyperprior), checked
+    before any CUDA work."""
+    if tau_prior is None and tau_out_prior is None:
+        return None
+    descs = log_prob_func if isinstance(log_prob_func, list) else [log_prob_func]
+    if not descs or not all(isinstance(d, T.MLPRegression) for d in descs):
+        raise NotImplementedError('hyperpriors on tau_list / tau_out: Bayesian-NN targets only (an MLPRegression or a '
+                                  'list of them)')
+    if sampler not in (Sampler.HMC, Sampler.HMC_NUTS):
+        raise NotImplementedError('hyperpriors on tau_list / tau_out: sampler HMC or HMC_NUTS')
+    K = 2 * descs[0].num_layers
+    if tau_prior is None:
+        groups = [None] * K
+    elif isinstance(tau_prior, list):
+        if len(tau_prior) != K:
+            raise ValueError('tau_prior needs one entry per parameter tensor (%d), got %d' % (K, len(tau_prior)))
+        groups = [None if ab is None else _check_gamma(ab, 'tau_prior[%d]' % k) for k, ab in enumerate(tau_prior)]
+    else:
+        groups = [_check_gamma(tau_prior, 'tau_prior')] * K
+    if tau_out_prior is None:
+        groups.append(None)
+    else:
+        if descs[0].loss_id != T.LOSS_REGRESSION:
+            raise NotImplementedError('tau_out_prior: regression only -- the classification losses use tau_out as a '
+                                      'tempering factor, not as a noise precision')
+        if descs[0].x is None:
+            raise RuntimeError('tau_out_prior needs data (x is None samples the prior)')
+        groups.append(_check_gamma(tau_out_prior, 'tau_out_prior'))
+    return groups
+
+
+def _reference_gamma_shapes(log_prob_func, hyper):
+    """The posterior shapes a_k + n_k / 2 and a_o + N O / 2 of the sampled groups, 0 at the fixed ones (fp64)."""
+    descs = log_prob_func if isinstance(log_prob_func, list) else [log_prob_func]
+    n_obs = sum(d.x.shape[0] for d in descs if d.x is not None) * descs[0].widths[-1]
+    sizes = list(descs[0].sizes) + [n_obs]
+    return torch.tensor([0.0 if ab is None else ab[0] + 0.5 * n for ab, n in zip(hyper, sizes)], dtype=torch.float64)
 
 
 def _check_adapt_mass(log_prob_func, sampler, integrator, inv_mass, burn, host_windows):
@@ -393,8 +475,10 @@ def _run_chains(log_prob_func, q0, num_samples, L, step_size, burn, jitter, inv_
                 explicit_binding_const, fixed_point_threshold, fixed_point_max_iterations, jitter_max_tries,
                 sampler, integrator, metric, desired_accept_rate, rng='philox', seed=None, chain_offset=0,
                 normals=None, log_uniforms=None, record_ham=False, out=None, injected_perms=None,
-                injected_uniforms=None, sink=None):
+                injected_uniforms=None, sink=None, hyper=None, gammas=None):
     nuts = sampler == Sampler.HMC_NUTS
+    hyper_kw = {} if hyper is None else dict(hyper=hyper)
+    gshapes = None if hyper is None else _reference_gamma_shapes(log_prob_func, hyper)
     sink = sink or {}
     if (sink.get('thin', 1) != 1 or sink.get('moments') or not sink.get('keep_samples', True) or
             sink.get('host_samples')) and not _sink_supported(log_prob_func, sampler, integrator, inv_mass):
@@ -411,9 +495,12 @@ def _run_chains(log_prob_func, q0, num_samples, L, step_size, burn, jitter, inv_
         if rng == 'reference':
             if q0.shape[0] != 1:
                 raise RuntimeError("rng='reference' replays torch's global stream and is defined for one chain")
-            z, logu = _draw_reference_stream(D, num_samples, q0.device,
-                                             blocks=[b.shape[0] for b in inv_mass] if isinstance(inv_mass, list) else None)
+            drawn = _draw_reference_stream(D, num_samples, q0.device, gamma_shapes=gshapes,
+                                           blocks=[b.shape[0] for b in inv_mass] if isinstance(inv_mass, list) else None)
+            z, logu = drawn[0], drawn[1]
             normals, log_uniforms = z.unsqueeze(1), logu.unsqueeze(1)
+            if hyper is not None:
+                gammas = drawn[-1].unsqueeze(1)
         elif rng == 'injected':
             if normals is None or log_uniforms is None:
                 raise RuntimeError("rng='injected' needs normals and log_uniforms")
@@ -426,7 +513,8 @@ def _run_chains(log_prob_func, q0, num_samples, L, step_size, burn, jitter, inv_
         return engine.hmc_run(log_prob_func, q0, num_samples, L, step_size, burn=burn, inv_mass=inv_mass, nuts=nuts,
                               desired_accept_rate=desired_accept_rate, seed=seed or 0, chain_offset=chain_offset,
                               normals=normals, log_uniforms=log_uniforms, record_ham=record_ham, out=out,
-                              scheme=N.SCHEME_PLAIN if isinstance(log_prob_func, T.MLPRegression) else None, **sink)
+                              scheme=N.SCHEME_PLAIN if isinstance(log_prob_func, T.MLPRegression) else None,
+                              gammas=gammas, **hyper_kw, **sink)
     if sampler == Sampler.HMC:
         if type(log_prob_func) is not list:
             raise RuntimeError('For splitting log_prob_func must be list of functions')            # :466-467
@@ -446,9 +534,11 @@ def _run_chains(log_prob_func, q0, num_samples, L, step_size, burn, jitter, inv_
         if rng == 'reference':
             if q0.shape[0] != 1:
                 raise RuntimeError("rng='reference' replays torch's global stream and is defined for one chain")
-            drawn = _draw_reference_stream(D, num_samples, q0.device,
-                                           M if integrator == Integrator.SPLITTING_RAND else 0)
-            z, logu, pm = drawn if len(drawn) == 3 else (drawn[0], drawn[1], None)
+            rand_perm = integrator == Integrator.SPLITTING_RAND
+            drawn = _draw_reference_stream(D, num_samples, q0.device, M if rand_perm else 0, gamma_shapes=gshapes)
+            z, logu, pm = drawn[0], drawn[1], (drawn[2] if rand_perm else None)
+            if hyper is not None:
+                gammas = drawn[-1].unsqueeze(1)
             normals, log_uniforms = z.unsqueeze(1), logu.unsqueeze(1)
             perms = None if pm is None else pm.unsqueeze(1)
         elif rng == 'injected':
@@ -464,7 +554,9 @@ def _run_chains(log_prob_func, q0, num_samples, L, step_size, burn, jitter, inv_
         return engine.hmc_run(log_prob_func, q0, num_samples, L, step_size, burn=burn, inv_mass=inv_mass, nuts=nuts,
                               desired_accept_rate=desired_accept_rate, seed=seed or 0, chain_offset=chain_offset,
                               normals=normals, log_uniforms=log_uniforms, record_ham=record_ham, out=out,
-                              scheme=scheme, perms=perms, **sink)
+                              scheme=scheme, perms=perms, gammas=gammas, **hyper_kw, **sink)
+    if hyper is not None:
+        raise NotImplementedError('hyperpriors on tau_list / tau_out: sampler HMC or HMC_NUTS')
     if sampler == Sampler.RMHMC and integrator in (Integrator.EXPLICIT, Integrator.IMPLICIT):
         if isinstance(log_prob_func, list) or not isinstance(log_prob_func, (T.Funnel, T.GaussianIso, T.GaussianDiag,
                                                                              T.GaussianFull)):

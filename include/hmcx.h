@@ -430,6 +430,57 @@ int hmcx_split_run_sink(const hmcx_target_t* target, const hmcx_mass_t* mass, co
                         int32_t* num_rejected, const hmcx_sink_t* sink, void* stream);
 
 /*
+ * Gamma hyperpriors on the precisions of a Bayesian NN (hmcx_split_run_hyper).  Group k < 2L is parameter tensor k in
+ * tau_list order (each Linear's weight, then its bias): w_k ~ Normal(0, tau_k^-1/2), tau_k ~ Gamma(a[k], b[k]) (shape,
+ * rate); group 2L is the regression likelihood's precision tau_out ~ Gamma(a[2L], b[2L]).  Every iteration n, after the MH
+ * step gives q_n, each sampled group is drawn from its conditional
+ *   tau_k ~ Gamma(a_k + n_k / 2, b_k + |w_k|^2 / 2),   tau_out ~ Gamma(a_o + N O / 2, b_o + SSE(q_n) / 2)
+ * (n_k = the tensor's size, N = data rows over all splits, O = outputs; |w_k|^2 a fixed-order fp64 sum, SSE the sum over
+ * splits of the MH evaluation's squared errors), and iteration n + 1 uses them.  Draws: PHILOX mode Marsaglia-Tsang in fp64
+ * on its own counter stream, keyed by (seed, chain_offset + c, n, k, attempt) as hmcx_hyper_gamma_draws writes them;
+ * INJECTED mode the standard-gamma draws `gammas`; tau_k = (float)(g / rate).
+ *   sampled[k]     non-zero: group k is Gibbs-updated (a[k], b[k] > 0 and finite); zero: fixed at the target's value
+ *   tau, tau_out   [C, 2L] / [C] device in/out: the chains' current precisions (initialise them to the target's tau_list /
+ *                  tau_out); windows of iterations chain through them
+ *   tau_trace, tau_out_trace   optional [C, keep, 2L] / [C, keep] device: the precisions of every retained sample slot
+ *                  (the sink's slots, thinned alike; slot 0 = the initial values)
+ *   gammas         INJECTED: [iter_end - iter_begin, C, 2L + 1] fp64 device, entry k of row (n, c) the Gamma(shape_k, 1)
+ *                  draw of group k (entries of fixed groups are not read)
+ */
+#define HMCX_HYPER_GROUPS (2 * HMCX_MLP_MAX_LAYERS + 1)
+typedef struct hmcx_hyper {
+    int32_t sampled[HMCX_HYPER_GROUPS];
+    double  a[HMCX_HYPER_GROUPS];
+    double  b[HMCX_HYPER_GROUPS];
+    float*  tau;
+    float*  tau_out;
+    float*  tau_trace;
+    float*  tau_out_trace;
+    const double* gammas;
+} hmcx_hyper_t;
+
+/* hmcx_split_run_sink with Gamma hyperpriors (hyper == NULL: identical to hmcx_split_run_sink; sink == NULL with a hyper:
+ * a thin = 1 sink).  Checked before any CUDA work: a sampled group outside [0, 2L], a or b not in (0, inf), NULL tau /
+ * tau_out, INJECTED without gammas, a tau_out prior without data: HMCX_ERR_INVALID_ARG; a tau_out prior with a
+ * classification loss (tau_out tempers those likelihoods, it is not a noise precision): HMCX_ERR_UNSUPPORTED.  The
+ * proposal's log p and any gradient carried into the next trajectory belong to the old precisions: after each update the
+ * kernel re-evaluates log p(q_n) (one forward pass) and starts the next trajectory with a fresh gradient. */
+int hmcx_split_run_hyper(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmcx_rng_t* rng,
+                         const hmcx_nuts_t* nuts, int32_t scheme,
+                         const float* q_init, float* q_cur, float* eps,
+                         int32_t C, int32_t ld, int32_t L, int32_t num_samples, int32_t burn,
+                         int32_t iter_begin, int32_t iter_end,
+                         float* samples_out, uint8_t* accept_out, uint8_t* diverged_out, float* ham_out,
+                         int32_t* num_rejected, const hmcx_sink_t* sink, const hmcx_hyper_t* hyper, void* stream);
+
+/* The PHILOX-mode standard-gamma draws of hmcx_split_run_hyper, from the same device function: out[n - iter_begin, c, k] =
+ * the Gamma(shapes[k], 1) draw of group k, chain chain_offset + c, iteration n.  shapes: HOST array of K <=
+ * HMCX_HYPER_GROUPS values in (0, inf); out: [iter_end - iter_begin, C, K] fp64 device.  Other arguments out of range:
+ * HMCX_ERR_INVALID_ARG. */
+int hmcx_hyper_gamma_draws(uint64_t seed, uint64_t chain_offset, int32_t C, int32_t iter_begin, int32_t iter_end,
+                           int32_t K, const double* shapes, double* out, void* stream);
+
+/*
  * hmcx_adapt_diag_mass (ABI v11): the pooled diagonal mass estimate at the end of a warm-up window (Stan's windowed
  * adaptation, regularised as Stan does) and the restart of the dual averaging that follows it.  One pass, fixed order, no
  * atomics.  Inputs: the per-chain compensated sums of a window of n >= 2 draws, [C, ld] each, as a sink launch with
@@ -544,6 +595,15 @@ int hmcx_rank_indicator(const float* x, int64_t chain_stride, int64_t draw_strid
 int hmcx_mlp_pointwise_ll(const hmcx_target_t* target, const float* samples, int64_t chain_stride, int64_t draw_stride,
                           int32_t C, int32_t n, int32_t row_begin, int32_t row_end, float* ll_out,
                           int64_t ll_chain_stride, int64_t ll_draw_stride, void* stream);
+/* hmcx_mlp_pointwise_ll with a per-draw tau_out (the draws of a run with a tau_out hyperprior, hmcx_split_run_hyper):
+ * draw (c, s) uses tau_out[c*tau_chain_stride + s*tau_draw_stride] (fp32 device) in the regression density, its constant
+ * 0.5 O log(tau / 2 pi) evaluated in fp64 and rounded to fp32 as hmcx_mlp_pointwise_ll does for the target's tau_out.
+ * tau_out == NULL: identical to hmcx_mlp_pointwise_ll.  Classification losses do not read it.  Negative tau strides:
+ * HMCX_ERR_INVALID_ARG; otherwise the checks of hmcx_mlp_pointwise_ll. */
+int hmcx_mlp_pointwise_ll_tau(const hmcx_target_t* target, const float* samples, int64_t chain_stride,
+                              int64_t draw_stride, int32_t C, int32_t n, int32_t row_begin, int32_t row_end,
+                              const float* tau_out, int64_t tau_chain_stride, int64_t tau_draw_stride, float* ll_out,
+                              int64_t ll_chain_stride, int64_t ll_draw_stride, void* stream);
 size_t hmcx_loo_workspace_bytes(int32_t C, int32_t n, int32_t k);
 int hmcx_loo_pass(const float* ll, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t N,
                   int32_t i0, int32_t k, double r_eff, double* pointwise, int32_t* tail_size, int32_t* nonfinite,
