@@ -168,6 +168,14 @@ _PROTOS = {
     'hmcx_loo_workspace_bytes': (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
     'hmcx_loo_pass': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                 C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    'hmcx_mlp_pointwise_out': (C.c_int, [C.POINTER(TargetStruct), C.c_void_p, C.c_int64, C.c_int64, C.c_int32,
+                                         C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int64, C.c_int64,
+                                         C.c_void_p]),
+    'hmcx_pred_workspace_bytes': (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    'hmcx_pred_pass': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                 C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
+                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    'hmcx_pred_totals': (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p]),
 }
 
 DIAG_LAG_BLOCK = 32                     # HMCX_DIAG_LAG_BLOCK: lags per hmcx_diag_acov pass

@@ -58,6 +58,13 @@ int mlp_pointwise_ll(const hmcx_target_t*, const float*, long long, long long, i
 size_t loo_workspace_bytes(int, int, int);
 int loo_pass(const float*, long long, long long, int, int, int, int, int, double, double*, int*, int*, void*,
              cudaStream_t);
+int mlp_pointwise_out(const hmcx_target_t*, const float*, long long, long long, int, int, int, int, float*, long long,
+                      long long, cudaStream_t);
+size_t pred_workspace_bytes(int, int, int, int);
+size_t pred_scan_smem(int, int);
+int pred_pass(const float*, long long, long long, int, int, int, int, const float*, const float*, long long, long long,
+              int, int, int, double*, double*, int*, double*, void*, cudaStream_t);
+int pred_totals(const double*, int, int, double*, cudaStream_t);
 }  // namespace hmcx
 
 static inline bool has_mu_chain(const hmcx_nuts_t* nuts) { return nuts && nuts->enabled && nuts->mu_chain; }
@@ -387,6 +394,53 @@ int hmcx_loo_pass(const float* ll, int64_t chain_stride, int64_t draw_stride, in
         return HMCX_ERR_INVALID_ARG;
     return hmcx::loo_pass(ll, chain_stride, draw_stride, C, n, N, i0, k, r_eff, pointwise, tail_size, nonfinite,
                           workspace, (cudaStream_t)stream);
+}
+
+int hmcx_mlp_pointwise_out(const hmcx_target_t* target, const float* samples, int64_t chain_stride,
+                           int64_t draw_stride, int32_t C, int32_t n, int32_t row_begin, int32_t row_end, float* out,
+                           int64_t out_chain_stride, int64_t out_draw_stride, void* stream) {
+    if (!target) return HMCX_ERR_INVALID_ARG;
+    if (target->kind != HMCX_TARGET_MLP) return HMCX_ERR_UNSUPPORTED;
+    return hmcx::mlp_pointwise_out(target, samples, chain_stride, draw_stride, C, n, row_begin, row_end, out,
+                                   out_chain_stride, out_draw_stride, (cudaStream_t)stream);
+}
+
+static inline bool pred_shape_ok(int32_t C, int32_t n, int32_t k) {
+    return C >= 1 && n >= 1 && (int64_t)C * n <= 0x7fffffffLL && k >= 1 && n <= (0x7fffffff - 64) / 2;
+}
+
+static inline int pred_form(int32_t loss) {
+    return loss == HMCX_LOSS_MULTICLASS_LOGSOFTMAX ? HMCX_LOSS_MULTICLASS : loss;
+}
+
+static inline bool pred_loss_ok(int32_t loss) {
+    return loss >= HMCX_LOSS_REGRESSION && loss <= HMCX_LOSS_MULTICLASS_LOGSOFTMAX;
+}
+
+size_t hmcx_pred_workspace_bytes(int32_t C, int32_t n, int32_t O, int32_t loss, int32_t k) {
+    if (!pred_shape_ok(C, n, k) || O < 1 || O > 0xffffff || !pred_loss_ok(loss)) return 0;
+    return hmcx::pred_workspace_bytes(n, O, pred_form(loss), k);
+}
+
+int hmcx_pred_pass(const float* f, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t O,
+                   int32_t loss, const float* y, const float* tau_out, int64_t tau_chain_stride, int64_t tau_draw_stride,
+                   int32_t N, int32_t i0, int32_t k, double* pointwise, double* per_output, int32_t* nonfinite,
+                   double* partials, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!f || !y || !pointwise || !per_output || !nonfinite || !partials || !workspace || chain_stride < 0 ||
+        draw_stride < 0 || !pred_shape_ok(C, n, k) || O < 1 || O > 0xffffff || N < 1 || i0 < 0 ||
+        (int64_t)i0 + k > N || !pred_loss_ok(loss) ||
+        (loss == HMCX_LOSS_REGRESSION && (!tau_out || tau_chain_stride < 0 || tau_draw_stride < 0)) ||
+        workspace_bytes < hmcx::pred_workspace_bytes(n, O, pred_form(loss), k))
+        return HMCX_ERR_INVALID_ARG;
+    if (hmcx::pred_scan_smem(pred_form(loss), O) > 227 * 1024) return HMCX_ERR_UNSUPPORTED;
+    return hmcx::pred_pass(f, chain_stride, draw_stride, C, n, O, pred_form(loss), y, tau_out, tau_chain_stride,
+                           tau_draw_stride, N, i0, k, pointwise, per_output, nonfinite, partials, workspace,
+                           (cudaStream_t)stream);
+}
+
+int hmcx_pred_totals(const double* partials, int32_t n, int32_t N, double* totals, void* stream) {
+    if (!partials || !totals || n < 1 || n > (0x7fffffff - 64) / 2 || N < 1) return HMCX_ERR_INVALID_ARG;
+    return hmcx::pred_totals(partials, n, N, totals, (cudaStream_t)stream);
 }
 
 int hmcx_adapt_diag_mass(float* sum, float* sumsq, float* sum_lo, float* sumsq_lo, int32_t C, int32_t ld, int32_t D,

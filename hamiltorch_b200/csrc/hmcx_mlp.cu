@@ -1822,6 +1822,57 @@ mlp_ll_tau_kernel(const MlpDev m, const float* __restrict__ samples, long long c
     }
 }
 
+// out[c, s, i - r_begin, :] = the network outputs of draw (c, s) at the rows [r_begin, r_end) (held-out evaluation,
+// DESIGN.md 3.16): the tile loop of mlp_ll_kernel, the outputs of mlp_predict_kernel -- the same forward, and a
+// LogSoftmax output layer applied by the loss stage of mlp_log_prob -- so the values are predict_model's, bit for bit.
+__global__ void __launch_bounds__(MLP_THREADS, 1)
+mlp_out_kernel(const MlpDev m, const float* __restrict__ samples, long long cs, long long ds, int n, int r_begin,
+               int r_end, float* __restrict__ out, long long ocs, long long ods) {
+    extern __shared__ __align__(128) float sm[];
+    __shared__ __align__(8) uint64_t s_bars[3];
+    float* q = sm;
+    float* tile = sm + m.tile_base;
+    const int c = blockIdx.x / n, s = blockIdx.x - c * n;
+    const float* qin = samples + (long long)c * cs + (long long)s * ds;
+    for (int i = threadIdx.x; i < m.Dp; i += MLP_THREADS) q[i] = i < m.D ? qin[i] : 0.0f;
+    __syncthreads();
+    const int nL = m.n[m.L];
+    float* orow = out + (long long)c * ocs + (long long)s * ods - (long long)r_begin * nL;
+    TcCtx tc = {};
+    TcEpi te;
+    if (m.tc) {
+        tc_init(tc, s_bars);
+        tc_epi_begin(m, q, te);
+        fence_async_smem();
+        __syncthreads();
+    }
+    for (int sp = 0; sp < m.M; ++sp) {
+        if (m.sb[sp + 1] <= r_begin || m.sb[sp] >= r_end) continue;
+        int ti = 0;
+        for (int r0 = m.sb[sp]; r0 < m.sb[sp + 1] && r0 < r_end; r0 += m.T, ++ti) {
+            if (r0 + m.T <= r_begin) continue;
+            const int cnt = min(m.T, m.sb[sp + 1] - r0);
+            if (m.tc) {
+                float act[16];
+                tc_prefetch_fwd(m, tile, tc, m.tb[sp] + ti, 0);
+                tc_prefetch_y(m, tile, r0, cnt);
+                tc_forward_tile(m, q, tile, tc, te, act, 0);
+            } else {
+                mlp_forward_tile(m, q, tile, r0, cnt);
+            }
+            if (m.loss == HMCX_LOSS_MULTICLASS_LOGSOFTMAX) {
+                mlp_loss_tile(m, tile + m.aoff[m.L], nullptr, r0, cnt, m.sb[sp + 1] - m.sb[sp], true,
+                              m.tc ? tile + m.tc_yraw : nullptr);
+                __syncthreads();
+            }
+            const int lo = max(r0, r_begin) - r0, hi = min(r0 + cnt, r_end) - r0;
+            for (int e = lo * nL + threadIdx.x; e < hi * nL; e += MLP_THREADS)
+                orow[(long long)r0 * nL + e] = tile[m.aoff[m.L] + e];
+            __syncthreads();
+        }
+    }
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------
@@ -2103,6 +2154,22 @@ int mlp_pointwise_ll(const hmcx_target_t* target, const float* samples, long lon
     const double tau_t = (double)target->mlp->tau_out;
     const float ll_const = (float)(0.5 * m.n[m.L] * log(tau_t / (2.0 * 3.14159265358979323846)));
     mlp_ll_kernel<<<C * n, MLP_THREADS, smem, st>>>(m, samples, cs, ds, n, r_begin, r_end, ll_const, ll, lcs, lds);
+    return cuda_status();
+}
+
+int mlp_pointwise_out(const hmcx_target_t* target, const float* samples, long long cs, long long ds, int C, int n,
+                      int r_begin, int r_end, float* out, long long ocs, long long ods, cudaStream_t st) {
+    MlpDev m = {};
+    int rc = fill_mlp(target, m);
+    if (rc != HMCX_OK) return rc;
+    if (!samples || !out || C < 1 || n < 1 || (long long)C * n > 0x7fffffffLL || cs < 0 || ds < 0 || ocs < 0 ||
+        ods < 0 || !m.has_data || r_begin < 0 || r_end > m.N || r_begin >= r_end)
+        return HMCX_ERR_INVALID_ARG;
+    if (!mlp_pick_tile(m, 1, target->mlp->tensor_cores != HMCX_MLP_TC_OFF)) return HMCX_ERR_UNSUPPORTED;
+    const size_t smem = (size_t)(m.tile_base + m.tile_floats) * sizeof(float);
+    rc = prepare_smem(mlp_out_kernel, smem);
+    if (rc != HMCX_OK) return rc;
+    mlp_out_kernel<<<C * n, MLP_THREADS, smem, st>>>(m, samples, cs, ds, n, r_begin, r_end, out, ocs, ods);
     return cuda_status();
 }
 

@@ -609,6 +609,63 @@ int hmcx_loo_pass(const float* ll, int64_t chain_stride, int64_t draw_stride, in
                   int32_t i0, int32_t k, double r_eff, double* pointwise, int32_t* tail_size, int32_t* nonfinite,
                   void* workspace, size_t workspace_bytes, void* stream);
 
+/*
+ * Held-out evaluation of Bayesian NNs (additive v12 symbols; hamiltorch_b200/predictive.py).  Callers of an older v12
+ * library check for the symbols.
+ *   hmcx_mlp_pointwise_out  out[c*out_chain_stride + s*out_draw_stride + (i - row_begin)*O + o] = output o of the network
+ *                    of draw (c, s) at data row i in [row_begin, row_end), O the output width: the values hmcx_mlp_predict
+ *                    writes for that row (log-probabilities for HMCX_LOSS_MULTICLASS_LOGSOFTMAX), bit for bit, computed
+ *                    with the tile loop of hmcx_mlp_pointwise_ll (SIMT tiles, or the tensor-core form when x_packed is
+ *                    set; split targets: rows in split order, read in place).  Argument checks as hmcx_mlp_pointwise_ll:
+ *                    NULL pointers, C < 1, n < 1, C*n > INT32_MAX, negative strides, a target without data or a row range
+ *                    outside [0, num_rows) or empty: HMCX_ERR_INVALID_ARG; other target kinds: HMCX_ERR_UNSUPPORTED.
+ *   hmcx_pred_workspace_bytes  workspace hmcx_pred_pass needs for a slab of k points: 8 (2n + 46 + n R) k bytes with
+ *                    R = O + 4 (multi-class), 3 O + 2 (binary) or 3 O + 4 (regression) per-step sums (0 for C < 1, n < 1,
+ *                    C*n > INT32_MAX, O < 1, k < 1 or an unknown loss).
+ *   hmcx_pred_pass   for the points i in [i0, i0 + k) of an fp32 block f[c, s, i, o] at f + c*chain_stride +
+ *                    s*draw_stride + i*O + o (C chains of n draws, N points): the posterior predictive over the S = C*n
+ *                    pooled draws, in fp64, and the curves over the first t draws of every chain (St = C*t draws).
+ *                    y: fp32 targets, [N, O] (regression, binary) or [N] labels in [0, O) (multi-class, both losses).
+ *                    tau_out: fp32 per-draw noise precision at tau_out + c*tau_chain_stride + s*tau_draw_stride
+ *                    (regression only; a stride of 0 repeats one value; classification may pass NULL).
+ *                      MULTICLASS*   p = softmax(f) per draw, pbar = its mean; label argmax pbar (lowest on ties);
+ *                                    nll = -(logsumexp_s log p_s[y] - log S)
+ *                      BINARY        each output a Bernoulli, pbar = mean sigmoid(f); predicted pbar > 0.5, correct when
+ *                                    it equals y > 0.5; nll, brier, entropies summed over the outputs; log p(y) =
+ *                                    y log sigmoid(f) + (1 - y) log sigmoid(-f)
+ *                      REGRESSION    mu = mean f, var = mean 1/tau + var f (ddof 0), ll_s = sum_o -0.5 tau (f_o - y_o)^2
+ *                                    + 0.5 O log(tau / 2 pi), lppd = logsumexp_s ll_s - log S, pit = mean Phi((y - f)
+ *                                    sqrt(tau))
+ *                    pointwise [7, N] fp64 rows: 0 nll (regression -lppd), 1 brier (regression sum_o (mu_o - y_o)^2),
+ *                      2 entropy H[pbar], 3 mean_s H[p_s], 4 mutual information 2 - 3, 5 correct predictions of the
+ *                      point, 6 predicted label (multi-class; rows 2-6 are 0 where they do not apply).
+ *                    per_output [1, N, O] fp64 (classification: pbar) or [4, N, O] (regression: mu, var, var f, pit).
+ *                    nonfinite [N] int32: 1 where the point has a non-finite output (all its outputs are NaN).
+ *                    partials [2n + 46, ceil(N / 128)] fp64, the sums of 128-point groups aligned to the point index,
+ *                    each in point order, continued across slabs (so every slab of a call sequence that covers [0, N) in
+ *                    order adds to the same array); rows: t - 1 < n: correct predictions with St draws (regression:
+ *                    squared error of the St-draw mean); n + t - 1: nll with St draws; 2n: brier; 2n + 1 + 3b .. 3 + 3b:
+ *                    count, confidence sum, correct sum of confidence bin b ((b/15, (b + 1)/15], b < 15; top label,
+ *                    binary: max(pbar, 1 - pbar) per output); regression 2n .. 2n + 3: the outputs with |pit - 0.5| <=
+ *                    level / 2 for levels 0.5, 0.8, 0.9, 0.95.  No atomics: the results depend on the block alone.
+ *                    NULL pointers (tau_out for regression), C < 1, n < 1, O < 1, N < 1, k < 1, negative strides, a slab
+ *                    outside [0, N), an unknown loss or a workspace smaller than
+ *                    hmcx_pred_workspace_bytes(C, n, O, loss, k): HMCX_ERR_INVALID_ARG; running sums beyond one SM's
+ *                    shared memory (128 (1, 3 or 4) O doubles): HMCX_ERR_UNSUPPORTED.  The pass sums the C draws of
+ *                    every step t per point in parallel (fp64, chain order) into the workspace, then scans t per point.
+ *   hmcx_pred_totals totals[r] = sum over groups of partials[r, :] in group order, 2n + 46 rows, once every slab is in.
+ *                    NULL pointers, n < 1 or N < 1: HMCX_ERR_INVALID_ARG.
+ */
+int hmcx_mlp_pointwise_out(const hmcx_target_t* target, const float* samples, int64_t chain_stride,
+                           int64_t draw_stride, int32_t C, int32_t n, int32_t row_begin, int32_t row_end, float* out,
+                           int64_t out_chain_stride, int64_t out_draw_stride, void* stream);
+size_t hmcx_pred_workspace_bytes(int32_t C, int32_t n, int32_t O, int32_t loss, int32_t k);
+int hmcx_pred_pass(const float* f, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t O,
+                   int32_t loss, const float* y, const float* tau_out, int64_t tau_chain_stride, int64_t tau_draw_stride,
+                   int32_t N, int32_t i0, int32_t k, double* pointwise, double* per_output, int32_t* nonfinite,
+                   double* partials, void* workspace, size_t workspace_bytes, void* stream);
+int hmcx_pred_totals(const double* partials, int32_t n, int32_t N, double* totals, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
