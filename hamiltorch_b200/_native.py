@@ -77,6 +77,13 @@ class HyperStruct(C.Structure):
                 ('gammas', C.c_void_p)]
 
 
+TEMPER_MAX_TEMPS = 32
+
+
+class TemperStruct(C.Structure):
+    _fields_ = [('num_temps', C.c_int32), ('tau_out', C.c_float * TEMPER_MAX_TEMPS), ('ll_out', C.c_void_p)]
+
+
 class NutsStruct(C.Structure):
     _fields_ = [('enabled', C.c_int32), ('desired_accept_rate', C.c_double), ('mu', C.c_double),
                 ('table', C.c_void_p), ('h_bar', C.c_void_p), ('eps_bar', C.c_void_p),
@@ -134,6 +141,13 @@ _PROTOS = {
                                        C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                        C.POINTER(SinkStruct), C.POINTER(HyperStruct), C.c_void_p]),
+    'hmcx_split_run_temper': (C.c_int, [C.POINTER(TargetStruct), C.POINTER(MassStruct), C.POINTER(RngStruct),
+                                        C.POINTER(NutsStruct), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.POINTER(SinkStruct), C.POINTER(TemperStruct), C.c_void_p]),
+    'hmcx_temper_swap': (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_double), C.c_void_p,
+                                   C.c_int32, C.POINTER(RngStruct), C.c_void_p, C.c_void_p, C.c_void_p]),
     'hmcx_hyper_gamma_draws': (C.c_int, [C.c_uint64, C.c_uint64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                          C.POINTER(C.c_double), C.c_void_p, C.c_void_p]),
     'hmcx_gemm_nt_tf32x3': (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p]),

@@ -952,9 +952,10 @@ __device__ __forceinline__ float mlp_log_prior(const MlpDev& m, const float* q, 
 template <int CS>
 __device__ __forceinline__ float mlp_log_prob(const MlpDev& m, const float* q, float* tile, float* sred, int s,
                                               float* pred_out, ClusterCtx cc, float* xslot, TcCtx& tc,
-                                              double* sse_out = nullptr) {
+                                              double* sse_out = nullptr, double* lsum_out = nullptr) {
     const float prior_term = __fdiv_rn(mlp_log_prior(m, q, sred), m.prior_scale);
     if (sse_out) *sse_out = 0.0;
+    if (lsum_out) *lsum_out = 0.0;
     if (!m.has_data) return prior_term;
     TcEpi te;
     if (m.tc) {
@@ -993,6 +994,10 @@ __device__ __forceinline__ float mlp_log_prob(const MlpDev& m, const float* q, f
         __syncthreads();
         sse[0] = cluster_sum_scalar<CS>(sse[0], xslot);
         if (sse_out) *sse_out += (double)sse[0];
+        // lsum_out: the sum over splits of ll_m / c_ll in fp64 -- the log-softmax loss is a per-split mean
+        if (lsum_out)
+            *lsum_out += m.loss == HMCX_LOSS_MULTICLASS_LOGSOFTMAX ? (double)sse[0] / (double)(m.sb[sp + 1] - m.sb[sp])
+                                                                   : (double)sse[0];
         const float ll = mlp_ll_from_sum(m, sse[0], m.sb[sp + 1] - m.sb[sp]);
         lp = (sp == s0) ? add(ll, prior_term) : add(lp, add(ll, prior_term));
     }
@@ -1030,6 +1035,14 @@ __device__ __forceinline__ HyperSm& hyper_sm() {
     __shared__ HyperSm s;
     return s;
 }
+// Replica exchange (hmcx_temper_t), read by the TEMPER instantiations only: row c runs rung c % T, whose likelihood
+// precision tau_out[c % T] replaces the target's (the power posterior at beta_t, DESIGN.md 3.17)
+struct MlpTemperDev {
+    int T;
+    float tau_out[HMCX_TEMPER_MAX_TEMPS];
+    double* ll_out;               // [C] or NULL: the untempered log-likelihood at q_cur when the launch ends
+};
+
 template <bool HYPER>
 __device__ __forceinline__ const MlpDev& run_model(const MlpDev& m) {
     if constexpr (HYPER) return hyper_sm().m;
@@ -1107,6 +1120,7 @@ struct MlpRunArgs {
     int moments_all;
     const double* mu_chain;
     MlpHyperDev hy;               // HYPER instantiations only
+    MlpTemperDev tp;              // TEMPER instantiations only
 };
 
 // One sink accumulator [C, ld] (sum, or sum of squares when `squares`) += the float4 x at element offset `off`, read and
@@ -1136,8 +1150,10 @@ __device__ __forceinline__ void sink_accumulate(float* hi, float* lo, size_t off
 
 // SINK = false: the plain sample() loop (rank 0 stores every post-burn row); SINK = true adds the sample sink, its row
 // work divided over the cluster's ranks (see sink_row below).  HYPER (with SINK only) adds the Gibbs updates of the Gamma
-// hyperpriors on the precisions after every MH step (DESIGN.md 3.15).
-template <int CS, bool SINK, bool HYPER = false>
+// hyperpriors on the precisions after every MH step (DESIGN.md 3.15).  TEMPER (with SINK only) runs row c at rung c % T of
+// a replica-exchange ladder: its descriptor copy carries the rung's tau_out, it tracks the untempered log-likelihood at
+// q_cur, and only rung 0 (beta = 1) rows store samples, to row c / T of samples_out (DESIGN.md 3.17).
+template <int CS, bool SINK, bool HYPER = false, bool TEMPER = false>
 __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArgs a) {
     extern __shared__ __align__(128) float sm[];
     __shared__ float sred[64];
@@ -1147,6 +1163,7 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
     __shared__ __align__(8) uint64_t s_bars[3];
 
     static_assert(SINK || !HYPER, "the hyperprior form is a sink form");
+    static_assert((SINK && !HYPER) || !TEMPER, "the tempered form is a sink form without hyperpriors");
     if constexpr (HYPER) {                                     // this chain's precisions and the constants they give
         HyperSm& hs = hyper_sm();
         if (threadIdx.x == 0) {
@@ -1158,7 +1175,17 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
         }
         __syncthreads();
     }
-    const MlpDev& m = run_model<HYPER>(a.m);
+    if constexpr (TEMPER) {                                    // the rung's tau_out and c_ll, as fill_mlp derives them
+        HyperSm& hs = hyper_sm();
+        if (threadIdx.x == 0) {
+            const float tau = a.tp.tau_out[(blockIdx.x / CS) % a.tp.T];
+            hs.m = a.m;
+            hs.m.tau_out = tau;
+            hs.m.c_ll = (a.m.loss == HMCX_LOSS_REGRESSION) ? (float)(-0.5 * (double)tau) : (float)(-(double)tau);
+        }
+        __syncthreads();
+    }
+    const MlpDev& m = run_model<HYPER || TEMPER>(a.m);
     ClusterCtx cc = {0, 1};
     if (CS > 1) { cc.rank = (int)cg::this_cluster().block_rank(); cc.size = CS; }
     const bool lead = cc.rank == 0;                            // rank 0 owns every global-memory output but the sink rows
@@ -1175,8 +1202,9 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
     for (int i = tid; i < m.Dp; i += MLP_THREADS) { q[i] = i < D ? a.q_cur[row + i] : 0.0f; p[i] = 0.0f; g[i] = 0.0f; }
     __syncthreads();
     double sse_cur = 0.0, sse_new = 0.0;                      // HYPER: the loss sum at q_cur / at the proposal
+    double ls_cur = 0.0, ls_new = 0.0;                        // TEMPER: untempered log-likelihood / c_ll, likewise
     float lp_cur = a.p_given ? 0.0f : mlp_log_prob<CS>(m, q, tile, sred, -1, nullptr, cc, &s_xchg, tc,
-                                                       HYPER ? &sse_cur : nullptr);
+                                                       HYPER ? &sse_cur : nullptr, TEMPER ? &ls_cur : nullptr);
 
     float eps = a.eps[c];
     double h_bar = 0.0, eps_bar = 1.0;
@@ -1187,7 +1215,9 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
     }
     int rejected = 0;
     const int keep = SINK ? 1 + (a.S - a.burn - 1) / a.thin : a.S - a.burn;      // slots per chain in samples_out
-    float* const my_samples = (a.samples && (SINK || lead)) ? a.samples + (size_t)c * keep * a.ld : nullptr;
+    float* const my_samples = TEMPER ? ((a.samples && c % a.tp.T == 0) ? a.samples + (size_t)(c / a.tp.T) * keep * a.ld
+                                                                       : nullptr)
+                                     : ((a.samples && (SINK || lead)) ? a.samples + (size_t)c * keep * a.ld : nullptr);
     // Sink: rank r owns the float4 vectors [sv0, sv1) of the row -- their thinned stores (16-byte streaming stores, which is
     // what lets rows leave over PCIe when samples_out is pinned host memory) and their moment updates.  Every rank holds a
     // bit-identical replica of q, so this needs no DSMEM traffic and no barrier beyond the loop's own.
@@ -1492,7 +1522,8 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
         }
         if (a.p_given) break;                                             // stand-alone leapfrog: no Hamiltonian, no MH
         // ---- Hamiltonians + MH ----
-        const float lp_new = mlp_log_prob<CS>(m, q, tile, sred, -1, nullptr, cc, &s_xchg, tc, HYPER ? &sse_new : nullptr);
+        const float lp_new = mlp_log_prob<CS>(m, q, tile, sred, -1, nullptr, cc, &s_xchg, tc, HYPER ? &sse_new : nullptr,
+                                              TEMPER ? &ls_new : nullptr);
         const float kin1 = kinetic();
         const float h_old = add(-lp_cur, mul(0.5f, kin0));
         const float h_new = add(-lp_new, mul(0.5f, kin1));
@@ -1508,6 +1539,7 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
         if (acc) {
             lp_cur = lp_new;
             if constexpr (HYPER) sse_cur = sse_new;
+            if constexpr (TEMPER) ls_cur = ls_new;
             if (lead) for (int i = tid; i < D; i += MLP_THREADS) a.q_cur[row + i] = q[i];
         } else {
             ++rejected;
@@ -1516,7 +1548,8 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
             for (int i = tid; i < D; i += MLP_THREADS) q[i] = src[row + i];
             __syncthreads();
             if (n == a.burn + 1) {
-                lp_cur = mlp_log_prob<CS>(m, q, tile, sred, -1, nullptr, cc, &s_xchg, tc, HYPER ? &sse_cur : nullptr);
+                lp_cur = mlp_log_prob<CS>(m, q, tile, sred, -1, nullptr, cc, &s_xchg, tc, HYPER ? &sse_cur : nullptr,
+                                          TEMPER ? &ls_cur : nullptr);
                 if (lead) for (int i = tid; i < D; i += MLP_THREADS) a.q_cur[row + i] = q[i];
             }
         }
@@ -1603,6 +1636,9 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
             for (int k = 0; k < 2 * m.L; ++k) a.hy.tau[(size_t)c * 2 * m.L + k] = hs.tau[k];
             a.hy.tau_out[c] = hs.tau_out;
         }
+    }
+    if constexpr (TEMPER) {                                    // the untempered c_ll is the constant bank's
+        if (tid == 0 && lead && a.tp.ll_out) a.tp.ll_out[c] = (double)a.m.c_ll * ls_cur;
     }
     if (tid == 0 && lead && !a.p_given) {
         a.eps[c] = eps;
@@ -2006,10 +2042,10 @@ int mlp_split_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hm
                   int scheme, const float* q_init, float* q_cur, float* eps, int C, int ld, int L, int S, int burn,
                   int it0, int it1, float* samples, uint8_t* accept, uint8_t* diverged, float* ham,
                   int32_t* num_rejected, cudaStream_t st, const float* p_given, float* q_traj, float* p_traj,
-                  const hmcx_sink_t* sink, const hmcx_hyper_t* hyper) {
+                  const hmcx_sink_t* sink, const hmcx_hyper_t* hyper, const hmcx_temper_t* temper) {
     MlpRunArgs a = {};
     hmcx_sink_t thin1 = {};
-    if (hyper && !sink) { thin1.thin = 1; sink = &thin1; }      // the hyperprior form is a sink form
+    if ((hyper || temper) && !sink) { thin1.thin = 1; sink = &thin1; }    // the hyperprior and tempered forms are sink forms
     a.p_given = p_given; a.q_traj = q_traj; a.p_traj = p_traj;
     if (sink) {
         a.thin = sink->thin; a.msum = sink->sum; a.msumsq = sink->sumsq;
@@ -2051,6 +2087,18 @@ int mlp_split_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hm
         a.hy.tau_trace = hyper->tau_trace; a.hy.tau_out_trace = hyper->tau_out_trace;
         a.hy.gammas = hyper->gammas;
     }
+    if (temper) {
+        if (hyper) return HMCX_ERR_UNSUPPORTED;
+        const int T = temper->num_temps;
+        if (p_given || T < 1 || T > HMCX_TEMPER_MAX_TEMPS || C % T != 0) return HMCX_ERR_INVALID_ARG;
+        a.tp.T = T;
+        for (int t = 0; t < T; ++t) {
+            const float v = temper->tau_out[t];
+            if (!(v >= 0.0f) || !(v <= FLT_MAX) || (t > 0 && !(v <= temper->tau_out[t - 1]))) return HMCX_ERR_INVALID_ARG;
+            a.tp.tau_out[t] = v;
+        }
+        a.tp.ll_out = temper->ll_out;
+    }
     a.scheme = scheme; a.mk = mk; a.C = C; a.ld = ld;
     a.im = mass ? mass->inv_mass : nullptr; a.sd = mass ? mass->mass_factor : nullptr;
     a.rng_mode = rng->mode; a.seed = rng->seed; a.chain_offset = rng->chain_offset;
@@ -2065,7 +2113,7 @@ int mlp_split_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hm
     }
     a.q_init = q_init; a.q_cur = q_cur; a.eps = eps; a.L = L; a.S = S; a.burn = burn; a.it0 = it0; a.it1 = it1;
     a.samples = samples; a.accept = accept; a.diverged = diverged; a.ham = ham; a.num_rejected = num_rejected;
-    if (!mlp_pick_tile(a.m, 3, target->mlp->tensor_cores != HMCX_MLP_TC_OFF, hyper ? sizeof(HyperSm) : 0))
+    if (!mlp_pick_tile(a.m, 3, target->mlp->tensor_cores != HMCX_MLP_TC_OFF, (hyper || temper) ? sizeof(HyperSm) : 0))
         return HMCX_ERR_UNSUPPORTED;                            // q, p, g do not fit one SM's shared memory
     const size_t smem = (size_t)(a.m.tile_base + a.m.tile_floats) * sizeof(float);
     // CTAs per chain (thread-block cluster size): at most the tiles of the smallest split, at most 4, and -- unless the
@@ -2092,7 +2140,10 @@ int mlp_split_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hm
     attr[0].val.clusterDim.x = cs; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
     void (*kern)(MlpRunArgs);
-    if (hyper) kern = cs == 4 ? mlp_run_kernel<4, true, true> : cs == 2 ? mlp_run_kernel<2, true, true> : mlp_run_kernel<1, true, true>;
+    if (temper)
+        kern = cs == 4 ? mlp_run_kernel<4, true, false, true>
+                       : cs == 2 ? mlp_run_kernel<2, true, false, true> : mlp_run_kernel<1, true, false, true>;
+    else if (hyper) kern = cs == 4 ? mlp_run_kernel<4, true, true> : cs == 2 ? mlp_run_kernel<2, true, true> : mlp_run_kernel<1, true, true>;
     else if (cs == 4) kern = sink ? mlp_run_kernel<4, true> : mlp_run_kernel<4, false>;
     else if (cs == 2) kern = sink ? mlp_run_kernel<2, true> : mlp_run_kernel<2, false>;
     else kern = sink ? mlp_run_kernel<1, true> : mlp_run_kernel<1, false>;
@@ -2182,7 +2233,7 @@ int mlp_leapfrog(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmc
     hmcx_nuts_t no_nuts = {};
     no_nuts.step_size_init = step_size;                        // the Python double the drifts divide (:513, :558)
     return mlp_split_run(target, mass, rng, &no_nuts, scheme, q_in, const_cast<float*>(q_in), eps, C, ld, L, 1, 0, 0, 1,
-                         nullptr, nullptr, nullptr, nullptr, nullptr, st, p_in, q_traj, p_traj, nullptr, nullptr);
+                         nullptr, nullptr, nullptr, nullptr, nullptr, st, p_in, q_traj, p_traj, nullptr, nullptr, nullptr);
 }
 
 // hmcx_hyper_gamma_draws: one thread per (iteration, chain, group), the device function of the HYPER kernels

@@ -106,14 +106,22 @@ def sample_chains_sharded(log_prob_func, params_init, gather_samples=False, runn
     then holds the adapted (D,) mass.
     With hyperpriors (``tau_prior`` / ``tau_out_prior``, passed through) and ``gather_samples``, ``tau_list_trace``
     (C, keep, 2L) and ``tau_out_trace`` (C, keep) are gathered alongside the samples.
+    With replica exchange (``betas``, T values) the partition is over the R = C / T ladders, not the chains: rank r owns the
+    rows T * shard_bounds(R, r, world), ``swap_log_uniforms`` (rounds, R, T - 1) is sliced by ladder, the per-row vectors are
+    gathered with that partition and the gathered ``samples`` are the (R, keep, D) beta = 1 rows.
     ``runner`` replaces ``samplers.sample_chains`` and ``diagnostics_partials`` the diagnostics' CUDA stages (used by
     the CPU tests of this host logic).
     """
     from . import samplers
     rank, world = _world()
     C = params_init.shape[0]
-    lo, hi = shard_bounds(C, rank, world)
     kw = dict(kwargs)
+    T = 1 if kw.get('betas') is None else len(kw['betas'])
+    if C % T != 0:
+        raise ValueError('sample_chains_sharded: C = %d rows is not a multiple of T = %d' % (C, T))
+    R = C // T                                     # ladders (T = 1: every chain is its own)
+    llo, lhi = shard_bounds(R, rank, world)
+    lo, hi = T * llo, T * lhi
     if hi == lo:
         raise RuntimeError('sample_chains_sharded: rank %d of %d would own no chain (C=%d < world); use fewer ranks'
                            % (rank, world, C))
@@ -122,14 +130,24 @@ def sample_chains_sharded(log_prob_func, params_init, gather_samples=False, runn
             if kw[name].shape[1] != C:
                 raise RuntimeError('%s must be (S, C=%d, ...), got %s' % (name, C, tuple(kw[name].shape)))
             kw[name] = kw[name][:, lo:hi]
+    if kw.get('swap_log_uniforms') is not None:
+        if kw['swap_log_uniforms'].shape[1] != R:
+            raise RuntimeError('swap_log_uniforms must be (rounds, R=%d, T - 1), got %s'
+                               % (R, tuple(kw['swap_log_uniforms'].shape)))
+        kw['swap_log_uniforms'] = kw['swap_log_uniforms'][:, llo:lhi]
     kw['chain_offset'] = kw.get('chain_offset', 0) + lo
     if kw.get('adapt_mass'):
         kw['mass_pool'] = lambda t: all_gather_rows(t, C)
+
+    def gather_rows(t):                            # per-row vectors, gathered ladder by ladder
+        if T == 1:
+            return all_gather_rows(t, C)
+        return all_gather_rows(t.reshape((lhi - llo, T) + tuple(t.shape[1:])), R).reshape((C,) + tuple(t.shape[1:]))
     run = runner if runner is not None else samplers.sample_chains
     local = run(log_prob_func, params_init[lo:hi], **kw)
     out = {'bounds': (lo, hi), 'local': local,
-           'num_rejected': all_gather_rows(local.num_rejected, C),
-           'step_size': all_gather_rows(local.step_size, C)}
+           'num_rejected': gather_rows(local.num_rejected),
+           'step_size': gather_rows(local.step_size)}
     if kw.get('adapt_mass'):
         out['inv_mass'] = local.inv_mass
     if gather_samples:
@@ -137,13 +155,13 @@ def sample_chains_sharded(log_prob_func, params_init, gather_samples=False, runn
         if not blk.is_cuda and dist.is_initialized() and dist.get_backend() == 'nccl':
             raise RuntimeError('gather_samples with store_on_GPU=False: the samples live in pinned host memory, which '
                                'NCCL cannot gather -- keep them on the GPU or gather on the host')
-        out['samples'] = all_gather_rows(blk, C)[..., :local.dim]
+        out['samples'] = all_gather_rows(blk, R)[..., :local.dim]
         if getattr(local, 'tau_list_trace', None) is not None:         # hyperpriors: the precisions of the same slots
             out['tau_list_trace'] = all_gather_rows(local.tau_list_trace, C)
             out['tau_out_trace'] = all_gather_rows(local.tau_out_trace, C)
     if getattr(local, 'moment_sum', None) is not None:          # sink moments requested: pool them over all ranks
-        out['posterior_mean'], out['posterior_var'], out['posterior_n'] = pooled_moments(
-            local.moment_sum, local.moment_sumsq, local.moment_count)
+        out['posterior_mean'], out['posterior_var'], out['posterior_n'] = pooled_moments(   # (the beta = 1 rows)
+            local.moment_sum[::T], local.moment_sumsq[::T], local.moment_count)
     if diagnostics:
         from .engine import HMCResult
         src = local if isinstance(local, HMCResult) else local.samples_padded[..., :local.dim]

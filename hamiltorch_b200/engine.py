@@ -460,7 +460,7 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
             nuts=False, desired_accept_rate=0.8, seed=0, chain_offset=0, normals=None, log_uniforms=None,
             record_ham=False, out=None, device=None, tuning=0, eps_schedule=None, record_eps=False, scheme=None,
             perms=None, thin=1, moments=False, keep_samples=True, host_samples=False, host_windows=0, adapt_mass=False,
-            mass_pool=None, hyper=None, gammas=None):
+            mass_pool=None, hyper=None, gammas=None, temper=None):
     """The reference's sample() loop for sampler in {HMC, HMC_NUTS} as one persistent kernel over C chains.
 
     params_init (C, D) | (D,).  Randomness: in-kernel Philox keyed by (seed, chain_offset+c, iteration), or -- when
@@ -491,6 +491,12 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
     (S, C, 2L + 1) fp64 standard-gamma draws.  The result gains ``tau_list_trace`` (C, keep, 2L), ``tau_out_trace``
     (C, keep) -- on the device whatever ``host_samples`` says -- and the final state ``tau_list_final`` (C, 2L),
     ``tau_out_final`` (C,).
+    ``temper`` (Bayesian-NN targets with a ``scheme``): replica exchange, a dict with ``betas`` (T Python floats, 1.0 first,
+    strictly decreasing), ``swap_every`` and ``swap_log_uniforms`` ((rounds, R, T - 1) fp64 or None: Philox).  The C = R T
+    rows are R ladders, row r T + t at beta_t (include/hmcx.h hmcx_temper_t, DESIGN §3.17): the run goes in windows of
+    ``swap_every`` iterations with a swap round (hmcx_temper_swap) after each window but the last.  ``samples`` / ``out``
+    hold the beta = 1 rows only, (R, keep, ld); the result gains ``betas``, ``swap_accepted`` (rounds, R, T - 1) int8,
+    ``swap_ll`` (rounds, C) fp64 and ``swap_rate`` (T - 1,).
     """
     N.require_cuda()
     lib = N.load_library()
@@ -529,18 +535,24 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
             raise NotImplementedError('adapt_mass: inv_mass None or 1-D, no windowed copy-engine delivery')
     use_sink = thin > 1 or moments or not keep_samples or host_samples
     keep = 1 + (S - burn - 1) // thin
+    if temper is not None:
+        if scheme is None or hyper is not None or adapt_mass:
+            raise NotImplementedError('replica exchange: Bayesian-NN targets, without hyperpriors or adapt_mass')
+        if Cn % len(temper['betas']) != 0:
+            raise ValueError('replica exchange: C = %d rows is not a multiple of T = %d' % (Cn, len(temper['betas'])))
+    Cs = Cn if temper is None else Cn // len(temper['betas'])      # rows of the sample block
     if not keep_samples:
         samples = None
     elif host_samples and out is None:
         # pinned host memory is device-addressable under unified virtual addressing: the kernel's st.global.cs rows go
         # over PCIe while the chains keep running (no device-side sample buffer, no separate D2H copy)
-        samples = torch.empty((Cn, keep, ld), dtype=torch.float32, pin_memory=True)
+        samples = torch.empty((Cs, keep, ld), dtype=torch.float32, pin_memory=True)
     elif out is None:
-        samples = torch.empty((Cn, keep, ld), dtype=torch.float32, device=device)
+        samples = torch.empty((Cs, keep, ld), dtype=torch.float32, device=device)
     else:
         samples = out
-        if tuple(samples.shape) != (Cn, keep, ld) or samples.dtype != torch.float32 or not samples.is_contiguous():
-            raise RuntimeError('out must be a contiguous fp32 (C, S-burn, ld) tensor')
+        if tuple(samples.shape) != (Cs, keep, ld) or samples.dtype != torch.float32 or not samples.is_contiguous():
+            raise RuntimeError('out must be a contiguous fp32 (%s, S-burn, ld) tensor' % ('C' if temper is None else 'R'))
     accepted = torch.empty((Cn, S), dtype=torch.uint8, device=device)
     diverged = torch.empty((Cn, S), dtype=torch.uint8, device=device)
     ham = torch.empty((Cn, S, 2), dtype=torch.float32, device=device) if record_ham else None
@@ -626,8 +638,13 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
             hyper_s.gammas = gm.data_ptr()
             keep_alive.append(gm)
     mass_out = None
+    temper_out = None
     with torch.cuda.device(device):
-        if adapt_mass:
+        if temper is not None:
+            temper_out = _tempered_launches(lib, nt, nm, rng, nuts_s, scheme, q_init, q_cur, eps, Cn, ld, L, S, burn,
+                                            samples, accepted, diverged, ham, num_rejected, sink, temper, device,
+                                            keep_alive)
+        elif adapt_mass:
             if sink is None:
                 sink = N.SinkStruct()
                 sink.thin = 1
@@ -706,8 +723,67 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
     if hyper_s is not None:
         res.tau_list_trace, res.tau_out_trace = tau_trace, tau_out_trace
         res.tau_list_final, res.tau_out_final = tau, tau_out
+    if temper_out is not None:
+        res.betas, res.swap_accepted, res.swap_ll = temper_out
+        a = res.swap_accepted
+        tried = (a >= 0).sum(dim=(0, 1))
+        res.swap_rate = (a == 1).sum(dim=(0, 1)).double() / tried.clamp_min(1).double()
     res._keep_alive = keep_alive          # buffers the asynchronous kernel still reads
     return res
+
+
+def swap_rounds(num_samples, swap_every):
+    """The number of swap rounds of a tempered run: one after every window of ``swap_every`` iterations but the last."""
+    return max(0, -(-int(num_samples) // int(swap_every)) - 1)
+
+
+def _tempered_launches(lib, nt, nm, rng, nuts_s, scheme, q_init, q_cur, eps, Cn, ld, L, S, burn, samples, accepted,
+                       diverged, ham, num_rejected, sink, temper, device, keep_alive):
+    """hmc_run with replica exchange: the windows [k E, min(S, (k + 1) E)) of E = swap_every iterations, each a tempered
+    sink launch (hmcx_split_run_temper) that leaves the untempered log-likelihood of every row in swap_ll[k], followed by
+    swap round k (hmcx_temper_swap) when iterations remain.  All on the current stream, no host synchronisation.  Returns
+    (betas (T,) fp64, swap_accepted (rounds, R, T - 1) int8, swap_ll (rounds, C) fp64)."""
+    betas = [float(b) for b in temper['betas']]
+    T, E = len(betas), int(temper['swap_every'])
+    R, rounds = Cn // T, swap_rounds(S, E)
+    tau0 = nt.mlp_desc.tau_out
+    ts = N.TemperStruct()
+    ts.num_temps = T
+    for t, b in enumerate(betas):
+        ts.tau_out[t] = b * tau0                 # the Python-double product, rounded to fp32 as MLPTarget(tau_out=b*tau0)
+    sink_s = sink
+    if sink_s is None:
+        sink_s = N.SinkStruct()
+        sink_s.thin = 1
+    swap_acc = torch.empty((rounds, R, T - 1), dtype=torch.int8, device=device)
+    swap_ll = torch.empty((rounds, Cn), dtype=torch.float64, device=device)
+    lu = temper.get('swap_log_uniforms')
+    if lu is not None:
+        if tuple(lu.shape) != (rounds, R, T - 1):
+            raise ValueError('swap_log_uniforms must be (rounds, R, T - 1) = (%d, %d, %d), got %s'
+                             % (rounds, R, T - 1, tuple(lu.shape)))
+        lu = lu.detach().to(device=device, dtype=torch.float64).contiguous()
+    srng = N.RngStruct()
+    srng.mode = N.RNG_INJECTED if lu is not None else N.RNG_PHILOX
+    srng.seed, srng.chain_offset = rng.seed, rng.chain_offset
+    cb = (C.c_double * T)(*betas)
+    keep_alive += [swap_acc, swap_ll, lu, ts, sink_s, srng, cb]
+    stream = N.stream_ptr(device)
+    for k in range(rounds + 1):
+        it0, it1 = k * E, min(S, (k + 1) * E)
+        r = _window_rng(rng, it0, Cn, ld, nt.num_splits)
+        keep_alive.append(r)
+        ts.ll_out = swap_ll[k].data_ptr() if k < rounds else None
+        rc = lib.hmcx_split_run_temper(nt.ref(), nm.ref(), C.byref(r), C.byref(nuts_s), int(scheme), N.ptr(q_init),
+                                       N.ptr(q_cur), N.ptr(eps), Cn, ld, L, S, burn, it0, it1, N.ptr(samples),
+                                       N.ptr(accepted), N.ptr(diverged), N.ptr(ham), N.ptr(num_rejected),
+                                       C.byref(sink_s), C.byref(ts), stream)
+        N.check(rc, 'hmcx_split_run_temper')
+        if k < rounds and T > 1:
+            rc = lib.hmcx_temper_swap(N.ptr(q_cur), Cn, ld, T, cb, N.ptr(swap_ll[k]), k, C.byref(srng),
+                                      None if lu is None else C.c_void_p(lu[k].data_ptr()), N.ptr(swap_acc[k]), stream)
+            N.check(rc, 'hmcx_temper_swap')
+    return torch.tensor(betas, dtype=torch.float64), swap_acc, swap_ll
 
 
 def _window_hyper(hyper_s, it0, Cn, groups):

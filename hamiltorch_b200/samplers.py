@@ -344,7 +344,7 @@ def sample_chains(log_prob_func, params_init, num_samples=10, num_steps_per_samp
                   desired_accept_rate=0.8, rng='philox', seed=0, chain_offset=0, normals=None, log_uniforms=None,
                   record_ham=False, out=None, perms=None, uniforms=None, thin=1, moments=False, keep_samples=True,
                   store_on_GPU=True, host_windows=0, adapt_mass=False, mass_pool=None, tau_prior=None,
-                  tau_out_prior=None, gammas=None):
+                  tau_out_prior=None, gammas=None, betas=None, swap_every=10, swap_log_uniforms=None):
     """The engine's native entry: C independent chains at once.  ``params_init`` is (C, D); every chain gets the
     reference's ``sample`` semantics.  Returns an ``engine.HMCResult`` whose ``.samples`` is (C, S-burn, D) on the
     GPU (row c = what ``sample`` would have returned for chain c, stacked).
@@ -386,6 +386,20 @@ def sample_chains(log_prob_func, params_init, num_samples=10, num_steps_per_samp
     standard-gamma draw of every group (tensors, then tau_out).  The result gains ``.tau_list_trace`` (C, keep, 2L) and
     ``.tau_out_trace`` (C, keep) for the retained sample slots (slot 0 = the initial values; on the device even with
     ``store_on_GPU=False``) and the final state ``.tau_list_final`` / ``.tau_out_final``.
+
+    Replica exchange (an ``MLPTarget`` or a split list of them, HMC / HMC_NUTS; DESIGN §3.17): ``betas`` are T likelihood
+    exponents, ``betas[0] == 1.0``, strictly decreasing, all >= 0; rung t samples the power posterior p(theta) L(theta)^beta_t,
+    i.e. the target with ``tau_out`` replaced by ``beta_t * tau_out``.  ``params_init`` is (C, D) with C = R T, ladder-major:
+    row r T + t is ladder r at beta_t.  The run goes in windows of ``swap_every`` iterations; after window k, if iterations
+    remain, swap round k pairs the rungs (t, t + 1) with t = k (mod 2) of every ladder and exchanges their states when
+    log u < (beta_t - beta_{t+1}) (ll_{t+1} - ll_t) in fp64, ll the untempered log-likelihood at the row's state.  Step
+    sizes, dual averaging, moments and counters stay with the row; swaps run during burn-in too.  ``rng='philox'`` draws u
+    from its own stream keyed by the global ladder (``chain_offset`` must be a multiple of T); ``rng='injected'`` reads
+    ``swap_log_uniforms`` (rounds, R, T - 1).  Only the beta = 1 rows store samples: ``.samples`` is (R, keep, D) (``thin``,
+    ``keep_samples``, ``store_on_GPU`` and ``out`` (R, keep, ld) apply to it); per-row outputs stay (C, ...).  The result
+    gains ``.betas``, ``.swap_accepted`` (rounds, R, T - 1) int8 (-1: the pair was not in that round), ``.swap_ll``
+    (rounds, C) fp64 and ``.swap_rate`` (T - 1,).  Not combined with RMHMC, non-BNN targets, a 2-D or block ``inv_mass``,
+    ``adapt_mass``, hyperpriors or ``rng='reference'``.
     """
     if params_init.dim() != 2:
         raise RuntimeError('sample_chains: params_init must be (num_chains, D)')
@@ -394,6 +408,8 @@ def sample_chains(log_prob_func, params_init, num_samples=10, num_steps_per_samp
     if adapt_mass:
         _check_adapt_mass(log_prob_func, sampler, integrator, inv_mass, burn, host_windows)
     hyper = _hyper_groups(log_prob_func, sampler, tau_prior, tau_out_prior)
+    temper = _temper_args(log_prob_func, params_init, num_samples, sampler, inv_mass, adapt_mass, hyper, rng,
+                          chain_offset, betas, swap_every, swap_log_uniforms)
     return _run_chains(log_prob_func, params_init, num_samples, num_steps_per_sample, step_size, burn, jitter,
                        inv_mass, softabs_const, explicit_binding_const, fixed_point_threshold,
                        fixed_point_max_iterations, jitter_max_tries, sampler, integrator, metric,
@@ -403,7 +419,51 @@ def sample_chains(log_prob_func, params_init, num_samples=10, num_steps_per_samp
                        sink=dict(thin=thin, moments=moments, keep_samples=keep_samples, host_samples=not store_on_GPU,
                                  host_windows=host_windows, **(dict(adapt_mass=True, mass_pool=mass_pool)
                                                                if adapt_mass else {})),
-                       hyper=hyper, gammas=gammas)
+                       hyper=hyper, gammas=gammas, temper=temper)
+
+
+def _temper_args(log_prob_func, params_init, num_samples, sampler, inv_mass, adapt_mass, hyper, rng, chain_offset,
+                 betas, swap_every, swap_log_uniforms):
+    """sample_chains(betas=...) -> engine.hmc_run's ``temper`` dict (None without betas), checked before any CUDA work."""
+    if betas is None:
+        return None
+    descs = log_prob_func if isinstance(log_prob_func, list) else [log_prob_func]
+    if not descs or not all(isinstance(d, T.MLPRegression) for d in descs):
+        raise NotImplementedError('replica exchange: Bayesian-NN targets only (an MLPRegression or a list of them)')
+    if sampler not in (Sampler.HMC, Sampler.HMC_NUTS):
+        raise NotImplementedError('replica exchange: sampler HMC or HMC_NUTS')
+    if isinstance(inv_mass, list) or (torch.is_tensor(inv_mass) and inv_mass.dim() != 1):
+        raise NotImplementedError('replica exchange: inv_mass None or 1-D')
+    if adapt_mass:
+        raise NotImplementedError('replica exchange is not combined with adapt_mass')
+    if hyper is not None:
+        raise NotImplementedError('replica exchange is not combined with hyperpriors (tau_prior / tau_out_prior)')
+    if rng == 'reference':
+        raise NotImplementedError("replica exchange: rng='philox' or 'injected' (the reference stream is one chain)")
+    try:
+        b = [float(v) for v in (betas.tolist() if torch.is_tensor(betas) else betas)]
+    except (TypeError, ValueError):
+        raise ValueError('betas must be a sequence of floats, got %r' % (betas,))
+    if not 1 <= len(b) <= N.TEMPER_MAX_TEMPS:
+        raise ValueError('betas needs 1 to %d values, got %d' % (N.TEMPER_MAX_TEMPS, len(b)))
+    if b[0] != 1.0 or not all(math.isfinite(v) and v >= 0 for v in b) or any(x <= y for x, y in zip(b, b[1:])):
+        raise ValueError('betas must start at 1.0 and decrease strictly to values >= 0, got %r' % (b,))
+    Tn, Cn = len(b), params_init.shape[0]
+    if Cn % Tn != 0:
+        raise ValueError('replica exchange: params_init has %d rows, not a multiple of T = %d' % (Cn, Tn))
+    if int(chain_offset) % Tn != 0:
+        raise ValueError('replica exchange: chain_offset %d is not a multiple of T = %d' % (chain_offset, Tn))
+    if isinstance(swap_every, bool) or int(swap_every) != swap_every or int(swap_every) < 1:
+        raise ValueError('swap_every must be an integer >= 1, got %r' % (swap_every,))
+    rounds = engine.swap_rounds(num_samples, swap_every)
+    if rng == 'injected':
+        shape = (rounds, Cn // Tn, Tn - 1)
+        if swap_log_uniforms is None or tuple(swap_log_uniforms.shape) != shape:
+            raise ValueError("rng='injected' with betas needs swap_log_uniforms of shape (rounds, R, T - 1) = %s, got %s"
+                             % (shape, None if swap_log_uniforms is None else tuple(swap_log_uniforms.shape)))
+    else:
+        swap_log_uniforms = None
+    return dict(betas=b, swap_every=int(swap_every), swap_log_uniforms=swap_log_uniforms)
 
 
 def _check_gamma(ab, what):
@@ -475,9 +535,11 @@ def _run_chains(log_prob_func, q0, num_samples, L, step_size, burn, jitter, inv_
                 explicit_binding_const, fixed_point_threshold, fixed_point_max_iterations, jitter_max_tries,
                 sampler, integrator, metric, desired_accept_rate, rng='philox', seed=None, chain_offset=0,
                 normals=None, log_uniforms=None, record_ham=False, out=None, injected_perms=None,
-                injected_uniforms=None, sink=None, hyper=None, gammas=None):
+                injected_uniforms=None, sink=None, hyper=None, gammas=None, temper=None):
     nuts = sampler == Sampler.HMC_NUTS
     hyper_kw = {} if hyper is None else dict(hyper=hyper)
+    if temper is not None:
+        hyper_kw['temper'] = temper
     gshapes = None if hyper is None else _reference_gamma_shapes(log_prob_func, hyper)
     sink = sink or {}
     if (sink.get('thin', 1) != 1 or sink.get('moments') or not sink.get('keep_samples', True) or

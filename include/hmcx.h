@@ -481,6 +481,56 @@ int hmcx_hyper_gamma_draws(uint64_t seed, uint64_t chain_offset, int32_t C, int3
                            int32_t K, const double* shapes, double* out, void* stream);
 
 /*
+ * Replica exchange (parallel tempering) for Bayesian NNs (additive v12 symbols; DESIGN §3.17).  Callers of an older v12
+ * library check for the symbols.  The C rows form R = C / T ladders laid out ladder-major: row r*T + t runs rung t of
+ * ladder r, the power posterior p(theta) L(theta)^beta_t, which is the target with tau_out replaced by beta_t * tau_out
+ * (every loss is linear in its c_ll).  Rung 0 is beta = 1.
+ *   num_temps      T in [1, HMCX_TEMPER_MAX_TEMPS]; C must be a multiple of T
+ *   tau_out        HOST values: rung t's tau_out, rounded to fp32 as hmcx_mlp_t.tau_out holds it; finite, >= 0,
+ *                  non-increasing in t.  The kernel derives the rung's c_ll from it as it does from hmcx_mlp_t.tau_out.
+ *   ll_out         optional [C] fp64 device: when the launch ends, the UNTEMPERED log-likelihood at q_cur, sum over splits
+ *                  of c_ll * loss_m (the log-softmax loss: c_ll * loss_m / n_m, its per-split mean), c_ll the target's
+ *                  own; the value the kernel's last MH evaluation of q_cur produced (no extra forward pass).
+ */
+#define HMCX_TEMPER_MAX_TEMPS 32
+typedef struct hmcx_temper {
+    int32_t num_temps;
+    float   tau_out[HMCX_TEMPER_MAX_TEMPS];
+    double* ll_out;
+} hmcx_temper_t;
+
+/* hmcx_split_run_sink with every row at its rung (the sink form; sink == NULL: a thin = 1 sink).  Samples are stored for
+ * rung 0 only: row r*T of the ladders goes to row r of samples_out, [C / T, keep, ld]; accept / diverged / ham / step
+ * sizes / num_rejected and the sink moments stay per row ([C, ...]).  Windows of iterations chain through q_cur as in
+ * hmcx_split_run_sink (log p(q_cur) is re-evaluated at the start of every launch), so q_cur rows may be exchanged between
+ * two launches.  Checked before any CUDA work: NULL target or temper, T out of range, C % T != 0, a tau_out value that is
+ * negative, not finite or larger than its predecessor, the sink checks of hmcx_split_run_sink: HMCX_ERR_INVALID_ARG;
+ * non-MLP targets: HMCX_ERR_UNSUPPORTED; otherwise the checks of hmcx_split_run_sink. */
+int hmcx_split_run_temper(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmcx_rng_t* rng,
+                          const hmcx_nuts_t* nuts, int32_t scheme,
+                          const float* q_init, float* q_cur, float* eps,
+                          int32_t C, int32_t ld, int32_t L, int32_t num_samples, int32_t burn,
+                          int32_t iter_begin, int32_t iter_end,
+                          float* samples_out, uint8_t* accept_out, uint8_t* diverged_out, float* ham_out,
+                          int32_t* num_rejected, const hmcx_sink_t* sink, const hmcx_temper_t* temper, void* stream);
+
+/* Swap round `round` of the ladders: deterministic even-odd pairing, the pairs (t, t + 1) with t = round (mod 2).  Pair t of
+ * ladder r swaps when  log u < (beta_t - beta_{t+1}) (ll[r*T + t + 1] - ll[r*T + t])  in fp64; an accepted pair exchanges
+ * its two q_cur rows (16-byte copies), nothing else.  accepted[r*(T-1) + t] = 1 / 0, or -1 where the pair is not in this
+ * round.  One thread per (ladder, pair) decides, no atomics: the same bytes on every call.
+ *   betas          HOST [T] fp64: betas[0] == 1, strictly decreasing, finite, >= 0
+ *   ll             [C] fp64 device (hmcx_temper_t.ll_out of the launch before)
+ *   rng            PHILOX: log u = log((double)u01(x)), x word 0 of the Philox block with counter (t, round, STREAM_SWAP << 24,
+ *                  ladder lo) and key (seed lo, seed hi ^ ladder hi), ladder = chain_offset / T + r, so the decisions do not
+ *                  depend on how ladders are sharded (chain_offset must be a multiple of T); INJECTED: log_uniforms
+ *                  [R, T - 1] fp64 device (this round's)
+ * NULL pointers, C < 1, T < 2 or > HMCX_TEMPER_MAX_TEMPS, C % T != 0, ld < 4 or not a multiple of 4, q_cur not 16-byte
+ * aligned, round < 0, bad betas, a PHILOX chain_offset that is not a multiple of T, an unknown rng mode:
+ * HMCX_ERR_INVALID_ARG. */
+int hmcx_temper_swap(float* q_cur, int32_t C, int32_t ld, int32_t num_temps, const double* betas, const double* ll,
+                     int32_t round, const hmcx_rng_t* rng, const double* log_uniforms, int8_t* accepted, void* stream);
+
+/*
  * hmcx_adapt_diag_mass (ABI v11): the pooled diagonal mass estimate at the end of a warm-up window (Stan's windowed
  * adaptation, regularised as Stan does) and the restart of the dual averaging that follows it.  One pass, fixed order, no
  * atomics.  Inputs: the per-chain compensated sums of a window of n >= 2 draws, [C, ld] each, as a sink launch with
