@@ -1698,89 +1698,7 @@ mlp_predict_kernel(const MlpDev m, const float* __restrict__ samples, int ld, fl
 //   multi-class  log_softmax(f)[y];  LogSoftmax output: f[y], the same value of the logits
 // tau_out tempers the classification likelihoods during sampling only; it does not enter these densities.
 __device__ __forceinline__ void mlp_ll_rows(const MlpDev& m, const float* out, const float* ytile, int r0, int cnt,
-                                            int r_begin, int r_end, float ll_const, float* llrow) {
-    const int nL = m.n[m.L];
-    for (int r = threadIdx.x; r < cnt; r += MLP_THREADS) {
-        const int i = r0 + r;
-        if (i < r_begin || i >= r_end) continue;
-        const float* z = out + r * nL;
-        float v = 0.0f;
-        if (m.loss == HMCX_LOSS_REGRESSION || m.loss == HMCX_LOSS_BINARY) {
-            for (int o = 0; o < nL; ++o) {
-                const float yv = ytile ? ytile[r * nL + o] : __ldg(m.y + (size_t)i * nL + o), f = z[o];
-                if (m.loss == HMCX_LOSS_REGRESSION) {
-                    const float d = f - yv;
-                    v += d * d;
-                } else {
-                    v -= (1.0f - yv) * f + fmaxf(-f, 0.0f) + log1pf(expf(-fabsf(f)));
-                }
-            }
-            if (m.loss == HMCX_LOSS_REGRESSION) v = ll_const + (-0.5f * m.tau_out) * v;
-        } else {
-            // both multi-class losses: the tile holds the logits (a LogSoftmax output layer is applied here, as in the
-            // loss stage), so f[y] of a LogSoftmax network is log_softmax(logits)[y]
-            int label = (int)(ytile ? ytile[r] : __ldg(m.y + i));
-            label = label < 0 ? 0 : (label >= nL ? nL - 1 : label);
-            float mx = z[0];
-            for (int k = 1; k < nL; ++k) mx = fmaxf(mx, z[k]);
-            float se = 0.0f;
-            for (int k = 0; k < nL; ++k) se += expf(z[k] - mx);
-            v = (z[label] - mx) - logf(se);
-        }
-        llrow[i] = v;
-    }
-}
-
-// ll[c, s, i - r_begin] = log p(y_i | theta_{c,s}) for the rows [r_begin, r_end): one CTA per draw, the tiles of the
-// target's own data (x, y and the packed tensor-core operands) read in place; tiles that straddle the slab's edges are
-// forwarded whole and only their rows inside it written.  The network outputs never leave shared memory.
-__global__ void __launch_bounds__(MLP_THREADS, 1)
-mlp_ll_kernel(const MlpDev m, const float* __restrict__ samples, long long cs, long long ds, int n, int r_begin,
-              int r_end, float ll_const, float* __restrict__ ll, long long lcs, long long lds) {
-    extern __shared__ __align__(128) float sm[];
-    __shared__ __align__(8) uint64_t s_bars[3];
-    float* q = sm;
-    float* tile = sm + m.tile_base;
-    const int c = blockIdx.x / n, s = blockIdx.x - c * n;
-    const float* qin = samples + (long long)c * cs + (long long)s * ds;
-    for (int i = threadIdx.x; i < m.Dp; i += MLP_THREADS) q[i] = i < m.D ? qin[i] : 0.0f;
-    __syncthreads();
-    float* llrow = ll + (long long)c * lcs + (long long)s * lds - r_begin;
-    TcCtx tc = {};
-    TcEpi te;
-    if (m.tc) {
-        tc_init(tc, s_bars);
-        tc_epi_begin(m, q, te);
-        fence_async_smem();
-        __syncthreads();
-    }
-    for (int sp = 0; sp < m.M; ++sp) {
-        if (m.sb[sp + 1] <= r_begin || m.sb[sp] >= r_end) continue;
-        int ti = 0;
-        for (int r0 = m.sb[sp]; r0 < m.sb[sp + 1] && r0 < r_end; r0 += m.T, ++ti) {
-            if (r0 + m.T <= r_begin) continue;
-            const int cnt = min(m.T, m.sb[sp + 1] - r0);
-            if (m.tc) {
-                float act[16];
-                tc_prefetch_fwd(m, tile, tc, m.tb[sp] + ti, 0);
-                tc_prefetch_y(m, tile, r0, cnt);
-                tc_forward_tile(m, q, tile, tc, te, act, 0);
-            } else {
-                mlp_forward_tile(m, q, tile, r0, cnt);
-            }
-            mlp_ll_rows(m, tile + m.aoff[m.L], m.tc ? tile + m.tc_yraw : nullptr, r0, cnt, r_begin, r_end, ll_const,
-                        llrow);
-            __syncthreads();
-        }
-    }
-}
-
-// mlp_ll_rows / mlp_ll_kernel with one tau_out per draw (the draws of a run with a tau_out hyperprior, DESIGN.md 3.15):
-// draw (c, s) reads tau[c * tcs + s * tds] and evaluates its constant 0.5 O log(tau / 2 pi) as the host does for the
-// target's tau_out (fp64 log, then the fp32 rounding).  A separate kernel, so that mlp_ll_kernel's code stays as it is.
-__device__ __forceinline__ void mlp_ll_rows_tau(const MlpDev& m, const float* out, const float* ytile, int r0, int cnt,
-                                            int r_begin, int r_end, float ll_const, float tau_out,
-                                                float* llrow) {
+                                            int r_begin, int r_end, float ll_const, float tau_out, float* llrow) {
     const int nL = m.n[m.L];
     for (int r = threadIdx.x; r < cnt; r += MLP_THREADS) {
         const int i = r0 + r;
@@ -1813,22 +1731,22 @@ __device__ __forceinline__ void mlp_ll_rows_tau(const MlpDev& m, const float* ou
     }
 }
 
-
-__global__ void __launch_bounds__(MLP_THREADS, 1)
-mlp_ll_tau_kernel(const MlpDev m, const float* __restrict__ samples, long long cs, long long ds, int n, int r_begin,
-                  int r_end, float* __restrict__ ll, long long lcs, long long lds, const float* __restrict__ tau,
-                  long long tcs, long long tds) {
+// The draw pass of the pointwise kernels: one CTA per draw loads it (qin) into shared memory and forwards the rows
+// [r_begin, r_end) tile by tile with the code of mlp_predict_kernel, over the target's own tiles split by split, so x, y
+// and the packed tensor-core operands are read in place.  pro() runs once, after the draw's loads are issued and before
+// the barrier that publishes it, so a kernel's per-draw set-up overlaps them.  Tiles that straddle the slab's edges are
+// forwarded whole; epi(tile, sp, r0, cnt) then sees the outputs of the rows r0 .. r0 + cnt - 1 of split sp at
+// tile + m.aoff[m.L] (and, on the tensor-core path, their y at tile + m.tc_yraw) and handles the rows inside the slab.
+template <typename Pro, typename Epi>
+__device__ __forceinline__ void mlp_draw_pass(const MlpDev& m, const float* qin, int r_begin, int r_end, Pro pro,
+                                              Epi epi) {
     extern __shared__ __align__(128) float sm[];
     __shared__ __align__(8) uint64_t s_bars[3];
     float* q = sm;
     float* tile = sm + m.tile_base;
-    const int c = blockIdx.x / n, s = blockIdx.x - c * n;
-    const float* qin = samples + (long long)c * cs + (long long)s * ds;
     for (int i = threadIdx.x; i < m.Dp; i += MLP_THREADS) q[i] = i < m.D ? qin[i] : 0.0f;
-    const float tau_out = tau[(long long)c * tcs + (long long)s * tds];
-    const float ll_const = (float)(0.5 * m.n[m.L] * log((double)tau_out / (2.0 * 3.14159265358979323846)));
+    pro();
     __syncthreads();
-    float* llrow = ll + (long long)c * lcs + (long long)s * lds - r_begin;
     TcCtx tc = {};
     TcEpi te;
     if (m.tc) {
@@ -1851,62 +1769,59 @@ mlp_ll_tau_kernel(const MlpDev m, const float* __restrict__ samples, long long c
             } else {
                 mlp_forward_tile(m, q, tile, r0, cnt);
             }
-            mlp_ll_rows_tau(m, tile + m.aoff[m.L], m.tc ? tile + m.tc_yraw : nullptr, r0, cnt, r_begin, r_end, ll_const,
-                            tau_out, llrow);
+            epi(tile, sp, r0, cnt);
             __syncthreads();
         }
     }
 }
 
+// ll[c, s, i - r_begin] = log p(y_i | theta_{c,s}) for the rows [r_begin, r_end), one CTA per draw; the network outputs
+// never leave shared memory.  tau == NULL: the target's tau_out and the host's ll_const.  Otherwise draw (c, s) reads
+// its own tau_out at tau[c * tcs + s * tds] (the draws of a run with a tau_out hyperprior, DESIGN.md 3.15) and
+// evaluates its constant as the host does (fp64 log, then the fp32 rounding).
+__global__ void __launch_bounds__(MLP_THREADS, 1)
+mlp_ll_kernel(const MlpDev m, const float* __restrict__ samples, long long cs, long long ds, int n, int r_begin,
+              int r_end, float ll_const, const float* __restrict__ tau, long long tcs, long long tds,
+              float* __restrict__ ll, long long lcs, long long lds) {
+    const int c = blockIdx.x / n, s = blockIdx.x - c * n;
+    float tau_out = m.tau_out;
+    float* llrow = ll + (long long)c * lcs + (long long)s * lds - r_begin;
+    mlp_draw_pass(m, samples + (long long)c * cs + (long long)s * ds, r_begin, r_end,
+                  [&] {
+                      if (!tau) return;
+                      tau_out = tau[(long long)c * tcs + (long long)s * tds];
+                      ll_const = (float)(0.5 * m.n[m.L] * log((double)tau_out / (2.0 * 3.14159265358979323846)));
+                  },
+                  [&](const float* tile, int, int r0, int cnt) {
+                      mlp_ll_rows(m, tile + m.aoff[m.L], m.tc ? tile + m.tc_yraw : nullptr, r0, cnt, r_begin, r_end,
+                                  ll_const, tau_out, llrow);
+                  });
+}
+
 // out[c, s, i - r_begin, :] = the network outputs of draw (c, s) at the rows [r_begin, r_end) (held-out evaluation,
-// DESIGN.md 3.16): the tile loop of mlp_ll_kernel, the outputs of mlp_predict_kernel -- the same forward, and a
-// LogSoftmax output layer applied by the loss stage of mlp_log_prob -- so the values are predict_model's, bit for bit.
+// DESIGN.md 3.16): the forward of mlp_predict_kernel, and a LogSoftmax output layer applied by the loss stage of
+// mlp_log_prob, so the values are predict_model's, bit for bit.
 __global__ void __launch_bounds__(MLP_THREADS, 1)
 mlp_out_kernel(const MlpDev m, const float* __restrict__ samples, long long cs, long long ds, int n, int r_begin,
                int r_end, float* __restrict__ out, long long ocs, long long ods) {
-    extern __shared__ __align__(128) float sm[];
-    __shared__ __align__(8) uint64_t s_bars[3];
-    float* q = sm;
-    float* tile = sm + m.tile_base;
     const int c = blockIdx.x / n, s = blockIdx.x - c * n;
-    const float* qin = samples + (long long)c * cs + (long long)s * ds;
-    for (int i = threadIdx.x; i < m.Dp; i += MLP_THREADS) q[i] = i < m.D ? qin[i] : 0.0f;
-    __syncthreads();
-    const int nL = m.n[m.L];
-    float* orow = out + (long long)c * ocs + (long long)s * ods - (long long)r_begin * nL;
-    TcCtx tc = {};
-    TcEpi te;
-    if (m.tc) {
-        tc_init(tc, s_bars);
-        tc_epi_begin(m, q, te);
-        fence_async_smem();
-        __syncthreads();
-    }
-    for (int sp = 0; sp < m.M; ++sp) {
-        if (m.sb[sp + 1] <= r_begin || m.sb[sp] >= r_end) continue;
-        int ti = 0;
-        for (int r0 = m.sb[sp]; r0 < m.sb[sp + 1] && r0 < r_end; r0 += m.T, ++ti) {
-            if (r0 + m.T <= r_begin) continue;
-            const int cnt = min(m.T, m.sb[sp + 1] - r0);
-            if (m.tc) {
-                float act[16];
-                tc_prefetch_fwd(m, tile, tc, m.tb[sp] + ti, 0);
-                tc_prefetch_y(m, tile, r0, cnt);
-                tc_forward_tile(m, q, tile, tc, te, act, 0);
-            } else {
-                mlp_forward_tile(m, q, tile, r0, cnt);
-            }
-            if (m.loss == HMCX_LOSS_MULTICLASS_LOGSOFTMAX) {
-                mlp_loss_tile(m, tile + m.aoff[m.L], nullptr, r0, cnt, m.sb[sp + 1] - m.sb[sp], true,
-                              m.tc ? tile + m.tc_yraw : nullptr);
-                __syncthreads();
-            }
-            const int lo = max(r0, r_begin) - r0, hi = min(r0 + cnt, r_end) - r0;
-            for (int e = lo * nL + threadIdx.x; e < hi * nL; e += MLP_THREADS)
-                orow[(long long)r0 * nL + e] = tile[m.aoff[m.L] + e];
-            __syncthreads();
-        }
-    }
+    int nL;
+    float* orow;
+    mlp_draw_pass(m, samples + (long long)c * cs + (long long)s * ds, r_begin, r_end,
+                  [&] {
+                      nL = m.n[m.L];
+                      orow = out + (long long)c * ocs + (long long)s * ods - (long long)r_begin * nL;
+                  },
+                  [&](float* tile, int sp, int r0, int cnt) {
+                      if (m.loss == HMCX_LOSS_MULTICLASS_LOGSOFTMAX) {
+                          mlp_loss_tile(m, tile + m.aoff[m.L], nullptr, r0, cnt, m.sb[sp + 1] - m.sb[sp], true,
+                                        m.tc ? tile + m.tc_yraw : nullptr);
+                          __syncthreads();
+                      }
+                      const int lo = max(r0, r_begin) - r0, hi = min(r0 + cnt, r_end) - r0;
+                      for (int e = lo * nL + threadIdx.x; e < hi * nL; e += MLP_THREADS)
+                          orow[(long long)r0 * nL + e] = tile[m.aoff[m.L] + e];
+                  });
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -2182,43 +2097,44 @@ int mlp_predict(const hmcx_target_t* target, const float* samples, int S, int ld
     return cuda_status();
 }
 
+// fill_mlp, the argument checks, the tile pick and the shared-memory opt-in of the pointwise entries: C x n draws, one
+// CTA each, over the rows [r_begin, r_end) into a strided block; args_ok: the entry's own checks
+template <typename Kern>
+static int mlp_draw_pass_setup(const hmcx_target_t* target, MlpDev& m, Kern kern, const float* samples, long long cs,
+                               long long ds, int C, int n, int r_begin, int r_end, const float* out, long long ocs,
+                               long long ods, bool args_ok, size_t& smem) {
+    const int rc = fill_mlp(target, m);
+    if (rc != HMCX_OK) return rc;
+    if (!samples || !out || C < 1 || n < 1 || (long long)C * n > 0x7fffffffLL || cs < 0 || ds < 0 || ocs < 0 ||
+        ods < 0 || !m.has_data || r_begin < 0 || r_end > m.N || r_begin >= r_end || !args_ok)
+        return HMCX_ERR_INVALID_ARG;
+    if (!mlp_pick_tile(m, 1, target->mlp->tensor_cores != HMCX_MLP_TC_OFF)) return HMCX_ERR_UNSUPPORTED;
+    smem = (size_t)(m.tile_base + m.tile_floats) * sizeof(float);
+    return prepare_smem(kern, smem);
+}
+
 int mlp_pointwise_ll(const hmcx_target_t* target, const float* samples, long long cs, long long ds, int C, int n,
                      int r_begin, int r_end, float* ll, long long lcs, long long lds, cudaStream_t st,
                      const float* tau, long long tcs, long long tds) {
     MlpDev m = {};
-    int rc = fill_mlp(target, m);
+    size_t smem = 0;
+    const int rc = mlp_draw_pass_setup(target, m, mlp_ll_kernel, samples, cs, ds, C, n, r_begin, r_end, ll, lcs, lds,
+                                       tcs >= 0 && tds >= 0, smem);
     if (rc != HMCX_OK) return rc;
-    if (!samples || !ll || C < 1 || n < 1 || (long long)C * n > 0x7fffffffLL || cs < 0 || ds < 0 || lcs < 0 || lds < 0 ||
-        !m.has_data || r_begin < 0 || r_end > m.N || r_begin >= r_end || tcs < 0 || tds < 0)
-        return HMCX_ERR_INVALID_ARG;
-    if (!mlp_pick_tile(m, 1, target->mlp->tensor_cores != HMCX_MLP_TC_OFF)) return HMCX_ERR_UNSUPPORTED;
-    const size_t smem = (size_t)(m.tile_base + m.tile_floats) * sizeof(float);
-    if (tau) {
-        rc = prepare_smem(mlp_ll_tau_kernel, smem);
-        if (rc != HMCX_OK) return rc;
-        mlp_ll_tau_kernel<<<C * n, MLP_THREADS, smem, st>>>(m, samples, cs, ds, n, r_begin, r_end, ll, lcs, lds, tau, tcs,
-                                                            tds);
-        return cuda_status();
-    }
-    rc = prepare_smem(mlp_ll_kernel, smem);
-    if (rc != HMCX_OK) return rc;
-    const double tau_t = (double)target->mlp->tau_out;
-    const float ll_const = (float)(0.5 * m.n[m.L] * log(tau_t / (2.0 * 3.14159265358979323846)));
-    mlp_ll_kernel<<<C * n, MLP_THREADS, smem, st>>>(m, samples, cs, ds, n, r_begin, r_end, ll_const, ll, lcs, lds);
+    // the target's constant is evaluated here once, a per-draw block's by the kernel
+    const float ll_const =
+        tau ? 0.0f : (float)(0.5 * m.n[m.L] * log((double)m.tau_out / (2.0 * 3.14159265358979323846)));
+    mlp_ll_kernel<<<C * n, MLP_THREADS, smem, st>>>(m, samples, cs, ds, n, r_begin, r_end, ll_const, tau, tcs, tds, ll,
+                                                    lcs, lds);
     return cuda_status();
 }
 
 int mlp_pointwise_out(const hmcx_target_t* target, const float* samples, long long cs, long long ds, int C, int n,
                       int r_begin, int r_end, float* out, long long ocs, long long ods, cudaStream_t st) {
     MlpDev m = {};
-    int rc = fill_mlp(target, m);
-    if (rc != HMCX_OK) return rc;
-    if (!samples || !out || C < 1 || n < 1 || (long long)C * n > 0x7fffffffLL || cs < 0 || ds < 0 || ocs < 0 ||
-        ods < 0 || !m.has_data || r_begin < 0 || r_end > m.N || r_begin >= r_end)
-        return HMCX_ERR_INVALID_ARG;
-    if (!mlp_pick_tile(m, 1, target->mlp->tensor_cores != HMCX_MLP_TC_OFF)) return HMCX_ERR_UNSUPPORTED;
-    const size_t smem = (size_t)(m.tile_base + m.tile_floats) * sizeof(float);
-    rc = prepare_smem(mlp_out_kernel, smem);
+    size_t smem = 0;
+    const int rc = mlp_draw_pass_setup(target, m, mlp_out_kernel, samples, cs, ds, C, n, r_begin, r_end, out, ocs, ods,
+                                       true, smem);
     if (rc != HMCX_OK) return rc;
     mlp_out_kernel<<<C * n, MLP_THREADS, smem, st>>>(m, samples, cs, ds, n, r_begin, r_end, out, ocs, ods);
     return cuda_status();

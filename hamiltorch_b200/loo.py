@@ -78,14 +78,16 @@ class Comparison:
 # ------------------------------------------------------------------------------------------------------------------
 # Inputs
 # ------------------------------------------------------------------------------------------------------------------
-def _mlp_target(target):
+def _mlp_targets(target, prefix, use):
+    """The MLPTargets of an MLPTarget or a split list, each with data; errors read '<prefix>: ...' and name what the
+    points are for (``use``: 'leave out', 'evaluate')."""
     items = target if isinstance(target, list) else [target]
     if not items or not all(isinstance(t, T.MLPTarget) for t in items):
-        raise TypeError('loo: the target must be an MLPTarget (define_model_log_prob) or the list '
-                        'define_split_model_log_prob returns, got %s' % type(target).__name__)
+        raise TypeError('%s: the target must be an MLPTarget (define_model_log_prob) or the list '
+                        'define_split_model_log_prob returns, got %s' % (prefix, type(target).__name__))
     if any(t.x is None for t in items):
-        raise RuntimeError('loo: the target has no data (x is None): there are no points to leave out')
-    return items[0]
+        raise RuntimeError('%s: the target has no data (x is None): there are no points to %s' % (prefix, use))
+    return items
 
 
 def _check_r_eff(r_eff):
@@ -96,7 +98,7 @@ def _check_r_eff(r_eff):
 
 
 def _samples_block(samples, target):
-    first = _mlp_target(target)
+    first = _mlp_targets(target, 'loo', 'leave out')[0]
     if torch.is_tensor(samples) and samples.dim() in (2, 3) and samples.shape[-1] != first.dim:
         raise RuntimeError('loo: the samples have %d parameters per draw, the target has %d'
                            % (samples.shape[-1], first.dim))
@@ -137,14 +139,9 @@ def _native_target(target, device):
 def _ll_rows(lib, nt, x, r0, r1, out, tau=None):
     """out[c, s, :] = ll of rows [r0, r1) (out a (C, n, r1 - r0) view with unit stride along its last dimension);
     tau: the (C, n) per-draw tau_out, or None for the target's."""
-    C_, n = int(x.shape[0]), int(x.shape[1])
-    if tau is None:
-        rc = lib.hmcx_mlp_pointwise_ll(nt.ref(), N.ptr(x), x.stride(0), x.stride(1), C_, n, r0, r1, N.ptr(out),
-                                       out.stride(0), out.stride(1), N.stream_ptr(x.device))
-        N.check(rc, 'hmcx_mlp_pointwise_ll')
-        return
-    rc = lib.hmcx_mlp_pointwise_ll_tau(nt.ref(), N.ptr(x), x.stride(0), x.stride(1), C_, n, r0, r1, N.ptr(tau),
-                                       tau.stride(0), tau.stride(1), N.ptr(out), out.stride(0), out.stride(1),
+    tcs, tds = (0, 0) if tau is None else (tau.stride(0), tau.stride(1))
+    rc = lib.hmcx_mlp_pointwise_ll_tau(nt.ref(), N.ptr(x), x.stride(0), x.stride(1), int(x.shape[0]), int(x.shape[1]),
+                                       r0, r1, N.ptr(tau), tcs, tds, N.ptr(out), out.stride(0), out.stride(1),
                                        N.stream_ptr(x.device))
     N.check(rc, 'hmcx_mlp_pointwise_ll_tau')
 

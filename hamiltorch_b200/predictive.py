@@ -71,12 +71,7 @@ class PredictiveResult:
 # ------------------------------------------------------------------------------------------------------------------
 def _target_data(target):
     """(loss id, O, y (N, O) or (N,) fp32 CPU tensor in split order, tau_out) of an MLPTarget or a split list."""
-    items = target if isinstance(target, list) else [target]
-    if not items or not all(isinstance(t, T.MLPTarget) for t in items):
-        raise TypeError('predictive: the target must be an MLPTarget (define_model_log_prob) or the list '
-                        'define_split_model_log_prob returns, got %s' % type(target).__name__)
-    if any(t.x is None for t in items):
-        raise RuntimeError('predictive: the target has no data (x is None): there are no points to evaluate')
+    items = _loo._mlp_targets(target, 'predictive', 'evaluate')
     first = items[0]
     O_ = first.widths[-1]
     y = torch.cat([t.y.detach().cpu().reshape(-1, t.y_cols) for t in items])
@@ -180,16 +175,22 @@ def _run(lib, dev, C_, n, O_, Np, loss, y, tau, fill):
     return pw, po, flag, totals
 
 
+def _outputs(lib, nt, x, r0, r1, out):
+    """out[c, s, :r1 - r0] = the network outputs of draw (c, s) at rows [r0, r1) (out a (C, n, rows, O) block, each
+    draw's rows contiguous)."""
+    rc = lib.hmcx_mlp_pointwise_out(nt.ref(), N.ptr(x), x.stride(0), x.stride(1), x.shape[0], x.shape[1], r0, r1,
+                                    N.ptr(out), out.stride(0), out.stride(1), N.stream_ptr(x.device))
+    N.check(rc, 'hmcx_mlp_pointwise_out')
+
+
 class _FromSamples:
     def __init__(self, lib, nt, x, O_, k):
         self.lib, self.nt, self.x, self.O, self.k, self.device = lib, nt, x, O_, k, x.device
         self.blk = torch.empty((x.shape[0], x.shape[1], k, O_), dtype=torch.float32, device=x.device)
 
     def __call__(self, i0, kk):
-        x, b = self.x, self.blk
-        rc = self.lib.hmcx_mlp_pointwise_out(self.nt.ref(), N.ptr(x), x.stride(0), x.stride(1), x.shape[0], x.shape[1],
-                                             i0, i0 + kk, N.ptr(b), b.stride(0), b.stride(1), N.stream_ptr(x.device))
-        N.check(rc, 'hmcx_mlp_pointwise_out')
+        b = self.blk
+        _outputs(self.lib, self.nt, self.x, i0, i0 + kk, b)
         # the pass reads point i at row i of the block: the slab's block holds rows [i0, i0 + kk)
         return C.c_void_p(b.data_ptr() - 4 * i0 * self.O), b.stride(0), b.stride(1)
 
@@ -215,10 +216,7 @@ def pointwise_outputs(samples, target, row_begin=0, row_end=None):
     row_end = Np if row_end is None else int(row_end)
     out = torch.empty((x.shape[0], x.shape[1], row_end - row_begin, O_), dtype=torch.float32, device=x.device)
     with torch.cuda.device(x.device):
-        rc = lib.hmcx_mlp_pointwise_out(nt.ref(), N.ptr(x), x.stride(0), x.stride(1), x.shape[0], x.shape[1],
-                                        int(row_begin), row_end, N.ptr(out), out.stride(0), out.stride(1),
-                                        N.stream_ptr(x.device))
-    N.check(rc, 'hmcx_mlp_pointwise_out')
+        _outputs(lib, nt, x, int(row_begin), row_end, out)
     return out
 
 
