@@ -114,8 +114,9 @@ def _grad_wrt_momentum(q, p, args):
     return torch.autograd.grad(rm_hamiltonian(q.detach().requires_grad_(), x, *args), x)[0]
 
 
-def leapfrog_explicit(q, p, args, steps, step_size, omega, max_tries=10):
-    """samplers.py:389-462: Cobb et al. 2019 augmented integrator A-B-C-B-A with the SEQUENTIAL C update (:447-450)."""
+def leapfrog_explicit(q, p, args, steps, step_size, omega, max_tries=10, copies=None):
+    """samplers.py:389-462: Cobb et al. 2019 augmented integrator A-B-C-B-A with the SEQUENTIAL C update (:447-450).
+    ``copies``: a list that receives the final augmented pair (q_copy, p_copy) (:462)."""
     q, p = q.clone(), p.clone()
     qc, pc = q.clone(), p.clone()
     qs, ps = [], []
@@ -136,6 +137,8 @@ def leapfrog_explicit(q, p, args, steps, step_size, omega, max_tries=10):
         qc = qc + 0.5 * step_size * _grad_wrt_momentum(q, pc, args)
         qs.append(q.clone())
         ps.append(p.clone())
+    if copies is not None:
+        copies += [qc, pc]
     return qs, ps
 
 

@@ -72,7 +72,7 @@ class HMC:
             return p
         return p @ self.im.t() if self.im.dim() == 2 else self.im * p
 
-    def momentum(self, z):                                                      # :185-202
+    def momentum(self, z, q):                                                   # :185-202
         if self.im is None:
             return z
         return z @ self.tril.t() if self.tril is not None else z * torch.sqrt(1.0 / self.im)
@@ -105,7 +105,7 @@ class RMHMC:
     def minv(self, p):
         return p @ self.ginv.t()
 
-    def momentum(self, z):                                                      # :183-184
+    def momentum(self, z, q):                                                   # :183-184
         return z @ self.lower.t()
 
     def hamiltonian(self, q, p):                                                # :731
@@ -155,7 +155,9 @@ class Replay:
 
 def replay(model, params_init, accepted, samples, normals, eps, L, burn):
     """params_init (C, D); accepted (C, S) and samples (C, S - burn, >= D) as the kernel returned them; normals (S, C, D)
-    the injected stream; eps (C,) or, for a teacher-forced NUTS schedule, (S, C)."""
+    the injected stream; eps (C,) or, for a teacher-forced NUTS schedule, (S, C).  The momentum hook gets the start state
+    (a position-dependent metric draws p = chol G(q) z); a model with a ``begin`` hook is told each iteration's index
+    before its first evaluation (the in-kernel metric's jitter rows are per iteration)."""
     C, D = params_init.shape
     S = accepted.shape[1]
     dev = model.t.device
@@ -169,7 +171,9 @@ def replay(model, params_init, accepted, samples, normals, eps, L, burn):
     for n in range(S):
         if n >= burn + 2:
             start = rows[:, n - 1 - burn]
-        p = model.momentum(normals[n].to(dev, F64))
+        if hasattr(model, 'begin'):
+            model.begin(n)
+        p = model.momentum(normals[n].to(dev, F64), start)
         h_old[:, n] = model.hamiltonian(start, p)
         q1, p1 = model.trajectory(start, p, eps[n] if eps.dim() == 2 else eps, L)
         h_new[:, n] = model.hamiltonian(q1, p1)
