@@ -146,6 +146,11 @@ _PROTOS = {
                                         C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.POINTER(SinkStruct), C.POINTER(TemperStruct), C.c_void_p]),
+    'hmcx_split_run_folds': (C.c_int, [C.POINTER(TargetStruct), C.POINTER(MassStruct), C.POINTER(RngStruct),
+                                       C.POINTER(NutsStruct), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.POINTER(SinkStruct), C.c_int32, C.c_void_p]),
     'hmcx_temper_swap': (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_double), C.c_void_p,
                                    C.c_int32, C.POINTER(RngStruct), C.c_void_p, C.c_void_p, C.c_void_p]),
     'hmcx_hyper_gamma_draws': (C.c_int, [C.c_uint64, C.c_uint64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,

@@ -23,7 +23,7 @@ int dense_rmhmc_run(const hmcx_target_t*, const hmcx_rmhmc_t*, const hmcx_const_
 int mlp_split_run(const hmcx_target_t*, const hmcx_mass_t*, const hmcx_rng_t*, const hmcx_nuts_t*, int, const float*,
                   float*, float*, int, int, int, int, int, int, int, float*, uint8_t*, uint8_t*, float*, int32_t*,
                   cudaStream_t, const float*, float*, float*, const hmcx_sink_t*, const hmcx_hyper_t*,
-                  const hmcx_temper_t*);
+                  const hmcx_temper_t*, int);
 int temper_swap(float*, int, int, int, const double*, const double*, int, const hmcx_rng_t*, const double*, int8_t*,
                 cudaStream_t);
 int hyper_gamma_draws(uint64_t, uint64_t, int, int, int, int, const double*, double*, cudaStream_t);
@@ -165,7 +165,7 @@ int hmcx_hmc_run_sink(const hmcx_target_t* target, const hmcx_mass_t* mass, cons
         return hmcx::mlp_split_run(target, mass, rng, nuts, HMCX_SCHEME_PLAIN, q_init, q_cur, eps, C, ld, L,
                                    num_samples, burn, iter_begin, iter_end, samples_out, accept_out, diverged_out,
                                    ham_out, num_rejected, (cudaStream_t)stream, nullptr, nullptr, nullptr, nullptr, nullptr,
-                                   nullptr);
+                                   nullptr, 0);
     return HMCX_ERR_UNSUPPORTED;
 }
 
@@ -203,7 +203,7 @@ int hmcx_split_run_hyper(const hmcx_target_t* target, const hmcx_mass_t* mass, c
     if (!sink && !hyper && has_mu_chain(nuts)) return HMCX_ERR_UNSUPPORTED;
     return hmcx::mlp_split_run(target, mass, rng, nuts, scheme, q_init, q_cur, eps, C, ld, L, num_samples, burn,
                                iter_begin, iter_end, samples_out, accept_out, diverged_out, ham_out, num_rejected,
-                               (cudaStream_t)stream, nullptr, nullptr, nullptr, sink, hyper, nullptr);
+                               (cudaStream_t)stream, nullptr, nullptr, nullptr, sink, hyper, nullptr, 0);
 }
 
 int hmcx_split_run_temper(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmcx_rng_t* rng,
@@ -218,7 +218,23 @@ int hmcx_split_run_temper(const hmcx_target_t* target, const hmcx_mass_t* mass, 
     if (target->kind != HMCX_TARGET_MLP) return HMCX_ERR_UNSUPPORTED;
     return hmcx::mlp_split_run(target, mass, rng, nuts, scheme, q_init, q_cur, eps, C, ld, L, num_samples, burn,
                                iter_begin, iter_end, samples_out, accept_out, diverged_out, ham_out, num_rejected,
-                               (cudaStream_t)stream, nullptr, nullptr, nullptr, sink, nullptr, temper);
+                               (cudaStream_t)stream, nullptr, nullptr, nullptr, sink, nullptr, temper, 0);
+}
+
+int hmcx_split_run_folds(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmcx_rng_t* rng,
+                         const hmcx_nuts_t* nuts, int32_t scheme, const float* q_init, float* q_cur, float* eps,
+                         int32_t C, int32_t ld, int32_t L, int32_t num_samples, int32_t burn, int32_t iter_begin,
+                         int32_t iter_end, float* samples_out, uint8_t* accept_out, uint8_t* diverged_out,
+                         float* ham_out, int32_t* num_rejected, const hmcx_sink_t* sink, int32_t num_folds,
+                         void* stream) {
+    if (!target || num_folds < 2 || num_folds > HMCX_MLP_MAX_SPLITS) return HMCX_ERR_INVALID_ARG;
+    if (sink && (sink->thin < 1 || (sink->sum_lo && !sink->sum) || (sink->sumsq_lo && !sink->sumsq)))
+        return HMCX_ERR_INVALID_ARG;
+    if (target->kind != HMCX_TARGET_MLP || scheme != HMCX_SCHEME_PLAIN) return HMCX_ERR_UNSUPPORTED;
+    if (!sink && has_mu_chain(nuts)) return HMCX_ERR_UNSUPPORTED;
+    return hmcx::mlp_split_run(target, mass, rng, nuts, scheme, q_init, q_cur, eps, C, ld, L, num_samples, burn,
+                               iter_begin, iter_end, samples_out, accept_out, diverged_out, ham_out, num_rejected,
+                               (cudaStream_t)stream, nullptr, nullptr, nullptr, sink, nullptr, nullptr, num_folds);
 }
 
 int hmcx_temper_swap(float* q_cur, int32_t C, int32_t ld, int32_t num_temps, const double* betas, const double* ll,

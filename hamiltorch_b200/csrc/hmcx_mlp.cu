@@ -1121,6 +1121,7 @@ struct MlpRunArgs {
     const double* mu_chain;
     MlpHyperDev hy;               // HYPER instantiations only
     MlpTemperDev tp;              // TEMPER instantiations only
+    int folds;                    // K-fold (PLAIN only, 0 = off): global chain g's whole potential is split g % folds
 };
 
 // One sink accumulator [C, ld] (sum, or sum of squares when `squares`) += the float4 x at element offset `off`, read and
@@ -1196,6 +1197,10 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
     float* tile = sm + m.tile_base;
     const size_t row = (size_t)c * a.ld;
     const uint64_t chain_id = a.chain_offset + (uint64_t)c;
+    // the data split that is this chain's whole PLAIN potential: -1 (every split) unless a K-fold run gives the chain
+    // fold k = g mod K's training rows, split k (DESIGN.md 3.18).  The host refuses folds with hyperpriors or tempering:
+    // those forms keep a constant -1 and compile as before.
+    const int psp = (!HYPER && !TEMPER && a.folds) ? (int)(chain_id % (uint64_t)a.folds) : -1;
     TcCtx tc = {};
     if (m.tc) tc_init(tc, s_bars);
 
@@ -1203,7 +1208,7 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
     __syncthreads();
     double sse_cur = 0.0, sse_new = 0.0;                      // HYPER: the loss sum at q_cur / at the proposal
     double ls_cur = 0.0, ls_new = 0.0;                        // TEMPER: untempered log-likelihood / c_ll, likewise
-    float lp_cur = a.p_given ? 0.0f : mlp_log_prob<CS>(m, q, tile, sred, -1, nullptr, cc, &s_xchg, tc,
+    float lp_cur = a.p_given ? 0.0f : mlp_log_prob<CS>(m, q, tile, sred, psp, nullptr, cc, &s_xchg, tc,
                                                        HYPER ? &sse_cur : nullptr, TEMPER ? &ls_cur : nullptr);
 
     float eps = a.eps[c];
@@ -1463,7 +1468,7 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
             bool prev_post = !g_fresh, kicked_ahead = false;
 #pragma unroll 1
             for (int t = 0; t < T; ++t) {
-                int sp = -1, sp_next = -1;
+                int sp = psp, sp_next = psp;
                 float kc = half;
                 bool post = false, reuse = false, kick_twice = false, drift_done = false;
                 if (plain) {
@@ -1522,7 +1527,7 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
         }
         if (a.p_given) break;                                             // stand-alone leapfrog: no Hamiltonian, no MH
         // ---- Hamiltonians + MH ----
-        const float lp_new = mlp_log_prob<CS>(m, q, tile, sred, -1, nullptr, cc, &s_xchg, tc, HYPER ? &sse_new : nullptr,
+        const float lp_new = mlp_log_prob<CS>(m, q, tile, sred, psp, nullptr, cc, &s_xchg, tc, HYPER ? &sse_new : nullptr,
                                               TEMPER ? &ls_new : nullptr);
         const float kin1 = kinetic();
         const float h_old = add(-lp_cur, mul(0.5f, kin0));
@@ -1548,7 +1553,7 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
             for (int i = tid; i < D; i += MLP_THREADS) q[i] = src[row + i];
             __syncthreads();
             if (n == a.burn + 1) {
-                lp_cur = mlp_log_prob<CS>(m, q, tile, sred, -1, nullptr, cc, &s_xchg, tc, HYPER ? &sse_cur : nullptr,
+                lp_cur = mlp_log_prob<CS>(m, q, tile, sred, psp, nullptr, cc, &s_xchg, tc, HYPER ? &sse_cur : nullptr,
                                           TEMPER ? &ls_cur : nullptr);
                 if (lead) for (int i = tid; i < D; i += MLP_THREADS) a.q_cur[row + i] = q[i];
             }
@@ -1957,7 +1962,7 @@ int mlp_split_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hm
                   int scheme, const float* q_init, float* q_cur, float* eps, int C, int ld, int L, int S, int burn,
                   int it0, int it1, float* samples, uint8_t* accept, uint8_t* diverged, float* ham,
                   int32_t* num_rejected, cudaStream_t st, const float* p_given, float* q_traj, float* p_traj,
-                  const hmcx_sink_t* sink, const hmcx_hyper_t* hyper, const hmcx_temper_t* temper) {
+                  const hmcx_sink_t* sink, const hmcx_hyper_t* hyper, const hmcx_temper_t* temper, int folds) {
     MlpRunArgs a = {};
     hmcx_sink_t thin1 = {};
     if ((hyper || temper) && !sink) { thin1.thin = 1; sink = &thin1; }    // the hyperprior and tempered forms are sink forms
@@ -2013,6 +2018,13 @@ int mlp_split_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hm
             a.tp.tau_out[t] = v;
         }
         a.tp.ll_out = temper->ll_out;
+    }
+    if (folds) {                                               // K-fold: one split per fold, each chain on its own
+        if (hyper || temper) return HMCX_ERR_UNSUPPORTED;
+        if (scheme != HMCX_SCHEME_PLAIN) return HMCX_ERR_UNSUPPORTED;
+        if (p_given || folds < 2 || folds > HMCX_MLP_MAX_SPLITS || a.m.M != folds || !a.m.has_data)
+            return HMCX_ERR_INVALID_ARG;
+        a.folds = folds;
     }
     a.scheme = scheme; a.mk = mk; a.C = C; a.ld = ld;
     a.im = mass ? mass->inv_mass : nullptr; a.sd = mass ? mass->mass_factor : nullptr;
@@ -2149,7 +2161,8 @@ int mlp_leapfrog(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmc
     hmcx_nuts_t no_nuts = {};
     no_nuts.step_size_init = step_size;                        // the Python double the drifts divide (:513, :558)
     return mlp_split_run(target, mass, rng, &no_nuts, scheme, q_in, const_cast<float*>(q_in), eps, C, ld, L, 1, 0, 0, 1,
-                         nullptr, nullptr, nullptr, nullptr, nullptr, st, p_in, q_traj, p_traj, nullptr, nullptr, nullptr);
+                         nullptr, nullptr, nullptr, nullptr, nullptr, st, p_in, q_traj, p_traj, nullptr, nullptr, nullptr,
+                         0);
 }
 
 // hmcx_hyper_gamma_draws: one thread per (iteration, chain, group), the device function of the HYPER kernels

@@ -109,6 +109,10 @@ def sample_chains_sharded(log_prob_func, params_init, gather_samples=False, runn
     With replica exchange (``betas``, T values) the partition is over the R = C / T ladders, not the chains: rank r owns the
     rows T * shard_bounds(R, r, world), ``swap_log_uniforms`` (rounds, R, T - 1) is sliced by ladder, the per-row vectors are
     gathered with that partition and the gathered ``samples`` are the (R, keep, D) beta = 1 rows.
+    With K-fold refits (``folds``, K = max + 1 folds) the partition is over groups of K rows in the same way, so every rank
+    holds whole groups and its ``chain_offset`` stays a multiple of K; the injected streams are sliced by row, and the
+    gathered ``samples`` are the (C, keep, D) rows in global order (``samples[k::K]`` is fold k).  The folds are different
+    posteriors, so sink moments are not pooled across rows: each rank's ``local`` keeps its per-row sums.
     ``runner`` replaces ``samplers.sample_chains`` and ``diagnostics_partials`` the diagnostics' CUDA stages (used by
     the CPU tests of this host logic).
     """
@@ -117,11 +121,14 @@ def sample_chains_sharded(log_prob_func, params_init, gather_samples=False, runn
     C = params_init.shape[0]
     kw = dict(kwargs)
     T = 1 if kw.get('betas') is None else len(kw['betas'])
-    if C % T != 0:
-        raise ValueError('sample_chains_sharded: C = %d rows is not a multiple of T = %d' % (C, T))
-    R = C // T                                     # ladders (T = 1: every chain is its own)
+    K = 1 if kw.get('folds') is None else int(kw['folds'].max()) + 1
+    G = T if K == 1 else K                         # rows per group: a ladder, or one chain of every fold
+    if C % G != 0:
+        raise ValueError('sample_chains_sharded: C = %d rows is not a multiple of %s = %d'
+                         % (C, 'T' if K == 1 else 'K', G))
+    R = C // G                                     # groups (G = 1: every chain is its own)
     llo, lhi = shard_bounds(R, rank, world)
-    lo, hi = T * llo, T * lhi
+    lo, hi = G * llo, G * lhi
     if hi == lo:
         raise RuntimeError('sample_chains_sharded: rank %d of %d would own no chain (C=%d < world); use fewer ranks'
                            % (rank, world, C))
@@ -139,10 +146,10 @@ def sample_chains_sharded(log_prob_func, params_init, gather_samples=False, runn
     if kw.get('adapt_mass'):
         kw['mass_pool'] = lambda t: all_gather_rows(t, C)
 
-    def gather_rows(t):                            # per-row vectors, gathered ladder by ladder
-        if T == 1:
+    def gather_rows(t):                            # per-row vectors, gathered group by group
+        if G == 1:
             return all_gather_rows(t, C)
-        return all_gather_rows(t.reshape((lhi - llo, T) + tuple(t.shape[1:])), R).reshape((C,) + tuple(t.shape[1:]))
+        return all_gather_rows(t.reshape((lhi - llo, G) + tuple(t.shape[1:])), R).reshape((C,) + tuple(t.shape[1:]))
     run = runner if runner is not None else samplers.sample_chains
     local = run(log_prob_func, params_init[lo:hi], **kw)
     out = {'bounds': (lo, hi), 'local': local,
@@ -155,11 +162,11 @@ def sample_chains_sharded(log_prob_func, params_init, gather_samples=False, runn
         if not blk.is_cuda and dist.is_initialized() and dist.get_backend() == 'nccl':
             raise RuntimeError('gather_samples with store_on_GPU=False: the samples live in pinned host memory, which '
                                'NCCL cannot gather -- keep them on the GPU or gather on the host')
-        out['samples'] = all_gather_rows(blk, R)[..., :local.dim]
+        out['samples'] = (all_gather_rows(blk, R) if K == 1 else gather_rows(blk))[..., :local.dim]
         if getattr(local, 'tau_list_trace', None) is not None:         # hyperpriors: the precisions of the same slots
             out['tau_list_trace'] = all_gather_rows(local.tau_list_trace, C)
             out['tau_out_trace'] = all_gather_rows(local.tau_out_trace, C)
-    if getattr(local, 'moment_sum', None) is not None:          # sink moments requested: pool them over all ranks
+    if getattr(local, 'moment_sum', None) is not None and K == 1:   # sink moments requested: pool them over all ranks
         out['posterior_mean'], out['posterior_var'], out['posterior_n'] = pooled_moments(   # (the beta = 1 rows)
             local.moment_sum[::T], local.moment_sumsq[::T], local.moment_count)
     if diagnostics:

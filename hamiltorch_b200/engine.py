@@ -3,6 +3,7 @@
 Everything here is plumbing -- device buffers, padding to the (C, ld) layout, the step-size adaptation table,
 the random-stream modes.  The arithmetic of the hot path lives in csrc/*.cu.
 """
+import copy
 import ctypes as C
 import os
 import math
@@ -36,6 +37,31 @@ def _combine_mlp_splits(splits):
     for d in splits:
         begin.append(begin[-1] + d.x.shape[0])
     return first, x, y, begin
+
+
+def fold_targets(target, folds):
+    """The K training sets of a K-fold run as a split list: split k is a copy of the MLPTarget ``target`` holding every
+    data row i with ``folds[i] != k`` in the original order (rows with fold -1 are in every split), with the target's
+    network, prior, prior_scale, tau_out and settings.  ``folds``: (N,) integers in -1 .. K-1, K = max + 1.
+
+    Memory: the native form of the list (``NativeTarget``) concatenates the training sets, about (K - 1) N rows of x and
+    y -- K N rows with reloo's -1 rows.  A tensor-core stack (n0 -> 128 -> nL) also packs x as 16 n0 bytes per row (tf32
+    hi | lo in both GEMM layouts): once per training set, and once more for the all-rows tiling when a split boundary is
+    not a multiple of 64 rows, i.e. up to 2 (K - 1) N rows of packed operand."""
+    if not isinstance(target, T.MLPTarget) or target.x is None:
+        raise TypeError('fold_targets: an MLPTarget with data')
+    f = torch.as_tensor(folds).detach().to(device=target.x.device, dtype=torch.int64).reshape(-1)
+    n = target.x.shape[0]
+    if f.numel() != n:
+        raise ValueError('fold_targets: folds has %d entries, the target has %d data rows' % (f.numel(), n))
+    y = target.y.reshape(n, target.y_cols)
+    out = []
+    for k in range(int(f.max()) + 1):
+        keep = f != k
+        t = copy.copy(target)
+        t.x, t.y = target.x[keep], y[keep]
+        out.append(t)
+    return out
 
 
 class NativeTarget:
@@ -460,7 +486,7 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
             nuts=False, desired_accept_rate=0.8, seed=0, chain_offset=0, normals=None, log_uniforms=None,
             record_ham=False, out=None, device=None, tuning=0, eps_schedule=None, record_eps=False, scheme=None,
             perms=None, thin=1, moments=False, keep_samples=True, host_samples=False, host_windows=0, adapt_mass=False,
-            mass_pool=None, hyper=None, gammas=None, temper=None):
+            mass_pool=None, hyper=None, gammas=None, temper=None, folds=None):
     """The reference's sample() loop for sampler in {HMC, HMC_NUTS} as one persistent kernel over C chains.
 
     params_init (C, D) | (D,).  Randomness: in-kernel Philox keyed by (seed, chain_offset+c, iteration), or -- when
@@ -497,12 +523,24 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
     ``swap_every`` iterations with a swap round (hmcx_temper_swap) after each window but the last.  ``samples`` / ``out``
     hold the beta = 1 rows only, (R, keep, ld); the result gains ``betas``, ``swap_accepted`` (rounds, R, T - 1) int8,
     ``swap_ll`` (rounds, C) fp64 and ``swap_rate`` (T - 1,).
+    ``folds`` (an MLPTarget with ``scheme`` PLAIN): K-fold refits, an (N,) integer tensor assigning each data row to a fold
+    0 .. K-1 or to -1 (never left out).  The target becomes ``fold_targets(target, folds)`` and one hmcx_split_run_folds
+    launch runs chain g = chain_offset + c on fold g mod K's training rows (DESIGN §3.18).  The result gains ``folds``
+    (the assignment, on the device) and ``num_folds``.
     """
     N.require_cuda()
     lib = N.load_library()
     if device is None:
         device = params_init.device if params_init.is_cuda else torch.device('cuda', torch.cuda.current_device())
     device = torch.device(device)
+    num_folds = 0
+    if folds is not None:
+        if scheme != N.SCHEME_PLAIN or temper is not None or hyper is not None or adapt_mass:
+            raise NotImplementedError('K-fold runs: the plain integrator on an MLPTarget, without replica exchange, '
+                                      'hyperpriors or adapt_mass')
+        folds = torch.as_tensor(folds).to(device=device, dtype=torch.int64)
+        target = fold_targets(target, folds.cpu())
+        num_folds = len(target)
     nt = native_target(target, device)
     D, ld = nt.dim, N.padded_ld(nt.dim)
     nm = native_mass(inv_mass, D, device)
@@ -651,6 +689,12 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
             mass_out = _adapted_launches(lib, nt, nm, rng, nuts_s, scheme, q_init, q_cur, eps, Cn, D, ld, L, S, burn,
                                          samples, accepted, diverged, ham, num_rejected, int(tuning), sink, h_bar,
                                          eps_bar, mass_pool, device, keep_alive, hyper_s)
+        elif num_folds:
+            rc = lib.hmcx_split_run_folds(nt.ref(), nm.ref(), C.byref(rng), C.byref(nuts_s), int(scheme), N.ptr(q_init),
+                                          N.ptr(q_cur), N.ptr(eps), Cn, ld, L, S, burn, 0, S, N.ptr(samples),
+                                          N.ptr(accepted), N.ptr(diverged), N.ptr(ham), N.ptr(num_rejected),
+                                          None if sink is None else C.byref(sink), num_folds, N.stream_ptr(device))
+            N.check(rc, 'hmcx_split_run_folds')
         elif scheme is None:
             ws_bytes = lib.hmcx_hmc_workspace_bytes(nt.ref(), nm.ref(), Cn, ld)
             ws = torch.empty(ws_bytes // 4, dtype=torch.float32, device=device) if ws_bytes else None
@@ -723,6 +767,8 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
     if hyper_s is not None:
         res.tau_list_trace, res.tau_out_trace = tau_trace, tau_out_trace
         res.tau_list_final, res.tau_out_final = tau, tau_out
+    if num_folds:
+        res.folds, res.num_folds = folds, num_folds
     if temper_out is not None:
         res.betas, res.swap_accepted, res.swap_ll = temper_out
         a = res.swap_accepted

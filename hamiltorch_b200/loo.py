@@ -6,6 +6,9 @@ ArviZ's ``az.loo`` / ``az.waic`` and PyMC report, restated in numpy fp64 by test
     lo = hamiltorch_b200.loo.psis_loo(res, target)              # or psis_loo(ll)
     lo.elpd_loo, lo.se, lo.pareto_k.max(), lo.num_bad_k
     hamiltorch_b200.loo.compare(lo_a, lo_b)                     # elpd differences to the best model
+    lo = hamiltorch_b200.loo.reloo(lo, target, params_init, num_samples=..., ...)   # exact refits where k-hat is high
+    f = hamiltorch_b200.loo.kfold_split(N, K)                   # K-fold CV: one launch fits every fold
+    kf = hamiltorch_b200.loo.kfold(sample_chains(target, params_init, folds=f, ...), target)
 
 ``target`` is the ``MLPTarget`` of ``define_model_log_prob`` or the list ``define_split_model_log_prob`` returns (data
 points in split order).  Two CUDA passes:
@@ -19,6 +22,7 @@ points in split order).  Two CUDA passes:
 Samples plus a target are processed in slabs of data points, so the (S, N) log-likelihood block is never held whole:
 each slab's block and sort workspace fit in ``diagnostics.RANK_WORKSPACE_BUDGET`` bytes (at least one point per slab).
 """
+import copy
 import ctypes as C
 import math
 
@@ -185,8 +189,9 @@ def _slab_points(lib, C_, n, Np, extra_per_point=0):
     return k
 
 
-def _pointwise_pass(x, target, r_eff, tau=None):
-    """(C, n, N) draws -> (pw (6, N) fp64, tail (N,) int32, flag (N,) int32, S, N)."""
+def _pointwise_pass(x, target, r_eff, tau=None, nt=None, rows=None):
+    """(C, n, N) draws -> (pw (6, N) fp64, tail (N,) int32, flag (N,) int32, S, N).  ``nt`` / ``rows``: the native
+    form of ``target`` when the caller built it, and the data rows [r0, r1) of it to score (default: all of them)."""
     N.require_cuda()
     lib = N.load_library()
     dev = x.device
@@ -200,8 +205,9 @@ def _pointwise_pass(x, target, r_eff, tau=None):
         k = _slab_points(lib, C_, n, Np)
         nt = None
     else:
-        nt = _native_target(target, dev)
-        Np = int(nt.mlp_struct.num_rows)
+        nt = _native_target(target, dev) if nt is None else nt
+        r0, r1 = (0, int(nt.mlp_struct.num_rows)) if rows is None else rows
+        Np = r1 - r0
         k = _slab_points(lib, C_, n, Np, extra_per_point=4 * S)
     pw = torch.empty((6, Np), dtype=torch.float64, device=dev)
     tail = torch.empty(Np, dtype=torch.int32, device=dev)
@@ -216,7 +222,7 @@ def _pointwise_pass(x, target, r_eff, tau=None):
             if nt is None:
                 src, base = x, N.ptr(x)
             else:
-                _ll_rows(lib, nt, x, i0, i0 + kk, blk, tau)
+                _ll_rows(lib, nt, x, r0 + i0, r0 + i0 + kk, blk, tau)
                 # the pass reads point i at column i of the block: the slab's block holds columns [i0, i0 + kk)
                 src, base = blk, C.c_void_p(blk.data_ptr() - 4 * i0)
             rc = lib.hmcx_loo_pass(base, src.stride(0), src.stride(1), C_, n, Np, i0, kk, float(r_eff), N.ptr(pw),
@@ -295,21 +301,21 @@ def waic(x, target=None, tau_out=None):
 
 
 def compare(*results):
-    """Compare models fitted to the same N data points by their ``psis_loo`` (or ``waic``) results: the elpd
-    differences to the best model and se_diff = sqrt(N) sd(diff_i) of the pointwise differences (ddof 1).  Refuses
-    results of different kinds or different N.  Returns a ``Comparison``."""
+    """Compare models fitted to the same N data points by their ``psis_loo`` (``reloo`` results included), ``waic``
+    or ``kfold`` results: the elpd differences to the best model and se_diff = sqrt(N) sd(diff_i) of the pointwise
+    differences (ddof 1).  Refuses results of different kinds or different N.  Returns a ``Comparison``."""
     if len(results) == 1 and isinstance(results[0], (list, tuple)):
         results = tuple(results[0])
     if len(results) < 2:
         raise ValueError('compare: need at least two results')
     kinds = {getattr(r, 'kind', None) for r in results}
-    if len(kinds) != 1 or kinds.pop() not in ('loo', 'waic'):
-        raise TypeError('compare: pass psis_loo results only or waic results only')
+    if len(kinds) != 1 or kinds.pop() not in _ELPD:
+        raise TypeError('compare: pass psis_loo results only, waic results only or kfold results only')
     n0 = results[0].num_points
     if any(r.num_points != n0 for r in results):
         raise RuntimeError('compare: the results score different numbers of data points (%s); models are compared '
                            'on the same data' % ', '.join(str(r.num_points) for r in results))
-    elpd = [r.elpd_loo if r.kind == 'loo' else r.elpd_waic for r in results]
+    elpd = [getattr(r, _ELPD[r.kind]) for r in results]
     order = sorted(range(len(results)), key=lambda i: -elpd[i])
     best = results[order[0]].pointwise
     diff, se = [], []
@@ -318,3 +324,163 @@ def compare(*results):
         diff.append(elpd[i] - elpd[order[0]])
         se.append(0.0 if i == order[0] else _total(d)[1])
     return Comparison(elpd, diff, se, order)
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# K-fold cross-validation and exact refits (reloo)
+# ------------------------------------------------------------------------------------------------------------------
+_ELPD = {'loo': 'elpd_loo', 'waic': 'elpd_waic', 'kfold': 'elpd_kfold'}
+RELOO_MAX_POINTS = N.MLP_MAX_SPLITS     # refitted points per sample_chains call: one fold each
+
+
+class KfoldResult:
+    """``kfold``: ``pointwise`` (N,) fp64 elpd_i in the original data order; totals (Python floats) ``elpd_kfold``,
+    ``se`` = sqrt(N) sd(pointwise) (ddof 1), ``kfoldic`` = -2 elpd_kfold, ``kfoldic_se``; ``folds`` (N,) (the run's
+    assignment), ``num_folds``, ``num_points``, ``num_draws`` (per fold: R chains x n draws), ``num_nonfinite`` (points
+    with a non-finite draw: NaN elpd_i and NaN totals)."""
+
+    kind = 'kfold'
+
+    def __repr__(self):
+        return ('KfoldResult(elpd_kfold=%.3f, se=%.3f, K=%d, N=%d, S per fold=%d, nonfinite=%d)'
+                % (self.elpd_kfold, self.se, self.num_folds, self.num_points, self.num_draws, self.num_nonfinite))
+
+
+def kfold_split(N_, K, seed=0):
+    """A balanced random assignment of N_ data rows to K folds, as Stan's ``loo::kfold_split_random``: a random
+    permutation from a CPU ``torch.Generator`` seeded with ``seed``, dealt round-robin, so fold sizes differ by at most
+    one and the same seed gives the same (N_,) int64 CPU tensor on every machine.  2 <= K <= min(N_, 64)."""
+    N_, K = int(N_), int(K)
+    if not 2 <= K <= min(N_, N.MLP_MAX_SPLITS):
+        raise ValueError('kfold_split: need 2 <= K <= min(N, %d), got N=%d, K=%d' % (N.MLP_MAX_SPLITS, N_, K))
+    perm = torch.randperm(N_, generator=torch.Generator().manual_seed(int(seed)))
+    f = torch.empty(N_, dtype=torch.int64)
+    f[perm] = torch.arange(N_, dtype=torch.int64) % K
+    return f
+
+
+def _fold_elpd(x, target, f, K):
+    """elpd_i = logsumexp_s ll_is - log S_k (fp64) of every row i with f[i] = k >= 0 under the draws x[k::K] (the chains
+    that fit without fold k), in data order; NaN at rows with f = -1.  The likelihood runs on one fold-ordered copy of
+    the scored rows, where fold k is the row range [start_k, start_k + n_k); the logsumexp is hmcx_loo_pass's lppd term
+    (sorted draws, fixed order), in slabs within the workspace budget.  Returns (elpd (N,), nonfinite count, S_k)."""
+    dev = x.device
+    n_rows = f.numel()
+    order = torch.sort(f, stable=True).indices
+    order = order[f[order] >= 0]
+    counts = torch.bincount(f[order], minlength=K).tolist()
+    ft = copy.copy(target)
+    ft.x, ft.y = target.x[order.to(target.x.device)], target.y.reshape(n_rows, target.y_cols)[order.to(target.y.device)]
+    nt = _native_target(ft, dev)
+    scored = torch.empty(order.numel(), dtype=torch.float64, device=dev)
+    bad, s_k, r0 = 0, 0, 0
+    for k in range(K):
+        pw, _, flag, s_k, _ = _pointwise_pass(x[k::K], ft, 1.0, nt=nt, rows=(r0, r0 + counts[k]))
+        scored[r0:r0 + counts[k]] = pw[3]
+        bad += int((flag != 0).sum())
+        r0 += counts[k]
+    out = torch.full((n_rows,), float('nan'), dtype=torch.float64, device=dev)
+    out[order.to(dev)] = scored
+    return out, bad, s_k
+
+
+def _whole_target(target, prefix):
+    t = _mlp_targets(target, prefix, 'leave out')
+    if isinstance(target, list):
+        raise TypeError('%s: pass the MLPTarget of the whole data set, not a split list' % prefix)
+    return t[0]
+
+
+def kfold(res, target):
+    """K-fold cross-validation of a Bayesian NN from one fold run (``sample_chains(..., folds=f)``, every row in a fold):
+    for each fold k the likelihood of its held-out rows under the draws of chains k::K, through
+    hmcx_mlp_pointwise_ll_tau, and elpd_i = logsumexp_s ll_is - log S_k in fp64 with S_k = R n.  ``target``: the
+    full-data ``MLPTarget`` the run was given.  The same run gives the same bits on every call, whatever the slab size.
+    Returns a ``KfoldResult``."""
+    f = getattr(res, 'folds', None)
+    if f is None:
+        raise TypeError('kfold: expected the result of sample_chains(..., folds=...)')
+    t = _whole_target(target, 'kfold')
+    fc = f.detach().cpu().to(torch.int64)
+    if bool((fc < 0).any()):
+        raise RuntimeError('kfold: the run leaves rows in every fit (fold -1, as reloo assigns them); kfold scores a run '
+                           'that assigns every data row to a fold')
+    if fc.numel() != t.x.shape[0]:
+        raise RuntimeError('kfold: the run assigns %d rows to folds, the target has %d' % (fc.numel(), t.x.shape[0]))
+    K = int(res.num_folds)
+    x = _samples_block(res, t)
+    if x.shape[0] % K:
+        raise RuntimeError('kfold: %d chains are not a multiple of K = %d' % (x.shape[0], K))
+    pw, bad, s_k = _fold_elpd(x, t, fc, K)
+    r = KfoldResult()
+    r.pointwise = pw
+    r.elpd_kfold, r.se = _total(pw)
+    r.kfoldic, r.kfoldic_se = -2.0 * r.elpd_kfold, 2.0 * r.se
+    r.folds, r.num_folds = f, K
+    r.num_points, r.num_draws, r.num_nonfinite = fc.numel(), s_k, bad
+    return r
+
+
+def _reloo_batches(points):
+    """At most RELOO_MAX_POINTS points per batch, in balanced batches (so no batch holds one point unless only one is
+    flagged)."""
+    nb = -(-len(points) // RELOO_MAX_POINTS)
+    out, i = [], 0
+    for b in range(nb):
+        size = len(points) // nb + (1 if b < len(points) % nb else 0)
+        out.append(points[i:i + size])
+        i += size
+    return out
+
+
+def reloo(lo, target, params_init, **sample_kwargs):
+    """Exact refits of the points PSIS-LOO cannot score (ArviZ's ``reloo``): every point with pareto_k above
+    ``lo.k_threshold`` is left out of a fit of its own and scored exactly under it.  The flagged points go in batches of
+    at most 64, each one ``sample_chains`` K-fold run in which every flagged point of the batch is a singleton fold and
+    every other row is -1 (in every fit); ``params_init`` ((R, D) or (D,)) starts the R chains of every fold, and
+    ``sample_kwargs`` (num_samples, step_size, burn, sampler, seed, ...) go to ``sample_chains``.  A lone flagged point
+    is refitted by a plain run on the other rows, which samples the same posterior.  ``target``: the full-data
+    ``MLPTarget`` ``lo`` scored.
+
+    Returns a NEW ``LooResult`` (``lo`` is not modified): refitted points take their exact elpd_i, p_loo_i = lppd_i -
+    elpd_i and pareto_k = 0 (as ArviZ reports them) and are listed in ``refit_points`` (int64); the totals and
+    ``num_bad_k`` are recomputed.  With no flagged point it returns an equal copy and launches nothing."""
+    from . import samplers
+    from .engine import fold_targets
+    if getattr(lo, 'kind', None) != 'loo':
+        raise TypeError('reloo: expected a psis_loo result')
+    t = _whole_target(target, 'reloo')
+    if t.x.shape[0] != lo.num_points:
+        raise RuntimeError('reloo: the result scores %d points, the target has %d data rows'
+                           % (lo.num_points, t.x.shape[0]))
+    if 'folds' in sample_kwargs:
+        raise ValueError('reloo: the folds are the flagged points; do not pass folds')
+    out = LooResult()
+    for k, v in lo.__dict__.items():
+        setattr(out, k, v.clone() if torch.is_tensor(v) else v)
+    bad = torch.nonzero(lo.pareto_k > lo.k_threshold).flatten().cpu()
+    out.refit_points = bad
+    if bad.numel() == 0:
+        return out
+    q0 = params_init if params_init.dim() == 2 else params_init.unsqueeze(0)
+    n_rows = lo.num_points
+    for batch in _reloo_batches(bad.tolist()):
+        K = len(batch)
+        f = torch.full((n_rows,), -1, dtype=torch.int64)
+        f[batch] = torch.arange(K, dtype=torch.int64)
+        if K == 1:                                  # fold 0's training set: every row but the flagged one
+            res = samplers.sample_chains(fold_targets(t, f)[0], q0, **sample_kwargs)
+        else:
+            res = samplers.sample_chains(t, q0.repeat_interleave(K, dim=0), folds=f, **sample_kwargs)
+        e, _, _ = _fold_elpd(_samples_block(res, t), t, f, K)
+        idx = torch.tensor(batch, dtype=torch.int64, device=out.pointwise.device)
+        out.pointwise[idx] = e[idx.to(e.device)].to(out.pointwise.device)
+    idx = bad.to(out.pointwise.device)
+    out.p_loo_i[idx] = out.lppd[idx] - out.pointwise[idx]
+    out.pareto_k[idx] = 0.0
+    out.elpd_loo, out.se = _total(out.pointwise)
+    out.p_loo, out.p_loo_se = _total(out.p_loo_i)
+    out.looic, out.looic_se = -2.0 * out.elpd_loo, 2.0 * out.se
+    out.num_bad_k = int((out.pareto_k > out.k_threshold).sum())
+    return out
+

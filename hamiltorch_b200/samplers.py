@@ -344,7 +344,7 @@ def sample_chains(log_prob_func, params_init, num_samples=10, num_steps_per_samp
                   desired_accept_rate=0.8, rng='philox', seed=0, chain_offset=0, normals=None, log_uniforms=None,
                   record_ham=False, out=None, perms=None, uniforms=None, thin=1, moments=False, keep_samples=True,
                   store_on_GPU=True, host_windows=0, adapt_mass=False, mass_pool=None, tau_prior=None,
-                  tau_out_prior=None, gammas=None, betas=None, swap_every=10, swap_log_uniforms=None):
+                  tau_out_prior=None, gammas=None, betas=None, swap_every=10, swap_log_uniforms=None, folds=None):
     """The engine's native entry: C independent chains at once.  ``params_init`` is (C, D); every chain gets the
     reference's ``sample`` semantics.  Returns an ``engine.HMCResult`` whose ``.samples`` is (C, S-burn, D) on the
     GPU (row c = what ``sample`` would have returned for chain c, stacked).
@@ -400,6 +400,16 @@ def sample_chains(log_prob_func, params_init, num_samples=10, num_steps_per_samp
     gains ``.betas``, ``.swap_accepted`` (rounds, R, T - 1) int8 (-1: the pair was not in that round), ``.swap_ll``
     (rounds, C) fp64 and ``.swap_rate`` (T - 1,).  Not combined with RMHMC, non-BNN targets, a 2-D or block ``inv_mass``,
     ``adapt_mass``, hyperpriors or ``rng='reference'``.
+
+    K-fold refits (an ``MLPTarget`` with data, HMC / HMC_NUTS, the plain integrator; DESIGN §3.18): ``folds`` is an (N,)
+    integer tensor assigning each data row to a fold 0 .. K-1, or to -1 (never left out); K = max + 1, 2 <= K <= 64, and
+    every fold id occurs.  ``params_init`` is (C, D) with C = R K: row r K + k is chain r of the fit WITHOUT fold k, so
+    ``.samples[k::K]`` is fold k's posterior.  That row samples exactly what the same call without ``folds`` samples on
+    the MLPTarget of the rows {i : folds[i] != k} in their original order (the prior counted once, the log-softmax loss
+    a mean over those rows); step size, dual averaging, counters and the sink options stay with the row.  All K fits run
+    in one launch.  ``chain_offset`` must be a multiple of K.  The result gains ``.folds`` (on the device) and
+    ``.num_folds``; ``loo.kfold`` scores it.  Not combined with split lists, SPLITTING integrators, ``betas``,
+    hyperpriors, ``adapt_mass``, RMHMC, a 2-D or block ``inv_mass``, non-BNN targets or ``rng='reference'``.
     """
     if params_init.dim() != 2:
         raise RuntimeError('sample_chains: params_init must be (num_chains, D)')
@@ -410,6 +420,8 @@ def sample_chains(log_prob_func, params_init, num_samples=10, num_steps_per_samp
     hyper = _hyper_groups(log_prob_func, sampler, tau_prior, tau_out_prior)
     temper = _temper_args(log_prob_func, params_init, num_samples, sampler, inv_mass, adapt_mass, hyper, rng,
                           chain_offset, betas, swap_every, swap_log_uniforms)
+    folds = _fold_args(log_prob_func, params_init, sampler, integrator, inv_mass, adapt_mass, hyper, betas, rng,
+                       chain_offset, folds)
     return _run_chains(log_prob_func, params_init, num_samples, num_steps_per_sample, step_size, burn, jitter,
                        inv_mass, softabs_const, explicit_binding_const, fixed_point_threshold,
                        fixed_point_max_iterations, jitter_max_tries, sampler, integrator, metric,
@@ -419,7 +431,55 @@ def sample_chains(log_prob_func, params_init, num_samples=10, num_steps_per_samp
                        sink=dict(thin=thin, moments=moments, keep_samples=keep_samples, host_samples=not store_on_GPU,
                                  host_windows=host_windows, **(dict(adapt_mass=True, mass_pool=mass_pool)
                                                                if adapt_mass else {})),
-                       hyper=hyper, gammas=gammas, temper=temper)
+                       hyper=hyper, gammas=gammas, temper=temper, folds=folds)
+
+
+def _fold_args(log_prob_func, params_init, sampler, integrator, inv_mass, adapt_mass, hyper, betas, rng, chain_offset,
+               folds):
+    """sample_chains(folds=...) -> the (N,) int64 CPU assignment engine.hmc_run takes (None without folds), checked
+    before any CUDA work."""
+    if folds is None:
+        return None
+    if isinstance(log_prob_func, list) or integrator in _SPLIT_INTEGRATORS:
+        raise NotImplementedError('K-fold runs: not with split lists or SPLITTING integrators -- pass the MLPTarget of '
+                                  'the whole data set with the plain integrator')
+    if not isinstance(log_prob_func, T.MLPTarget):
+        raise NotImplementedError('K-fold runs: Bayesian-NN targets only (an MLPTarget)')
+    if sampler not in (Sampler.HMC, Sampler.HMC_NUTS):
+        raise NotImplementedError('K-fold runs: sampler HMC or HMC_NUTS (not RMHMC)')
+    if log_prob_func.x is None:
+        raise RuntimeError('K-fold runs: the target has no data (x is None): there are no rows to leave out')
+    if isinstance(inv_mass, list) or (torch.is_tensor(inv_mass) and inv_mass.dim() != 1):
+        raise NotImplementedError('K-fold runs: inv_mass None or 1-D')
+    if betas is not None:
+        raise NotImplementedError('K-fold runs are not combined with replica exchange (betas)')
+    if hyper is not None:
+        raise NotImplementedError('K-fold runs are not combined with hyperpriors (tau_prior / tau_out_prior)')
+    if adapt_mass:
+        raise NotImplementedError('K-fold runs are not combined with adapt_mass: it would pool one mass across the '
+                                  'different posteriors of the folds')
+    if rng == 'reference':
+        raise NotImplementedError("K-fold runs: rng='philox' or 'injected' (the reference stream is one chain)")
+    if not torch.is_tensor(folds) or folds.dtype.is_floating_point or folds.dtype.is_complex or \
+            folds.dtype == torch.bool:
+        raise ValueError('folds must be an integer tensor, got %s' % (folds.dtype if torch.is_tensor(folds)
+                                                                      else type(folds).__name__))
+    f = folds.detach().to('cpu', torch.int64)
+    Nr = log_prob_func.x.shape[0]
+    if f.dim() != 1 or f.numel() != Nr:
+        raise ValueError('folds must be (N,) = (%d,), one fold per data row, got %s' % (Nr, tuple(folds.shape)))
+    K = int(f.max()) + 1
+    if int(f.min()) < -1 or not 2 <= K <= N.MLP_MAX_SPLITS:
+        raise ValueError('folds must hold values in -1 .. K-1 with 2 <= K <= %d, got min %d, max %d'
+                         % (N.MLP_MAX_SPLITS, int(f.min()), K - 1))
+    missing = [k for k in range(K) if not bool((f == k).any())]
+    if missing:
+        raise ValueError('folds: every fold id 0 .. K-1 must occur; missing %s' % missing)
+    if params_init.shape[0] % K != 0:
+        raise ValueError('K-fold runs: params_init has %d rows, not a multiple of K = %d' % (params_init.shape[0], K))
+    if int(chain_offset) % K != 0:
+        raise ValueError('K-fold runs: chain_offset %d is not a multiple of K = %d' % (chain_offset, K))
+    return f
 
 
 def _temper_args(log_prob_func, params_init, num_samples, sampler, inv_mass, adapt_mass, hyper, rng, chain_offset,
@@ -535,11 +595,13 @@ def _run_chains(log_prob_func, q0, num_samples, L, step_size, burn, jitter, inv_
                 explicit_binding_const, fixed_point_threshold, fixed_point_max_iterations, jitter_max_tries,
                 sampler, integrator, metric, desired_accept_rate, rng='philox', seed=None, chain_offset=0,
                 normals=None, log_uniforms=None, record_ham=False, out=None, injected_perms=None,
-                injected_uniforms=None, sink=None, hyper=None, gammas=None, temper=None):
+                injected_uniforms=None, sink=None, hyper=None, gammas=None, temper=None, folds=None):
     nuts = sampler == Sampler.HMC_NUTS
     hyper_kw = {} if hyper is None else dict(hyper=hyper)
     if temper is not None:
         hyper_kw['temper'] = temper
+    if folds is not None:
+        hyper_kw['folds'] = folds
     gshapes = None if hyper is None else _reference_gamma_shapes(log_prob_func, hyper)
     sink = sink or {}
     if (sink.get('thin', 1) != 1 or sink.get('moments') or not sink.get('keep_samples', True) or

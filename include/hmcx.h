@@ -531,6 +531,26 @@ int hmcx_temper_swap(float* q_cur, int32_t C, int32_t ld, int32_t num_temps, con
                      int32_t round, const hmcx_rng_t* rng, const double* log_uniforms, int8_t* accepted, void* stream);
 
 /*
+ * K-fold refits of a Bayesian NN in one launch (additive v12 symbol; DESIGN §3.18).  Callers of an older v12 library check
+ * for the symbol.  hmcx_split_run_sink (sink may be NULL) with the target's K = num_folds splits read as K training sets:
+ * split k holds the rows of fold k's fit (every row not in fold k, in data order).  The chain with GLOBAL id
+ * g = rng->chain_offset + c evaluates split g mod K as its whole potential -- ll of that split plus the prior once -- in
+ * every gradient, both Hamiltonians and the gradient carried between iterations, i.e. it samples what hmcx_split_run_sink
+ * with HMCX_SCHEME_PLAIN samples on a target holding split k alone.  The automatic cluster size counts the tiles of the
+ * smallest split, a whole training set.  Checked before any CUDA work: NULL target, num_folds < 2 or
+ * > HMCX_MLP_MAX_SPLITS, num_splits != num_folds, a target without data, the sink checks of hmcx_split_run_sink:
+ * HMCX_ERR_INVALID_ARG; non-MLP targets and a scheme other than HMCX_SCHEME_PLAIN: HMCX_ERR_UNSUPPORTED; otherwise the
+ * checks of hmcx_split_run_sink.
+ */
+int hmcx_split_run_folds(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmcx_rng_t* rng,
+                         const hmcx_nuts_t* nuts, int32_t scheme,
+                         const float* q_init, float* q_cur, float* eps,
+                         int32_t C, int32_t ld, int32_t L, int32_t num_samples, int32_t burn,
+                         int32_t iter_begin, int32_t iter_end,
+                         float* samples_out, uint8_t* accept_out, uint8_t* diverged_out, float* ham_out,
+                         int32_t* num_rejected, const hmcx_sink_t* sink, int32_t num_folds, void* stream);
+
+/*
  * hmcx_adapt_diag_mass (ABI v11): the pooled diagonal mass estimate at the end of a warm-up window (Stan's windowed
  * adaptation, regularised as Stan does) and the restart of the dual averaging that follows it.  One pass, fixed order, no
  * atomics.  Inputs: the per-chain compensated sums of a window of n >= 2 draws, [C, ld] each, as a sink launch with
