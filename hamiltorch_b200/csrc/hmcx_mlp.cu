@@ -947,14 +947,14 @@ __device__ __forceinline__ float mlp_log_prior(const MlpDev& m, const float* q, 
 }
 
 // log p(q) = sum over splits of (ll_m + l_prior/prior_scale)  (hamiltonian's split loop, samplers.py:787-796);
-// with s >= 0 only that split.  Optionally writes the network outputs (predict_model) and, to every thread's *sse_out, the
-// loss sums of the splits added in fp64 in split order (the regression SSE the tau_out Gibbs step needs).
+// with s >= 0 only that split.  Optionally writes the network outputs (predict_model) and, to every thread's *lsum_out,
+// the sum over splits of ll_m / c_ll added in fp64 in split order: the untempered log-likelihood over c_ll, and for
+// regression the SSE the tau_out Gibbs step needs.
 template <int CS>
 __device__ __forceinline__ float mlp_log_prob(const MlpDev& m, const float* q, float* tile, float* sred, int s,
                                               float* pred_out, ClusterCtx cc, float* xslot, TcCtx& tc,
-                                              double* sse_out = nullptr, double* lsum_out = nullptr) {
+                                              double* lsum_out = nullptr) {
     const float prior_term = __fdiv_rn(mlp_log_prior(m, q, sred), m.prior_scale);
-    if (sse_out) *sse_out = 0.0;
     if (lsum_out) *lsum_out = 0.0;
     if (!m.has_data) return prior_term;
     TcEpi te;
@@ -993,8 +993,7 @@ __device__ __forceinline__ float mlp_log_prob(const MlpDev& m, const float* q, f
         block_sum<1>(sse, sred);
         __syncthreads();
         sse[0] = cluster_sum_scalar<CS>(sse[0], xslot);
-        if (sse_out) *sse_out += (double)sse[0];
-        // lsum_out: the sum over splits of ll_m / c_ll in fp64 -- the log-softmax loss is a per-split mean
+        // (the log-softmax loss is a per-split mean)
         if (lsum_out)
             *lsum_out += m.loss == HMCX_LOSS_MULTICLASS_LOGSOFTMAX ? (double)sse[0] / (double)(m.sb[sp + 1] - m.sb[sp])
                                                                    : (double)sse[0];
@@ -1009,8 +1008,8 @@ __device__ __forceinline__ float mlp_log_prob(const MlpDev& m, const float* q, f
 // ---------------------------------------------------------------------------------------------------------
 constexpr int HYPER_GROUPS = 2 * HMCX_MLP_MAX_LAYERS + 1;     // the parameter tensors, then tau_out
 
-// Gamma hyperpriors on the precisions (hmcx_hyper_t), read by the HYPER instantiations only.  Group k < 2L is parameter
-// tensor k (tau_list order), group 2L the regression likelihood's tau_out.
+// Gamma hyperpriors on the precisions (hmcx_hyper_t), read by the PER_CHAIN instantiations only (tau == NULL: none).
+// Group k < 2L is parameter tensor k (tau_list order), group 2L the regression likelihood's tau_out.
 struct MlpHyperDev {
     int sampled;                  // bit k: group k is Gibbs-updated
     double a[HYPER_GROUPS], b[HYPER_GROUPS];
@@ -1022,32 +1021,27 @@ struct MlpHyperDev {
     const double* gammas;         // INJECTED: standard-gamma draws [it1 - it0, C, 2L + 1]
 };
 
-// A HYPER kernel reads the model descriptor from a shared-memory copy whose prior constants and c_ll follow the chain's
-// current precisions (the constant bank holds the launch-wide ones).
-struct HyperSm {
+// A PER_CHAIN kernel reads the model descriptor from a shared-memory copy whose constants are the chain's own: the prior
+// constants and c_ll of its current precisions, or its rung's tau_out and c_ll (the constant bank holds the launch-wide
+// ones).
+struct ChainModelSm {
     MlpDev m;
     double red[MLP_THREADS / 32];
     double ssq[2 * HMCX_MLP_MAX_LAYERS];
     float tau[2 * HMCX_MLP_MAX_LAYERS];
     float tau_out;
 };
-__device__ __forceinline__ HyperSm& hyper_sm() {
-    __shared__ HyperSm s;
+__device__ __forceinline__ ChainModelSm& chain_model_sm() {
+    __shared__ ChainModelSm s;
     return s;
 }
-// Replica exchange (hmcx_temper_t), read by the TEMPER instantiations only: row c runs rung c % T, whose likelihood
+// Replica exchange (hmcx_temper_t), read by the PER_CHAIN instantiations only: row c runs rung c % T, whose likelihood
 // precision tau_out[c % T] replaces the target's (the power posterior at beta_t, DESIGN.md 3.17)
 struct MlpTemperDev {
-    int T;
+    int T;                        // 0: no replica exchange
     float tau_out[HMCX_TEMPER_MAX_TEMPS];
     double* ll_out;               // [C] or NULL: the untempered log-likelihood at q_cur when the launch ends
 };
-
-template <bool HYPER>
-__device__ __forceinline__ const MlpDev& run_model(const MlpDev& m) {
-    if constexpr (HYPER) return hyper_sm().m;
-    else return m;
-}
 
 // The prior constants of the sampled tensors and c_ll from the precisions, in fp32 with the host's operation order
 // (targets.MLPTarget.__init__: scale = tau ** -0.5, two_var = 2 * scale ** 2, log_scale = log(scale),
@@ -1110,17 +1104,17 @@ struct MlpRunArgs {
     const float* p_given;         // [C, ld] or NULL
     float* q_traj;                // [L, C, ld]: params after every step (ret_params)
     float* p_traj;                // [L, C, ld]: momentum after every step (ret_momenta)
-    // sample sink (hmcx_sink_t), read by the SINK instantiations only: thinning + running moments of the post-burn states
+    // sample sink (hmcx_sink_t; {thin = 1} when the caller gives none): thinning + running moments of the post-burn states
     int thin;
     float* msum;
     float* msumsq;
     float* msum_lo;               // optional compensation terms (true sum = hi + lo)
     float* msumsq_lo;
-    // mass adaptation (ABI v11), SINK only: moments over every iteration of the launch; per-chain mu (may be null)
+    // mass adaptation (ABI v11): moments over every iteration of the launch; per-chain mu (may be null)
     int moments_all;
     const double* mu_chain;
-    MlpHyperDev hy;               // HYPER instantiations only
-    MlpTemperDev tp;              // TEMPER instantiations only
+    MlpHyperDev hy;               // PER_CHAIN instantiations only
+    MlpTemperDev tp;              // PER_CHAIN instantiations only
     int folds;                    // K-fold (PLAIN only, 0 = off): global chain g's whole potential is split g % folds
 };
 
@@ -1149,12 +1143,13 @@ __device__ __forceinline__ void sink_accumulate(float* hi, float* lo, size_t off
     *reinterpret_cast<float4*>(hi + off) = s;
 }
 
-// SINK = false: the plain sample() loop (rank 0 stores every post-burn row); SINK = true adds the sample sink, its row
-// work divided over the cluster's ranks (see sink_row below).  HYPER (with SINK only) adds the Gibbs updates of the Gamma
-// hyperpriors on the precisions after every MH step (DESIGN.md 3.15).  TEMPER (with SINK only) runs row c at rung c % T of
-// a replica-exchange ladder: its descriptor copy carries the rung's tau_out, it tracks the untempered log-likelihood at
-// q_cur, and only rung 0 (beta = 1) rows store samples, to row c / T of samples_out (DESIGN.md 3.17).
-template <int CS, bool SINK, bool HYPER = false, bool TEMPER = false>
+// The sample() loop with the sample sink, its row work divided over the cluster's ranks (see sink_row below).  PER_CHAIN:
+// the chain's model constants live in a shared-memory copy of the descriptor, which the launch's settings fill.
+// Hyperpriors (a.hy.tau != NULL) add the Gibbs updates of the Gamma hyperpriors on the precisions after every MH step
+// (DESIGN.md 3.15).  Replica exchange (a.tp.T > 0) runs row c at rung c % T of a ladder: its descriptor copy carries the
+// rung's tau_out, it tracks the untempered log-likelihood at q_cur, and only rung 0 (beta = 1) rows store samples, to row
+// c / T of samples_out (DESIGN.md 3.17).  Both are tested once per launch or per iteration, never inside the trajectory.
+template <int CS, bool PER_CHAIN>
 __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArgs a) {
     extern __shared__ __align__(128) float sm[];
     __shared__ float sred[64];
@@ -1163,30 +1158,26 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
     __shared__ int s_perm[HMCX_MLP_MAX_SPLITS];
     __shared__ __align__(8) uint64_t s_bars[3];
 
-    static_assert(SINK || !HYPER, "the hyperprior form is a sink form");
-    static_assert((SINK && !HYPER) || !TEMPER, "the tempered form is a sink form without hyperpriors");
-    if constexpr (HYPER) {                                     // this chain's precisions and the constants they give
-        HyperSm& hs = hyper_sm();
+    const bool hyper = PER_CHAIN && a.hy.tau, temper = PER_CHAIN && a.tp.T > 0;
+    if constexpr (PER_CHAIN) {
+        ChainModelSm& cm = chain_model_sm();
         if (threadIdx.x == 0) {
             const int c0 = blockIdx.x / CS, K = 2 * a.m.L;
-            hs.m = a.m;
-            for (int k = 0; k < K; ++k) hs.tau[k] = a.hy.tau[(size_t)c0 * K + k];
-            hs.tau_out = a.hy.tau_out[c0];
-            hyper_constants(hs.m, hs.tau, hs.tau_out, a.hy.sampled);
+            cm.m = a.m;
+            if (hyper) {                                       // this chain's precisions and the constants they give
+                for (int k = 0; k < K; ++k) cm.tau[k] = a.hy.tau[(size_t)c0 * K + k];
+                cm.tau_out = a.hy.tau_out[c0];
+                hyper_constants(cm.m, cm.tau, cm.tau_out, a.hy.sampled);
+            }
+            if (temper) {                                      // the rung's tau_out and c_ll, as fill_mlp derives them
+                const float tau = a.tp.tau_out[c0 % a.tp.T];
+                cm.m.tau_out = tau;
+                cm.m.c_ll = (a.m.loss == HMCX_LOSS_REGRESSION) ? (float)(-0.5 * (double)tau) : (float)(-(double)tau);
+            }
         }
         __syncthreads();
     }
-    if constexpr (TEMPER) {                                    // the rung's tau_out and c_ll, as fill_mlp derives them
-        HyperSm& hs = hyper_sm();
-        if (threadIdx.x == 0) {
-            const float tau = a.tp.tau_out[(blockIdx.x / CS) % a.tp.T];
-            hs.m = a.m;
-            hs.m.tau_out = tau;
-            hs.m.c_ll = (a.m.loss == HMCX_LOSS_REGRESSION) ? (float)(-0.5 * (double)tau) : (float)(-(double)tau);
-        }
-        __syncthreads();
-    }
-    const MlpDev& m = run_model<HYPER || TEMPER>(a.m);
+    const MlpDev& m = PER_CHAIN ? chain_model_sm().m : a.m;
     ClusterCtx cc = {0, 1};
     if (CS > 1) { cc.rank = (int)cg::this_cluster().block_rank(); cc.size = CS; }
     const bool lead = cc.rank == 0;                            // rank 0 owns every global-memory output but the sink rows
@@ -1199,30 +1190,27 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
     const uint64_t chain_id = a.chain_offset + (uint64_t)c;
     // the data split that is this chain's whole PLAIN potential: -1 (every split) unless a K-fold run gives the chain
     // fold k = g mod K's training rows, split k (DESIGN.md 3.18).  The host refuses folds with hyperpriors or tempering:
-    // those forms keep a constant -1 and compile as before.
-    const int psp = (!HYPER && !TEMPER && a.folds) ? (int)(chain_id % (uint64_t)a.folds) : -1;
+    // the PER_CHAIN form keeps a constant -1 (one more live value there raises its spills).
+    const int psp = (!PER_CHAIN && a.folds) ? (int)(chain_id % (uint64_t)a.folds) : -1;
     TcCtx tc = {};
     if (m.tc) tc_init(tc, s_bars);
 
     for (int i = tid; i < m.Dp; i += MLP_THREADS) { q[i] = i < D ? a.q_cur[row + i] : 0.0f; p[i] = 0.0f; g[i] = 0.0f; }
     __syncthreads();
-    double sse_cur = 0.0, sse_new = 0.0;                      // HYPER: the loss sum at q_cur / at the proposal
-    double ls_cur = 0.0, ls_new = 0.0;                        // TEMPER: untempered log-likelihood / c_ll, likewise
+    double ls_cur = 0.0, ls_new = 0.0;                        // PER_CHAIN: log-likelihood / c_ll at q_cur / the proposal
     float lp_cur = a.p_given ? 0.0f : mlp_log_prob<CS>(m, q, tile, sred, psp, nullptr, cc, &s_xchg, tc,
-                                                       HYPER ? &sse_cur : nullptr, TEMPER ? &ls_cur : nullptr);
+                                                       PER_CHAIN ? &ls_cur : nullptr);
 
     float eps = a.eps[c];
     double h_bar = 0.0, eps_bar = 1.0;
     if (a.nuts && tid == 0) { h_bar = a.h_bar[c]; eps_bar = a.eps_bar[c]; }
-    double mu_sink = 0.0;                                      // SINK: this chain's mu (the restarted dual averaging's)
-    if constexpr (SINK) {
-        if (a.nuts && tid == 0) mu_sink = a.mu_chain ? a.mu_chain[c] : a.mu;
-    }
+    double mu_sink = 0.0;                                      // this chain's mu (the restarted dual averaging's)
+    if (a.nuts && tid == 0) mu_sink = a.mu_chain ? a.mu_chain[c] : a.mu;
     int rejected = 0;
-    const int keep = SINK ? 1 + (a.S - a.burn - 1) / a.thin : a.S - a.burn;      // slots per chain in samples_out
-    float* const my_samples = TEMPER ? ((a.samples && c % a.tp.T == 0) ? a.samples + (size_t)(c / a.tp.T) * keep * a.ld
+    const int keep = 1 + (a.S - a.burn - 1) / a.thin;                      // slots per chain in samples_out
+    float* const my_samples = temper ? ((a.samples && c % a.tp.T == 0) ? a.samples + (size_t)(c / a.tp.T) * keep * a.ld
                                                                        : nullptr)
-                                     : ((a.samples && (SINK || lead)) ? a.samples + (size_t)c * keep * a.ld : nullptr);
+                                     : (a.samples ? a.samples + (size_t)c * keep * a.ld : nullptr);
     // Sink: rank r owns the float4 vectors [sv0, sv1) of the row -- their thinned stores (16-byte streaming stores, which is
     // what lets rows leave over PCIe when samples_out is pinned host memory) and their moment updates.  Every rank holds a
     // bit-identical replica of q, so this needs no DSMEM traffic and no barrier beyond the loop's own.
@@ -1237,23 +1225,18 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
             if (moments && a.msumsq) sink_accumulate(a.msumsq, a.msumsq_lo, row + 4 * v, x, true);
         }
     };
-    if (a.it0 == 0 && my_samples) {
-        if constexpr (SINK) sink_row(my_samples, false);
-        else for (int i = tid; i < a.ld; i += MLP_THREADS) my_samples[i] = i < D ? q[i] : 0.0f;
-    }
-    // HYPER: the precisions of retained slot j (the slots of samples_out, thinned alike); slot 0 = the initial values
+    if (a.it0 == 0 && my_samples) sink_row(my_samples, false);
+    // hyperpriors: the precisions of retained slot j (the slots of samples_out, thinned alike); slot 0 = the initial values
     auto hyper_store = [&](int slot) {
-        if constexpr (HYPER) {
-            if (tid == 0 && lead) {
-                const HyperSm& hs = hyper_sm();
-                const int K = 2 * m.L;
-                if (a.hy.tau_trace)
-                    for (int k = 0; k < K; ++k) a.hy.tau_trace[((size_t)c * keep + slot) * K + k] = hs.tau[k];
-                if (a.hy.tau_out_trace) a.hy.tau_out_trace[(size_t)c * keep + slot] = hs.tau_out;
-            }
+        if (tid == 0 && lead) {
+            const ChainModelSm& cm = chain_model_sm();
+            const int K = 2 * m.L;
+            if (a.hy.tau_trace)
+                for (int k = 0; k < K; ++k) a.hy.tau_trace[((size_t)c * keep + slot) * K + k] = cm.tau[k];
+            if (a.hy.tau_out_trace) a.hy.tau_out_trace[(size_t)c * keep + slot] = cm.tau_out;
         }
     };
-    if (a.it0 == 0) hyper_store(0);
+    if (hyper && a.it0 == 0) hyper_store(0);
 
     auto kinetic = [&]() {                                    // 2*K: p.p or p.(im*p)   (samplers.py:801, :814)
         float s[1] = {0.0f};
@@ -1527,8 +1510,8 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
         }
         if (a.p_given) break;                                             // stand-alone leapfrog: no Hamiltonian, no MH
         // ---- Hamiltonians + MH ----
-        const float lp_new = mlp_log_prob<CS>(m, q, tile, sred, psp, nullptr, cc, &s_xchg, tc, HYPER ? &sse_new : nullptr,
-                                              TEMPER ? &ls_new : nullptr);
+        const float lp_new = mlp_log_prob<CS>(m, q, tile, sred, psp, nullptr, cc, &s_xchg, tc,
+                                              PER_CHAIN ? &ls_new : nullptr);
         const float kin1 = kinetic();
         const float h_old = add(-lp_cur, mul(0.5f, kin0));
         const float h_new = add(-lp_new, mul(0.5f, kin1));
@@ -1543,8 +1526,7 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
         const bool acc = !bad && (rho >= logu);
         if (acc) {
             lp_cur = lp_new;
-            if constexpr (HYPER) sse_cur = sse_new;
-            if constexpr (TEMPER) ls_cur = ls_new;
+            if constexpr (PER_CHAIN) ls_cur = ls_new;
             if (lead) for (int i = tid; i < D; i += MLP_THREADS) a.q_cur[row + i] = q[i];
         } else {
             ++rejected;
@@ -1553,17 +1535,17 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
             for (int i = tid; i < D; i += MLP_THREADS) q[i] = src[row + i];
             __syncthreads();
             if (n == a.burn + 1) {
-                lp_cur = mlp_log_prob<CS>(m, q, tile, sred, psp, nullptr, cc, &s_xchg, tc, HYPER ? &sse_cur : nullptr,
-                                          TEMPER ? &ls_cur : nullptr);
+                lp_cur = mlp_log_prob<CS>(m, q, tile, sred, psp, nullptr, cc, &s_xchg, tc,
+                                          PER_CHAIN ? &ls_cur : nullptr);
                 if (lead) for (int i = tid; i < D; i += MLP_THREADS) a.q_cur[row + i] = q[i];
             }
         }
         if (CS > 1) cg::this_cluster().sync();                 // q_cur is stable before any rank re-reads it
-        if constexpr (HYPER) {
+        if (hyper) {
             // Gibbs step of the precisions given q_n: tau_k ~ Gamma(a_k + n_k/2, b_k + |w_k|^2/2), tau_out ~ Gamma(a_o + N O/2,
-            // b_o + SSE(q_n)/2).  |w_k|^2 is a fixed-order fp64 sum over every rank's identical replica of q, SSE the cluster
-            // sum of the MH evaluation at q_cur, so every rank draws the same precisions.
-            HyperSm& hs = hyper_sm();
+            // b_o + SSE(q_n)/2).  |w_k|^2 is a fixed-order fp64 sum over every rank's identical replica of q, SSE (ls_cur, a
+            // regression run's) the cluster sum of the MH evaluation at q_cur, so every rank draws the same precisions.
+            ChainModelSm& cm = chain_model_sm();
             const int K = 2 * m.L;
             __syncthreads();                                   // nobody reads the constants thread 0 rewrites below
             for (int t = 0; t < K; ++t) {
@@ -1572,23 +1554,23 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
                 const int cnt = (t & 1) ? m.n[l + 1] : m.n[l] * m.n[l + 1];
                 double ss = 0.0;
                 for (int i = tid; i < cnt; i += MLP_THREADS) { const double w = (double)q[off + i]; ss = fma(w, w, ss); }
-                ss = block_sum_d(ss, hs.red);
-                if (tid == 0) hs.ssq[t] = ss;
+                ss = block_sum_d(ss, cm.red);
+                if (tid == 0) cm.ssq[t] = ss;
             }
             if (tid == 0) {
                 for (int k = 0; k <= K; ++k) {
                     if (!((a.hy.sampled >> k) & 1)) continue;
                     const int l = k >> 1;
                     const double nk = k < K ? (double)((k & 1) ? m.n[l + 1] : m.n[l] * m.n[l + 1]) : a.hy.n_obs;
-                    const double shape = a.hy.a[k] + 0.5 * nk, rate = a.hy.b[k] + 0.5 * (k < K ? hs.ssq[k] : sse_cur);
+                    const double shape = a.hy.a[k] + 0.5 * nk, rate = a.hy.b[k] + 0.5 * (k < K ? cm.ssq[k] : ls_cur);
                     const double g = a.rng_mode == HMCX_RNG_INJECTED
                                          ? a.hy.gammas[((size_t)(n - a.it0) * a.C + c) * (K + 1) + k]
                                          : philox_std_gamma(a.seed, chain_id, (uint64_t)n, (uint32_t)k, shape);
                     const float tau = (float)(g / rate);
-                    if (k < K) hs.tau[k] = tau;
-                    else hs.tau_out = tau;
+                    if (k < K) cm.tau[k] = tau;
+                    else cm.tau_out = tau;
                 }
-                hyper_constants(hs.m, hs.tau, hs.tau_out, a.hy.sampled);
+                hyper_constants(cm.m, cm.tau, cm.tau_out, a.hy.sampled);
             }
             __syncthreads();
             // log p(q_cur) and any carried gradient belong to the old precisions: re-evaluate the former, drop the latter
@@ -1596,16 +1578,11 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
             g_fresh = false;
             if (n > a.burn && (n - a.burn) % a.thin == 0) hyper_store((n - a.burn) / a.thin);
         }
-        if constexpr (SINK) {
-            if (n > a.burn)
-                sink_row((my_samples && (n - a.burn) % a.thin == 0) ? my_samples + (size_t)((n - a.burn) / a.thin) * a.ld
-                                                                    : nullptr, true);
-            else if (a.moments_all)
-                sink_row(nullptr, true);                                   // a warm-up window's moments
-        } else if (n > a.burn && my_samples) {
-            float* dst = my_samples + (size_t)(n - a.burn) * a.ld;
-            for (int i = tid; i < a.ld; i += MLP_THREADS) dst[i] = i < D ? q[i] : 0.0f;
-        }
+        if (n > a.burn)
+            sink_row((my_samples && (n - a.burn) % a.thin == 0) ? my_samples + (size_t)((n - a.burn) / a.thin) * a.ld
+                                                                : nullptr, true);
+        else if (a.moments_all)
+            sink_row(nullptr, true);                                       // a warm-up window's moments
         if (tid == 0 && lead) {
             const size_t o = (size_t)c * a.S + n;
             if (a.accept) a.accept[o] = acc ? 1 : 0;
@@ -1619,7 +1596,7 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
                     const double* T = a.table + 5 * (size_t)n;
                     const double alpha = bad ? 0.0 : (double)expf(rho);
                     h_bar = __dadd_rn(__dmul_rn(T[0], h_bar), __dmul_rn(T[1], a.delta - alpha));
-                    const double x_new = (SINK ? mu_sink : a.mu) - __dmul_rn(T[2], h_bar);
+                    const double x_new = mu_sink - __dmul_rn(T[2], h_bar);
                     e = expf((float)x_new);
                     const float xb = add((float)__dmul_rn(T[3], x_new), mul((float)T[4], logf((float)eps_bar)));
                     eps_bar = (double)expf(xb);
@@ -1635,16 +1612,13 @@ __global__ void __launch_bounds__(MLP_THREADS, 1) mlp_run_kernel(const MlpRunArg
         }
         __syncthreads();
     }
-    if constexpr (HYPER) {
-        if (tid == 0 && lead) {
-            const HyperSm& hs = hyper_sm();
-            for (int k = 0; k < 2 * m.L; ++k) a.hy.tau[(size_t)c * 2 * m.L + k] = hs.tau[k];
-            a.hy.tau_out[c] = hs.tau_out;
-        }
+    if (hyper && tid == 0 && lead) {
+        const ChainModelSm& cm = chain_model_sm();
+        for (int k = 0; k < 2 * m.L; ++k) a.hy.tau[(size_t)c * 2 * m.L + k] = cm.tau[k];
+        a.hy.tau_out[c] = cm.tau_out;
     }
-    if constexpr (TEMPER) {                                    // the untempered c_ll is the constant bank's
-        if (tid == 0 && lead && a.tp.ll_out) a.tp.ll_out[c] = (double)a.m.c_ll * ls_cur;
-    }
+    if (temper && tid == 0 && lead && a.tp.ll_out)           // the untempered c_ll is the constant bank's
+        a.tp.ll_out[c] = (double)a.m.c_ll * ls_cur;
     if (tid == 0 && lead && !a.p_given) {
         a.eps[c] = eps;
         if (a.nuts) { a.h_bar[c] = h_bar; a.eps_bar[c] = eps_bar; }
@@ -1850,7 +1824,7 @@ static bool mlp_tc_shape(const MlpDev& m) {
 }
 
 // tensor-core layout of the tile area (one-hidden-layer stacks n0 -> 128 -> nL, see the tensor-core section above);
-// `reserve`: static shared memory a kernel form holds beyond the common headroom (HyperSm for the HYPER forms)
+// `reserve`: static shared memory a kernel form holds beyond the common headroom (ChainModelSm for the PER_CHAIN forms)
 static bool mlp_layout_tc(MlpDev& m, int state_vectors, size_t reserve) {
     if (!mlp_tc_shape(m) || !m.xp) return false;
     const int n0 = m.n[0];
@@ -1965,14 +1939,12 @@ int mlp_split_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hm
                   const hmcx_sink_t* sink, const hmcx_hyper_t* hyper, const hmcx_temper_t* temper, int folds) {
     MlpRunArgs a = {};
     hmcx_sink_t thin1 = {};
-    if ((hyper || temper) && !sink) { thin1.thin = 1; sink = &thin1; }    // the hyperprior and tempered forms are sink forms
+    if (!sink) { thin1.thin = 1; sink = &thin1; }              // every run is a sink run: no sink = {thin = 1}
     a.p_given = p_given; a.q_traj = q_traj; a.p_traj = p_traj;
-    if (sink) {
-        a.thin = sink->thin; a.msum = sink->sum; a.msumsq = sink->sumsq;
-        a.msum_lo = sink->sum_lo; a.msumsq_lo = sink->sumsq_lo;
-        a.moments_all = sink->moments_all;
-        if (nuts && nuts->enabled) a.mu_chain = nuts->mu_chain;
-    }
+    a.thin = sink->thin; a.msum = sink->sum; a.msumsq = sink->sumsq;
+    a.msum_lo = sink->sum_lo; a.msumsq_lo = sink->sumsq_lo;
+    a.moments_all = sink->moments_all;
+    if (nuts && nuts->enabled) a.mu_chain = nuts->mu_chain;
     int rc = fill_mlp(target, a.m);
     if (rc != HMCX_OK) return rc;
     const int mk = mass ? mass->kind : HMCX_MASS_NONE;
@@ -2040,7 +2012,7 @@ int mlp_split_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hm
     }
     a.q_init = q_init; a.q_cur = q_cur; a.eps = eps; a.L = L; a.S = S; a.burn = burn; a.it0 = it0; a.it1 = it1;
     a.samples = samples; a.accept = accept; a.diverged = diverged; a.ham = ham; a.num_rejected = num_rejected;
-    if (!mlp_pick_tile(a.m, 3, target->mlp->tensor_cores != HMCX_MLP_TC_OFF, (hyper || temper) ? sizeof(HyperSm) : 0))
+    if (!mlp_pick_tile(a.m, 3, target->mlp->tensor_cores != HMCX_MLP_TC_OFF, (hyper || temper) ? sizeof(ChainModelSm) : 0))
         return HMCX_ERR_UNSUPPORTED;                            // q, p, g do not fit one SM's shared memory
     const size_t smem = (size_t)(a.m.tile_base + a.m.tile_floats) * sizeof(float);
     // CTAs per chain (thread-block cluster size): at most the tiles of the smallest split, at most 4, and -- unless the
@@ -2067,13 +2039,8 @@ int mlp_split_run(const hmcx_target_t* target, const hmcx_mass_t* mass, const hm
     attr[0].val.clusterDim.x = cs; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
     void (*kern)(MlpRunArgs);
-    if (temper)
-        kern = cs == 4 ? mlp_run_kernel<4, true, false, true>
-                       : cs == 2 ? mlp_run_kernel<2, true, false, true> : mlp_run_kernel<1, true, false, true>;
-    else if (hyper) kern = cs == 4 ? mlp_run_kernel<4, true, true> : cs == 2 ? mlp_run_kernel<2, true, true> : mlp_run_kernel<1, true, true>;
-    else if (cs == 4) kern = sink ? mlp_run_kernel<4, true> : mlp_run_kernel<4, false>;
-    else if (cs == 2) kern = sink ? mlp_run_kernel<2, true> : mlp_run_kernel<2, false>;
-    else kern = sink ? mlp_run_kernel<1, true> : mlp_run_kernel<1, false>;
+    if (hyper || temper) kern = cs == 4 ? mlp_run_kernel<4, true> : cs == 2 ? mlp_run_kernel<2, true> : mlp_run_kernel<1, true>;
+    else kern = cs == 4 ? mlp_run_kernel<4, false> : cs == 2 ? mlp_run_kernel<2, false> : mlp_run_kernel<1, false>;
     rc = prepare_smem(kern, smem);
     if (rc != HMCX_OK) return rc;
     if (cudaLaunchKernelEx(&cfg, kern, a) != cudaSuccess) { cudaGetLastError(); return HMCX_ERR_CUDA; }
@@ -2165,7 +2132,7 @@ int mlp_leapfrog(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmc
                          0);
 }
 
-// hmcx_hyper_gamma_draws: one thread per (iteration, chain, group), the device function of the HYPER kernels
+// hmcx_hyper_gamma_draws: one thread per (iteration, chain, group), the device function of the hyperprior runs
 struct GammaShapes { double v[HYPER_GROUPS]; };
 __global__ void __launch_bounds__(256) hyper_gamma_kernel(uint64_t seed, uint64_t chain_offset, int C, int it0, int n_it,
                                                           int K, const GammaShapes shapes, double* __restrict__ out) {

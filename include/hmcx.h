@@ -415,10 +415,10 @@ int hmcx_hmc_run_sink(const hmcx_target_t* target, const hmcx_mass_t* mass, cons
                       float* samples_out, uint8_t* accept_out, uint8_t* diverged_out, float* ham_out,
                       int32_t* num_rejected, int32_t tuning, float* workspace, const hmcx_sink_t* sink, void* stream);
 
-/* hmcx_split_run with a sample sink (sink == NULL: identical to hmcx_split_run).  Any non-NULL sink selects the sink form of
- * the Bayesian-NN kernel: the CTAs of a chain's cluster divide each retained row and its moment updates between them, and
- * the rows go out as 16-byte streaming stores (what pinned host samples_out wants); samples, flags and step sizes are those
- * of hmcx_split_run.  sum / sumsq are read and updated in place at every post-burn iteration, so without sum_lo / sumsq_lo
+/* hmcx_split_run with a sample sink (sink == NULL: identical to hmcx_split_run, which runs as a thin = 1 sink).  In the
+ * Bayesian-NN kernel the CTAs of a chain's cluster divide each retained row and its moment updates between them, and the
+ * rows go out as 16-byte streaming stores (what pinned host samples_out wants); samples, flags and step sizes are those of
+ * hmcx_split_run.  sum / sumsq are read and updated in place at every post-burn iteration, so without sum_lo / sumsq_lo
  * they are plain fp32 running sums: pass both for the compensated sums.  Windows of iterations chain through the
  * accumulators.  thin < 1, sum_lo without sum or sumsq_lo without sumsq: HMCX_ERR_INVALID_ARG. */
 int hmcx_split_run_sink(const hmcx_target_t* target, const hmcx_mass_t* mass, const hmcx_rng_t* rng,

@@ -1,7 +1,8 @@
 """Cost of the hyperprior Gibbs steps at BASELINE config 4 (Linear(64,128)-ReLU-Linear(128,1), D = 8449, N = 1024 in
-M = 4 splits, symmetric split HMC, 64 chains, L = 10, eps = 5e-4, S = 300).  Every variant runs a sink form of the kernel
-(moments=True), so the plain run and the hyperprior runs differ by the hyperprior work only:
-  plain       no hyperpriors (mlp_run_kernel<CS, true, false>)
+M = 4 splits, symmetric split HMC, 64 chains, L = 10, eps = 5e-4, S = 300).  Every variant keeps moments (moments=True),
+so the plain run and the hyperprior runs differ by the hyperprior work and the kernel form only:
+  plain       no hyperpriors (mlp_run_kernel<CS, false>)
+  (the hyperprior variants run mlp_run_kernel<CS, true>, the chain's model constants in shared memory)
   pinned      hyperpriors so tight (a = 1e8, mean = the initial value) that the precisions stay at tau_list = 1,
               tau_out = 100 to ~1e-4: the same posterior as `plain`, so the difference is the cost of the Gibbs steps
               (2L fp64 reductions, the gamma draws, one forward pass, the lost carried gradient)

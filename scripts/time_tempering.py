@@ -3,7 +3,8 @@
 Timing, device events per call, variants alternated three times after one warm-up run of each:
   config 4    Linear(64,128)-ReLU-Linear(128,1), D = 8449, N = 1024 in M = 4 splits, symmetric split HMC, L = 10,
               eps = 5e-4, S = 300: 64 chains as 16 ladders x betas (1, .3, .1, .03) at swap_every 1, 10 and 300, against
-              the plain 64-chain sink run (moments=True everywhere, so every variant runs a sink form of the kernel)
+              the plain 64-chain run (moments=True everywhere; the plain run is mlp_run_kernel<CS, false>, the tempered
+              ones mlp_run_kernel<CS, true>)
   iris        a 4-8-3 tanh classifier on 150 iris-shaped points, 1024 chains (256 ladders x 4 betas), L = 10,
               S = 300: the launch-bound regime
 Multimodal report: the sign-symmetric 1-1-1 tanh net of tests/test_tempering_gpu.py, plain chains against tempered cold
