@@ -1,7 +1,8 @@
-"""fp64 per-iteration replay of the dense (chains x D).(D x D) sampling paths.
+"""fp64 per-iteration replay of the dense (chains x D).(D x D) and the coupled sampling paths.
 
 A plain batched torch restatement, in fp64 and vectorised over chains, of what hmcx_tc.cu computes for
-GaussianIso / GaussianDiag / GaussianFull targets: HMC and HMC_NUTS with inv_mass None, 1-D or 2-D (the reference's
+GaussianIso / GaussianDiag / GaussianFull targets, and hmc_small_kernel / hmcx_coupled.cu for those and Neal's funnel:
+HMC and HMC_NUTS with inv_mass None, 1-D or 2-D (the reference's
 gibbs samplers.py:185-202, leapfrog :267-304, hamiltonian :779-815 and rho = min(0, H_old - H_new) :626), and
 constant-metric RMHMC (explicit A-B-C-B-A :389-462 with the sequential C rotation, implicit :305-387, whose fixed
 points are exact for a constant metric so that it is a leapfrog with G^-1 as the inverse mass).  It runs on whatever
@@ -55,11 +56,36 @@ class _Target64:
         return -0.5 * quad + self.log_norm
 
 
+class _Funnel64:
+    """log p and grad log p of targets.Funnel in fp64, from the fp32 constants the kernel receives: inv_var_v and
+    log_norm rounded to fp32, 0.5 (D - 1) exact."""
+
+    def __init__(self, target, device):
+        self.device = torch.device(device)
+        self.log_norm = _f32(target.log_norm)
+        self.inv_var_v = _f32(target.inv_var_v)
+        self.half_n = 0.5 * (target.dim - 1)
+
+    def grad(self, q):
+        v, x = q[:, :1], q[:, 1:]
+        ev = torch.exp(v)
+        gv = -self.inv_var_v * v + self.half_n - 0.5 * ev * (x * x).sum(1, keepdim=True)
+        return torch.cat([gv, -ev * x], 1)
+
+    def log_prob(self, q):
+        v, x = q[:, 0], q[:, 1:]
+        return -0.5 * self.inv_var_v * v * v + self.half_n * v - 0.5 * torch.exp(v) * (x * x).sum(1) + self.log_norm
+
+
+def target64(target, device):
+    return _Funnel64(target, device) if isinstance(target, T.Funnel) else _Target64(target, device)
+
+
 class HMC:
     """sampler HMC / HMC_NUTS: ``inv_mass`` None, (D,), (D, D) or a block list (= the block-diagonal matrix)."""
 
     def __init__(self, target, inv_mass=None, device='cpu'):
-        self.t = _Target64(target, device)
+        self.t = target64(target, device)
         if isinstance(inv_mass, list):
             inv_mass = torch.block_diag(*[b.to(torch.float32) for b in inv_mass])
         self.im = None if inv_mass is None else inv_mass.to(device, F64)
@@ -80,14 +106,21 @@ class HMC:
     def hamiltonian(self, q, p):                                                # :779-815
         return -self.t.log_prob(q) + 0.5 * (p * self.minv(p)).sum(1)
 
-    def trajectory(self, q, p, e, L):                                           # :267-304
+    def trajectory(self, q, p, e, L, per_step=False):                          # :267-304
+        """The state after L steps, or with ``per_step`` the (L, C, D) states after every step as the stand-alone
+        leapfrog returns them (:299-300): momenta after the full kick, the half-kick correction (:302) on the last."""
         e = e[:, None]
         p = p + 0.5 * e * self.t.grad(q)
+        qs, ps = [], []
         for _ in range(L):
             q = q + e * self.minv(p)
             g = self.t.grad(q)
             p = p + e * g
-        return q, p - 0.5 * e * g
+            qs.append(q), ps.append(p)
+        p = p - 0.5 * e * g
+        if per_step:
+            return torch.stack(qs), torch.stack(ps[:-1] + [p])
+        return q, p
 
 
 class RMHMC:
@@ -184,19 +217,23 @@ def replay(model, params_init, accepted, samples, normals, eps, L, burn):
     return Replay(h_old, h_new, prop)
 
 
-def check(tag, rep, params_init, samples, accepted, ham, log_u, burn, ceiling=2e-4):
+def check(tag, rep, params_init, samples, accepted, ham, log_u, burn, ceiling=2e-4, diverged=None):
     """Compare a kernel run with its replay; returns the number of decisions that differ from the fp64 ones (each
     within 4x the kernel's own Hamiltonian error of that iteration, else the check fails).
 
-    ham (C, S, 2) and log_u (S, C) as given to / returned by the kernel."""
+    ham (C, S, 2) and log_u (S, C) as given to / returned by the kernel.  ``diverged`` (C, S): the iterations the kernel
+    flagged (a non-finite log p, the reference's LogProbError :1045-1067).  Each must be rejected; its Hamiltonians are
+    not compared (fp32 overflows where fp64 does not), every other iteration of the chain is."""
     C, D = params_init.shape
     dev = rep.h_old.device
     ham = ham.to(dev, F64)
-    parity.assert_close(tag + '/ham_old', ham[..., 0].cpu().numpy(), rep.h_old.cpu().numpy(), ceiling)
-    parity.assert_close(tag + '/ham_new', ham[..., 1].cpu().numpy(), rep.h_new.cpu().numpy(), ceiling)
     acc = accepted.to(dev).bool()
+    live = torch.ones_like(acc) if diverged is None else ~diverged.to(dev).bool()
+    assert not bool((acc & ~live).any()), tag + ': a flagged (diverged) iteration was accepted'
+    parity.assert_close(tag + '/ham_old', ham[..., 0][live].cpu().numpy(), rep.h_old[live].cpu().numpy(), ceiling)
+    parity.assert_close(tag + '/ham_new', ham[..., 1][live].cpu().numpy(), rep.h_new[live].cpu().numpy(), ceiling)
     lu = log_u.to(dev, F64).t()
-    flip = acc != (rep.rho >= lu)
+    flip = live & (acc != (rep.rho >= lu))
     dh = (ham[..., 0] - rep.h_old).abs() + (ham[..., 1] - rep.h_new).abs()
     bad = flip & ((rep.rho - lu).abs() > 4 * dh)
     assert not bool(bad.any()), '%s: %d decisions differ from fp64 beyond the kernel\'s Hamiltonian error (first %s)' % (
@@ -215,20 +252,28 @@ def check(tag, rep, params_init, samples, accepted, ham, log_u, burn, ceiling=2e
     return int(flip.sum())
 
 
-def dual_averaging(ham, burn, step_size, desired_accept_rate=0.8):
+def dual_averaging(ham, burn, step_size, desired_accept_rate=0.8, diverged=None):
     """The step sizes HMC_NUTS proposes (samplers.py:629-674, :1030-1035) for iterations 0..burn, in fp64, from the
-    kernel's own Hamiltonians ham (C, S, 2): (C, burn + 1)."""
+    kernel's own Hamiltonians ham (C, S, 2): (C, burn + 1).  ``diverged`` (C, S): a flagged iteration (a LogProbError,
+    :1045-1067) adapts with alpha = 0, and at n == burn it also adapts before eps_bar is taken."""
     ham = ham.double().cpu()
     C = ham.shape[0]
+    flag = torch.zeros(C, burn + 1, dtype=torch.bool)
+    if diverged is not None:
+        flag = diverged[:, :burn + 1].cpu().bool()
     mu = math.log(10 * _f32(step_size))
     h_t, eps_bar = torch.zeros(C, dtype=F64), torch.ones(C, dtype=F64)
     out = torch.empty(C, burn + 1, dtype=F64)
-    for n in range(burn):
+    for n in range(burn + 1):
         t = n + 1
         alpha = torch.exp(torch.clamp(ham[:, n, 0] - ham[:, n, 1], max=0.0))
-        h_t = (1 - 1 / (t + 10)) * h_t + (1 / (t + 10)) * (desired_accept_rate - alpha)
-        x_new = mu - t ** 0.5 / 0.05 * h_t
-        out[:, n] = torch.exp(x_new)
-        eps_bar = torch.exp(t ** -0.75 * x_new + (1 - t ** -0.75) * torch.log(eps_bar))
+        alpha = torch.where(flag[:, n], torch.zeros_like(alpha), alpha)
+        h_new = (1 - 1 / (t + 10)) * h_t + (1 / (t + 10)) * (desired_accept_rate - alpha)
+        x_new = mu - t ** 0.5 / 0.05 * h_new
+        bar_new = torch.exp(t ** -0.75 * x_new + (1 - t ** -0.75) * torch.log(eps_bar))
+        upd = flag[:, n] if n == burn else torch.ones(C, dtype=torch.bool)
+        h_t, eps_bar = torch.where(upd, h_new, h_t), torch.where(upd, bar_new, eps_bar)
+        if n < burn:
+            out[:, n] = torch.exp(x_new)
     out[:, burn] = eps_bar
     return out

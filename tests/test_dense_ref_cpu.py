@@ -2,11 +2,14 @@
 (tests/test_dense_tiles_gpu.py) hold the kernels to, is itself checked here.
 
 * It accepts the unmodified reference's chains (the committed fixtures) as if they were kernel output: identical
-  decisions, states and Hamiltonians within FIXTURE_BOUND.
+  decisions, states and Hamiltonians within FIXTURE_BOUND (funnel11_nuts, whose LogProbError iterations go through
+  check(diverged=) and dual_averaging(diverged=), within FUNNEL_NUTS_BOUND).
 * It accepts the fp32 oracle's chains at D = 250 (a full target with a full and with a diagonal mass) within
   ORACLE_BOUND.
 * It rejects the same oracle runs made with one 64-column block of the precision or of inv_mass off by a relative 1e-4
   (of the order of one missing lo term of a 3xTF32 product, an estimate): the harness catches a one-tile error.
+* It accepts the fp32 oracle's funnel chains at D = 16 and rejects them when the oracle's exp(v) sum(x^2) term is
+  scaled by 1 + 1e-4.
 """
 import copy
 import os
@@ -20,10 +23,15 @@ from oracle import cases as K, hmc_oracle as O, rmhmc_oracle as R
 from tests import dense_ref
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
-# 2x the largest scaled error max|a - d| / (1 + |d|) measured on the CPU: fixtures 1.2e-6 (the explicit RMHMC states),
-# oracle at D = 250 4.9e-7.  The perturbed runs below measure 1.9e-6 (inv_mass block) and 5.1e-6 (precision block).
+# 2x the largest scaled error max|a - d| / (1 + |d|) measured on the CPU: fixtures 1.2e-6 (the explicit RMHMC states;
+# funnel11_hmc states 2.0e-6), oracle at D = 250 4.9e-7.  The perturbed runs below measure 1.9e-6 (inv_mass block) and
+# 5.1e-6 (precision block).
 FIXTURE_BOUND = 2.5e-6
 ORACLE_BOUND = 1e-6
+# funnel11_nuts: 2x its measured 5.3e-5 (states; Hamiltonians 9.1e-7).  Looser than the rest because its trajectories
+# are chaotic: dual averaging drives the step size up to 1.35 over L = 25 steps through the funnel's neck, where the
+# fp32 round-off of one evaluation (expf, summation order) is amplified along the trajectory before it ends.
+FUNNEL_NUTS_BOUND = 1.1e-4
 
 
 def _load(name):
@@ -39,7 +47,9 @@ def _run(model, init, acc, samples, z, logu, ham, eps, L, burn, tag, bound):
     return dense_ref.check(tag, rep, init, samples, acc, ham, logu, burn, ceiling=bound)
 
 
-@pytest.mark.parametrize('name', ['full48_dense', 'full40_fullmass', 'iso40_fullmass_nuts', 'iso40_blockmass'])
+@pytest.mark.parametrize('name', ['full48_dense', 'full40_fullmass', 'iso40_fullmass_nuts', 'iso40_blockmass',
+                                  'cfg1_corr_gauss3', 'diag5_fullmass', 'diag6_blockmass', 'funnel11_hmc',
+                                  'funnel11_nuts'])
 def test_replay_accepts_the_reference_hmc_chains(name):
     case = K.plain_cases()[name]
     kw = case['kw']
@@ -47,17 +57,21 @@ def test_replay_accepts_the_reference_hmc_chains(name):
     S, L, burn = kw['num_samples'], kw['num_steps_per_sample'], kw['burn']
     init = t('init')
     z, logu = t('z').transpose(0, 1), t('logu').t()
+    diverged = t('diverged')
     if kw.get('nuts'):
         eps = t('step_sizes').t().float()                    # teacher-forced: the step size each iteration used
-        # the dual averaging restated in fp64 proposes the reference's next step sizes (eps_bar at n = burn)
-        prop = dense_ref.dual_averaging(ham, burn, kw['step_size'], kw['desired_accept_rate'])
+        # the dual averaging restated in fp64 proposes the reference's next step sizes (eps_bar at n = burn); a
+        # LogProbError iteration adapts with alpha = 0
+        prop = dense_ref.dual_averaging(ham, burn, kw['step_size'], kw['desired_accept_rate'], diverged=diverged)
         np.testing.assert_allclose(prop.numpy(), eps[1:burn + 2].t().numpy(), rtol=2e-6)
     else:
         eps = torch.full((C,), kw['step_size'])
     model = dense_ref.HMC(case['target'], kw.get('inv_mass'))
-    flips = _run(model, init, t('accepted'), t('samples'), z, logu, ham, eps, L, burn, 'cpu_replay/' + name,
-                 FIXTURE_BOUND)
+    rep = dense_ref.replay(model, init, t('accepted'), t('samples'), z, eps, L, burn)
+    flips = dense_ref.check('cpu_replay/' + name, rep, init, t('samples'), t('accepted'), ham, logu, burn,
+                            ceiling=FUNNEL_NUTS_BOUND if name == 'funnel11_nuts' else FIXTURE_BOUND, diverged=diverged)
     assert flips == 0
+    assert bool(diverged.any()) == (name == 'funnel11_nuts')
 
 
 @pytest.mark.parametrize('name', ['rmhmc_exp_hess_full24', 'rmhmc_imp_softabs_diag20'])
@@ -132,3 +146,46 @@ def test_replay_rejects_one_perturbed_64_column_block(mass, operand):
     with pytest.raises(AssertionError, match='tolerance'):
         _run(dense_ref.HMC(tgt, im), init, acc, samples, z, logu, ham, EPS3, L5, 0,
              'cpu_replay/d250_%s_bad_%s' % (mass, operand), ORACLE_BOUND)
+
+
+# ---- Neal's funnel: the fp32 oracle at D = 16, and a mutated funnel ----------------------------------------------------
+class _ScaledFunnel(T.Funnel):
+    """targets.Funnel with its exp(v) sum(x^2) term scaled by 1 + rel."""
+
+    def __init__(self, dim, rel):
+        super().__init__(dim)
+        self.rel = rel
+
+    def __call__(self, w):
+        return super().__call__(w) - 0.5 * self.rel * torch.exp(w[0]) * (w[1:] * w[1:]).sum()
+
+
+def _funnel_oracle(tgt, eps):
+    D = tgt.dim
+    outs, inits, zs, lus = [], [], [], []
+    for c in range(C3):
+        init, z, logu, _ = O.reference_stream(
+            400 + c, D, S6, prior=lambda: torch.cat([0.3 * torch.randn(1), 0.6 * torch.randn(D - 1)]))
+        outs.append(O.sample_hmc(tgt, init, num_samples=S6, num_steps_per_sample=L5, step_size=float(eps[c]),
+                                 normals=z, log_uniforms=logu))
+        inits.append(init), zs.append(z), lus.append(logu)
+    acc = torch.tensor([o['accepted'] for o in outs])
+    samples = torch.stack([torch.stack(o['samples']) for o in outs])
+    ham = torch.tensor([[o['ham_old'], o['ham_new']] for o in outs], dtype=torch.float64).transpose(1, 2)
+    return torch.stack(inits), acc, samples, torch.stack(zs, 1), torch.stack(lus, 1), ham
+
+
+@pytest.mark.parametrize('rel', [0.0, 1e-4])
+def test_replay_checks_the_funnel(rel):
+    """The unmodified oracle passes within ORACLE_BOUND; scaling its exp(v) sum(x^2) term by 1 + 1e-4 fails the replay."""
+    eps = torch.tensor([0.1, 0.12, 0.14])
+    tgt = T.Funnel(16)
+    init, acc, samples, z, logu, ham = _funnel_oracle(_ScaledFunnel(16, rel) if rel else tgt, eps)
+    assert 0 < int(acc.sum()) < acc.numel()
+    args = (dense_ref.HMC(tgt), init, acc, samples, z, logu, ham, eps, L5, 0, 'cpu_replay/funnel16_%g' % rel,
+            ORACLE_BOUND)
+    if rel:
+        with pytest.raises(AssertionError, match='tolerance'):
+            _run(*args)
+    else:
+        assert _run(*args) == 0

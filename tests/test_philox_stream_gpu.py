@@ -193,6 +193,8 @@ SMALL_CASES = {            # hmc_small_kernel (D <= 16: coupled gradient or full
     'funnel3': lambda: (T.Funnel(3), None, 0.1),
     'blocks6': lambda: (T.GaussianDiag(torch.linspace(-1, 1, 6), 0.5 + torch.arange(6.) / 6),
                         [_spd(2, 2), _spd(4, 3)], 0.3),
+    'funnel2_mass': lambda: (T.Funnel(2), _spd(2, 4), 0.1),                        # DM = 2
+    'full16_nuts': lambda: (T.GaussianFull(torch.linspace(-0.5, 0.5, 16), cov=_spd(16, 5)), None, 0.2),   # DM = 16
 }
 
 
@@ -201,7 +203,7 @@ def test_small_kernel(name):
     tgt, im, eps = SMALL_CASES[name]()
     D, C, S = tgt.dim, 37, 14
     nuts = name.endswith('nuts')
-    q0 = _init(C, D, 3, scale=0.3) + (torch.tensor([0.] + [1.] * (D - 1)) if name == 'funnel3' else 0)
+    q0 = _init(C, D, 3, scale=0.3) + (torch.tensor([0.] + [1.] * (D - 1)) if name.startswith('funnel') else 0)
 
     def run(**rng):
         return engine.hmc_run(tgt, q0, S, 5, eps, burn=3, inv_mass=im, nuts=nuts, record_eps=nuts, record_ham=True, **rng)
