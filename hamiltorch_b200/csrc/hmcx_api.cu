@@ -68,6 +68,9 @@ size_t pred_scan_smem(int, int);
 int pred_pass(const float*, long long, long long, int, int, int, int, const float*, const float*, long long, long long,
               int, int, int, double*, double*, int*, double*, void*, cudaStream_t);
 int pred_totals(const double*, int, int, double*, cudaStream_t);
+int sbc_prior(const hmcx_target_t*, uint64_t, long long, int, int, int, float*, cudaStream_t);
+int sbc_simulate(const hmcx_target_t*, const float*, uint64_t, long long, int, float*, cudaStream_t);
+int sbc_rank(const float*, long long, long long, int, int, int, int, const float*, long long, int*, cudaStream_t);
 }  // namespace hmcx
 
 static inline bool has_mu_chain(const hmcx_nuts_t* nuts) { return nuts && nuts->enabled && nuts->mu_chain; }
@@ -492,6 +495,50 @@ int hmcx_adapt_diag_mass(float* sum, float* sumsq, float* sum_lo, float* sumsq_l
         return HMCX_ERR_INVALID_ARG;
     return hmcx::adapt_diag_mass(sum, sumsq, sum_lo, sumsq_lo, C, ld, D, n, eps, C_chains, inv_mass, mass_factor, mu_chain,
                                  h_bar, eps_bar, (cudaStream_t)stream);
+}
+
+// The SBC entry points take an MLP target with data: 1 on success, 0 for invalid arguments, -1 for other target kinds.
+static inline int sbc_target_ok(const hmcx_target_t* target) {
+    if (!target) return 0;
+    if (target->kind != HMCX_TARGET_MLP) return -1;
+    const hmcx_mlp_t* m = target->mlp;
+    return m && m->x && m->y && m->num_rows >= 1 && m->num_layers >= 1 && m->num_layers <= HMCX_MLP_MAX_LAYERS ? 1 : 0;
+}
+
+static inline int mlp_dim(const hmcx_mlp_t* m) {
+    int D = 0;
+    for (int l = 0; l < m->num_layers; ++l) D += m->widths[l] * m->widths[l + 1] + m->widths[l + 1];
+    return D;
+}
+
+int hmcx_sbc_prior(const hmcx_target_t* target, uint64_t seed, int64_t sim_begin, int32_t M, int32_t R, int32_t ld,
+                   float* out, void* stream) {
+    const int ok = sbc_target_ok(target);
+    if (ok < 0) return HMCX_ERR_UNSUPPORTED;
+    if (!ok || !out || sim_begin < 0 || M < 1 || R < 0 || ld < mlp_dim(target->mlp) || (ld & 3))
+        return HMCX_ERR_INVALID_ARG;
+    return hmcx::sbc_prior(target, seed, sim_begin, M, R, ld, out, (cudaStream_t)stream);
+}
+
+int hmcx_sbc_simulate(const hmcx_target_t* target, const float* f, uint64_t seed, int64_t sim_begin, int32_t M,
+                      float* y_out, void* stream) {
+    const int ok = sbc_target_ok(target);
+    if (ok < 0) return HMCX_ERR_UNSUPPORTED;
+    if (!ok || !f || !y_out || sim_begin < 0 || M < 1) return HMCX_ERR_INVALID_ARG;
+    const hmcx_mlp_t* m = target->mlp;
+    if (m->loss == HMCX_LOSS_MULTICLASS_LOGSOFTMAX || (m->loss != HMCX_LOSS_REGRESSION && m->tau_out != 1.0f) ||
+        m->loss < HMCX_LOSS_REGRESSION || m->loss > HMCX_LOSS_MULTICLASS_LOGSOFTMAX || !(m->tau_out > 0.0f))
+        return HMCX_ERR_UNSUPPORTED;
+    return hmcx::sbc_simulate(target, f, seed, sim_begin, M, y_out, (cudaStream_t)stream);
+}
+
+int hmcx_sbc_rank(const float* samples, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t keep, int32_t K,
+                  int32_t D, const float* truth, int64_t truth_stride, int32_t* ranks_out, void* stream) {
+    if (!samples || !truth || !ranks_out || chain_stride < 0 || draw_stride < 0 || truth_stride < 0 || C < 1 || K < 1 ||
+        K > 65535 || C % K || keep < 2 || D < 1 || (int64_t)(C / K) * (keep - 1) > 0x7fffffffLL)
+        return HMCX_ERR_INVALID_ARG;
+    return hmcx::sbc_rank(samples, chain_stride, draw_stride, C, keep, K, D, truth, truth_stride, ranks_out,
+                          (cudaStream_t)stream);
 }
 
 }  // extern "C"

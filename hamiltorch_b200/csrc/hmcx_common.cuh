@@ -45,7 +45,8 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
     return c;
 }
 
-enum { STREAM_MOMENTUM = 0, STREAM_ACCEPT = 1, STREAM_JITTER = 2, STREAM_PERM = 3, STREAM_HYPER = 4, STREAM_SWAP = 5 };
+enum { STREAM_MOMENTUM = 0, STREAM_ACCEPT = 1, STREAM_JITTER = 2, STREAM_PERM = 3, STREAM_HYPER = 4, STREAM_SWAP = 5,
+       STREAM_SBC_PRIOR = 6, STREAM_SBC_DATA = 7 };
 
 // The key schedule k_r = k_0 + r*(W0, W1) depends on (seed, chain) only: a persistent kernel that owns one chain computes it
 // once and keeps the 20 words in registers (the asm makes them opaque, otherwise the compiler re-derives each with an

@@ -486,7 +486,7 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
             nuts=False, desired_accept_rate=0.8, seed=0, chain_offset=0, normals=None, log_uniforms=None,
             record_ham=False, out=None, device=None, tuning=0, eps_schedule=None, record_eps=False, scheme=None,
             perms=None, thin=1, moments=False, keep_samples=True, host_samples=False, host_windows=0, adapt_mass=False,
-            mass_pool=None, hyper=None, gammas=None, temper=None, folds=None):
+            mass_pool=None, hyper=None, gammas=None, temper=None, folds=None, fits=None):
     """The reference's sample() loop for sampler in {HMC, HMC_NUTS} as one persistent kernel over C chains.
 
     params_init (C, D) | (D,).  Randomness: in-kernel Philox keyed by (seed, chain_offset+c, iteration), or -- when
@@ -527,6 +527,9 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
     0 .. K-1 or to -1 (never left out).  The target becomes ``fold_targets(target, folds)`` and one hmcx_split_run_folds
     launch runs chain g = chain_offset + c on fold g mod K's training rows (DESIGN §3.18).  The result gains ``folds``
     (the assignment, on the device) and ``num_folds``.
+    ``fits`` (instead of ``target`` and ``folds``): the list of K MLPTargets of the fits themselves, sharing the network,
+    prior and settings -- the fold path with the training sets given directly (sbc.fit passes K copies of one target, each
+    holding its own simulated y).  Chain g = chain_offset + c samples fits[g mod K].
     """
     N.require_cuda()
     lib = N.load_library()
@@ -534,13 +537,15 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
         device = params_init.device if params_init.is_cuda else torch.device('cuda', torch.cuda.current_device())
     device = torch.device(device)
     num_folds = 0
-    if folds is not None:
+    if folds is not None or fits is not None:
         if scheme != N.SCHEME_PLAIN or temper is not None or hyper is not None or adapt_mass:
             raise NotImplementedError('K-fold runs: the plain integrator on an MLPTarget, without replica exchange, '
                                       'hyperpriors or adapt_mass')
-        folds = torch.as_tensor(folds).to(device=device, dtype=torch.int64)
-        target = fold_targets(target, folds.cpu())
-        num_folds = len(target)
+        if folds is not None:
+            folds = torch.as_tensor(folds).to(device=device, dtype=torch.int64)
+            fits = fold_targets(target, folds.cpu())
+        target = fits
+        num_folds = len(fits)
     nt = native_target(target, device)
     D, ld = nt.dim, N.padded_ld(nt.dim)
     nm = native_mass(inv_mass, D, device)
@@ -767,7 +772,7 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
     if hyper_s is not None:
         res.tau_list_trace, res.tau_out_trace = tau_trace, tau_out_trace
         res.tau_list_final, res.tau_out_final = tau, tau_out
-    if num_folds:
+    if folds is not None:
         res.folds, res.num_folds = folds, num_folds
     if temper_out is not None:
         res.betas, res.swap_accepted, res.swap_ll = temper_out

@@ -736,6 +736,38 @@ int hmcx_pred_pass(const float* f, int64_t chain_stride, int64_t draw_stride, in
                    double* partials, void* workspace, size_t workspace_bytes, void* stream);
 int hmcx_pred_totals(const double* partials, int32_t n, int32_t N, double* totals, void* stream);
 
+/*
+ * Simulation-based calibration of Bayesian NNs (additive v12 symbols; DESIGN §3.19, hamiltorch_b200/sbc.py).  Callers of
+ * an older v12 library check for the symbols.  Sim m (GLOBAL id sim_begin + local index) draws from two Philox streams
+ * whose chain word is m, so a sim's values do not depend on how many sims a call holds:
+ *   prior  (stream 6) counter (v, j lo, j hi | 6 << 24, m lo), key (seed lo, seed hi ^ m hi)
+ *   data   (stream 7) the same counter layout with j = 0
+ * Normals are the canonical Box-Muller of the momentum stream: words (x, y) -> elements 4v, 4v + 1, (z, w) -> 4v + 2, 4v + 3;
+ * uniforms are u01(word) = fma((float)word, 2^-32, 2^-33) in (0, 1].
+ *   hmcx_sbc_prior     out[m, j, :] [M, 1 + R, ld] fp32: row j = 0 is the sim's true parameter vector, row 1 + r the start
+ *                      of chain r, element d < D = z_d sqrt(prior_scale / tau_k) (tau_k = 2 / prior_two_var[k], k the
+ *                      parameter tensor holding d), lanes D .. ld - 1 written as 0.
+ *   hmcx_sbc_simulate  y from the network outputs f [M, num_rows, O] fp32 (hmcx_mlp_pointwise_out of the true parameters):
+ *                        REGRESSION  y [M, num_rows, O] = f + z / sqrt(tau_out), z the normals of the flattened (row, o)
+ *                        BINARY      y [M, num_rows, O] = 1 if u01(word e mod 4 of vector e / 4) < sigmoid(f_e) (fp64)
+ *                                    else 0, e the flattened (row, o)
+ *                        MULTICLASS  y [M, num_rows] = the first class c with u sum_c' exp(f_c' - max f) <= the same sum
+ *                                    over c' <= c (fp64, class order; O - 1 if none), u = u01(word x of vector = row)
+ *                      The log-softmax loss is not a likelihood of independent labels (nll_loss takes the mean), and a
+ *                      classification tau_out other than 1 tempers the likelihood: both HMCX_ERR_UNSUPPORTED.
+ *   hmcx_sbc_rank      ranks[m, d] [K, D] int32 = #{(r, s) : x[r K + m, s, d] < truth[m, d]}, r < C / K, 1 <= s < keep,
+ *                      x[c, s, d] at samples + c chain_stride + s draw_stride + d, truth[m, d] at truth + m truth_stride + d
+ *                      (fp32 comparisons: NaN draws and ties count as "not less").  Slot 0 (params_init) is not a draw.
+ * NULL pointers, a target without data, M < 1, R < 0, ld < D or not a multiple of 4, C < 1, K < 1, C % K != 0, keep < 2,
+ * D < 1, negative strides: HMCX_ERR_INVALID_ARG; non-MLP targets and the two refused likelihoods: HMCX_ERR_UNSUPPORTED.
+ */
+int hmcx_sbc_prior(const hmcx_target_t* target, uint64_t seed, int64_t sim_begin, int32_t M, int32_t R, int32_t ld,
+                   float* out, void* stream);
+int hmcx_sbc_simulate(const hmcx_target_t* target, const float* f, uint64_t seed, int64_t sim_begin, int32_t M,
+                      float* y_out, void* stream);
+int hmcx_sbc_rank(const float* samples, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t keep, int32_t K,
+                  int32_t D, const float* truth, int64_t truth_stride, int32_t* ranks_out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
