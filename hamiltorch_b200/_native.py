@@ -201,6 +201,12 @@ _PROTOS = {
                                     C.c_void_p]),
     'hmcx_sbc_rank': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                 C.c_int64, C.c_void_p, C.c_void_p]),
+    'hmcx_ppc_pass': (C.c_int, [C.POINTER(TargetStruct), C.c_void_p, C.c_int32, C.c_void_p, C.c_uint64, C.c_void_p,
+                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    'hmcx_loo_pit_pass': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_int64, C.c_int64, C.c_int32,
+                                    C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_void_p,
+                                    C.c_void_p, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                    C.c_size_t, C.c_void_p]),
 }
 
 DIAG_LAG_BLOCK = 32                     # HMCX_DIAG_LAG_BLOCK: lags per hmcx_diag_acov pass

@@ -71,6 +71,10 @@ int pred_totals(const double*, int, int, double*, cudaStream_t);
 int sbc_prior(const hmcx_target_t*, uint64_t, long long, int, int, int, float*, cudaStream_t);
 int sbc_simulate(const hmcx_target_t*, const float*, uint64_t, long long, int, float*, cudaStream_t);
 int sbc_rank(const float*, long long, long long, int, int, int, int, const float*, long long, int*, cudaStream_t);
+int ppc_pass(const hmcx_target_t*, const float*, int, const long long*, uint64_t, const float*, float*, double*, double*,
+             int*, cudaStream_t);
+int loo_pit_pass(const float*, long long, long long, const float*, long long, long long, int, int, int, int, int, double,
+                 const float*, const float*, long long, long long, double*, double*, int*, void*, cudaStream_t);
 }  // namespace hmcx
 
 static inline bool has_mu_chain(const hmcx_nuts_t* nuts) { return nuts && nuts->enabled && nuts->mu_chain; }
@@ -539,6 +543,33 @@ int hmcx_sbc_rank(const float* samples, int64_t chain_stride, int64_t draw_strid
         return HMCX_ERR_INVALID_ARG;
     return hmcx::sbc_rank(samples, chain_stride, draw_stride, C, keep, K, D, truth, truth_stride, ranks_out,
                           (cudaStream_t)stream);
+}
+
+int hmcx_ppc_pass(const hmcx_target_t* target, const float* f, int32_t k, const int64_t* draws, uint64_t seed,
+                  const float* tau_out, float* y_rep, double* stats, double* dev_obs, int32_t* nonfinite, void* stream) {
+    const int ok = sbc_target_ok(target);
+    if (ok < 0) return HMCX_ERR_UNSUPPORTED;
+    if (!ok || !f || !draws || !y_rep || !stats || !dev_obs || !nonfinite || k < 1) return HMCX_ERR_INVALID_ARG;
+    const hmcx_mlp_t* m = target->mlp;
+    if (m->loss < HMCX_LOSS_REGRESSION || m->loss > HMCX_LOSS_MULTICLASS_LOGSOFTMAX) return HMCX_ERR_INVALID_ARG;
+    if (m->loss == HMCX_LOSS_REGRESSION && !tau_out && !(m->tau_out > 0.0f)) return HMCX_ERR_INVALID_ARG;
+    return hmcx::ppc_pass(target, f, k, (const long long*)draws, seed, tau_out, y_rep, stats, dev_obs, nonfinite,
+                          (cudaStream_t)stream);
+}
+
+int hmcx_loo_pit_pass(const float* ll, int64_t chain_stride, int64_t draw_stride, const float* f, int64_t f_chain_stride,
+                      int64_t f_draw_stride, int32_t C, int32_t n, int32_t O, int32_t N, int32_t i0, int32_t k,
+                      double r_eff, const float* y, const float* tau_out, int64_t tau_chain_stride,
+                      int64_t tau_draw_stride, double* pit, double* pareto_k, int32_t* nonfinite, void* workspace,
+                      size_t workspace_bytes, void* stream) {
+    if (!ll || !f || !y || !tau_out || !pit || !pareto_k || !nonfinite || !workspace || chain_stride < 0 ||
+        draw_stride < 0 || f_chain_stride < 0 || f_draw_stride < 0 || tau_chain_stride < 0 || tau_draw_stride < 0 ||
+        O < 1 || !loo_shape_ok(C, n) || N < 1 || i0 < 0 || !rank_slab_ok(k) || (int64_t)i0 + k > N ||
+        !(r_eff > 0.0) || !(r_eff <= DBL_MAX) || workspace_bytes < hmcx::loo_workspace_bytes(C, n, k))
+        return HMCX_ERR_INVALID_ARG;
+    return hmcx::loo_pit_pass(ll, chain_stride, draw_stride, f, f_chain_stride, f_draw_stride, C, n, O, i0, k, r_eff, y,
+                              tau_out, tau_chain_stride, tau_draw_stride, pit, pareto_k, nonfinite, workspace,
+                              (cudaStream_t)stream);
 }
 
 }  // extern "C"

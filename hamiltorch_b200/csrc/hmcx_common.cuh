@@ -46,7 +46,7 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
 }
 
 enum { STREAM_MOMENTUM = 0, STREAM_ACCEPT = 1, STREAM_JITTER = 2, STREAM_PERM = 3, STREAM_HYPER = 4, STREAM_SWAP = 5,
-       STREAM_SBC_PRIOR = 6, STREAM_SBC_DATA = 7 };
+       STREAM_SBC_PRIOR = 6, STREAM_SBC_DATA = 7, STREAM_PPC = 8 };
 
 // The key schedule k_r = k_0 + r*(W0, W1) depends on (seed, chain) only: a persistent kernel that owns one chain computes it
 // once and keeps the 20 words in registers (the asm makes them opaque, otherwise the compiler re-derives each with an
@@ -128,6 +128,34 @@ __device__ __forceinline__ void box_muller(uint32_t a, uint32_t b, float& z0, fl
     __sincosf(fmaf((float)b, 1.4629180792671596e-09f, -3.1415926521268f), &s, &c);   // 2 pi (b + 1/2) 2^-32 - pi
     z0 = r * c;
     z1 = r * s;
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// One data element simulated from a Bayesian NN's likelihood at the network output f: the definitions hmcx_sbc_simulate
+// (prior predictive) and hmcx_ppc_pass (posterior predictive) share, so both give the same bits for the same words.
+// ---------------------------------------------------------------------------------------------------------
+// regression: f + z sd, sd = 1 / sqrt(tau_out) rounded to fp32 (noise_sd)
+__device__ __forceinline__ float noise_sd(float tau) { return (float)(1.0 / sqrt((double)tau)); }
+__device__ __forceinline__ float sim_gaussian(float f, float z, float sd) { return add(f, mul(z, sd)); }
+// binary: 1 when the uniform word is below sigmoid(f) (fp64), else 0
+__device__ __forceinline__ float sim_bernoulli(float f, uint32_t w) {
+    const double p = 1.0 / (1.0 + exp(-(double)f));
+    return (double)u01(w) < p ? 1.0f : 0.0f;
+}
+// multi-class: Categorical(softmax f) over O classes, e_c = exp(f_c - max f) in class order (fp64); the label is the first
+// class c with u * sum_c' e_c' <= e_0 + ... + e_c (the last class if rounding leaves none)
+__device__ __forceinline__ int sim_categorical(const float* fr, int O, uint32_t w) {
+    double mx = (double)fr[0];
+    for (int c = 1; c < O; ++c) mx = fmax(mx, (double)fr[c]);
+    double tot = 0.0;
+    for (int c = 0; c < O; ++c) tot += exp((double)fr[c] - mx);
+    const double t = (double)u01(w) * tot;
+    double cum = 0.0;
+    for (int c = 0; c < O - 1; ++c) {
+        cum += exp((double)fr[c] - mx);
+        if (t <= cum) return c;
+    }
+    return O - 1;
 }
 
 // Canonical momentum stream (identical for every kernel geometry): one Philox call per float4 VECTOR of the chain

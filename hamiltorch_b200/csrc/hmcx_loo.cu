@@ -10,7 +10,9 @@
 //        log-ratios and the LOO / WAIC terms.  Every draw-sum is a thread-strided loop over the sorted draws followed by a
 //        fixed shuffle tree and a fixed in-order sum over warps; there are no atomics, so the outputs depend on the block
 //        alone (not on k or the launch geometry) and the same block gives the same bits.
-// The smoothed tail needs no draw index: each term of every sum is a function of the sorted position only.
+// The smoothed tail needs no draw index: each term of every sum is a function of the sorted position only.  LOO-PIT
+// (hmcx_loo_pit_pass, hamiltorch_b200/ppc.py) runs the same sort and the same smoothing (psis_smooth), then reads each
+// sorted draw's network outputs and noise precision through the flat index c*n + s the sort carries alongside the key.
 #include <cfloat>
 #include "hmcx_common.cuh"
 
@@ -18,7 +20,7 @@ namespace hmcx {
 
 size_t rank_sort_workspace_bytes(int C, int n, int k);
 int rank_sort(const float* x, long long cs, long long ds, int C, int n, int d0, int k, int* nonfinite, void* ws,
-              const uint32_t** sorted_keys, cudaStream_t st);
+              const uint32_t** sorted_keys, const int** sorted_idx, cudaStream_t st);
 
 namespace {
 
@@ -55,37 +57,47 @@ __device__ __forceinline__ double cta_max(double v, double* sh) {
     return s;
 }
 
-// One point per CTA.  keys: the slab's sorted keys, S per point.  M = ceil(min(0.2 S, 3 sqrt(S / r_eff))) (host).
-// out[row * N + i], rows: 0 elpd_loo, 1 p_loo, 2 pareto_k, 3 lppd, 4 p_waic, 5 elpd_waic; tail[i] = M'.
-// Dynamic shared memory: 30 + floor(sqrt(M)) doubles (the L_j of the fit).
-__global__ void __launch_bounds__(LT) loo_point_kernel(const uint32_t* __restrict__ keys, int S, int M, int N, int i0,
-                                                       const int* __restrict__ nonfinite, double* __restrict__ out,
-                                                       int* __restrict__ tail) {
-    extern __shared__ double sL[];
-    __shared__ double sh[LW];
-    const int j = blockIdx.x, i = i0 + j, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const uint32_t* kp = keys + (long long)j * S;
-    if (nonfinite[i]) {
-        if (tid == 0) {
-            const double nan = __longlong_as_double(0x7ff8000000000000LL);
-            for (int r = 0; r < 6; ++r) out[(long long)r * N + i] = nan;
-            tail[i] = 0;
+// The Pareto smoothing of one point's S sorted draws (steps 3-6, shared by the LOO / WAIC and LOO-PIT kernels): the tail
+// cut, the generalised-Pareto fit and the normalised log-weights lw(p) - lse_w of sorted position p.  Called by every
+// thread of the CTA; sL holds 30 + floor(sqrt(M)) doubles, sh one per warp.
+struct Psis {
+    const uint32_t* kp;
+    double rmax, ec, khat, sigma, lse_w;
+    int Mt;
+    bool smooth;
+    __device__ __forceinline__ double llv(int p) const { return ll_of_key(kp[p]); }
+    __device__ __forceinline__ double rr(int p) const { return -llv(p) - rmax; }   // shifted log-ratio, rr(0) = 0
+    // 6. log-ratios: the tail (ascending z = Mt - p) replaced by the GPD quantiles, then capped at 0 (the largest raw one)
+    __device__ __forceinline__ double lw(int p) const {
+        double v;
+        if (smooth && p < Mt) {
+            const double pz = (Mt - p - 0.5) / Mt;
+            const double q = khat == 0.0 ? -sigma * log1p(-pz) : sigma * expm1(-khat * log1p(-pz)) / khat;
+            v = log(q + ec);
+        } else {
+            v = rr(p);
         }
-        return;
+        return v > 0.0 ? 0.0 : v;
     }
-    auto llv = [&](int p) { return ll_of_key(kp[p]); };
-    const double rmax = -llv(0);
-    auto rr = [&](int p) { return -llv(p) - rmax; };           // shifted log-ratio, non-increasing in p, rr(0) = 0
+};
+
+__device__ __forceinline__ Psis psis_smooth(const uint32_t* kp, int S, int M, double* sL, double* sh) {
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    Psis w;
+    w.kp = kp;
+    w.rmax = -w.llv(0);
     // 3-4. cutoff = the (M+1)-th largest r, floored; the tail is {r > cutoff} = sorted positions [0, Mt)
-    const double c = fmax(rr(M), log(DBL_MIN));
+    const double c = fmax(w.rr(M), log(DBL_MIN));
     int lo = 0, hi = M;
     while (lo < hi) {
         const int mid = (lo + hi) >> 1;
-        if (rr(mid) > c) lo = mid + 1; else hi = mid;
+        if (w.rr(mid) > c) lo = mid + 1; else hi = mid;
     }
     const int Mt = lo;
+    w.Mt = Mt;
     const double ec = exp(c);
-    auto xt = [&](int t) { return exp(rr(Mt - t)) - ec; };     // ascending exceedances, t = 1..Mt
+    w.ec = ec;
+    auto xt = [&](int t) { return exp(w.rr(Mt - t)) - ec; };   // ascending exceedances, t = 1..Mt
     // 5. generalised-Pareto fit (Zhang & Stephens 2009, with the weakly informative prior of Vehtari et al.)
     double khat = __longlong_as_double(0x7ff0000000000000LL), sigma = 0.0;
     if (Mt > 4) {
@@ -107,8 +119,8 @@ __global__ void __launch_bounds__(LT) loo_point_kernel(const uint32_t* __restric
             const double Lj = sL[jj - 1];
             double d = 0.0;
             for (int l = 0; l < m; ++l) d += exp(sL[l] - Lj);
-            const double w = 1.0 / d;
-            if (w >= 10.0 * DBL_EPSILON) { wsum += w; wbsum += w * b_of(jj); }
+            const double wj = 1.0 / d;
+            if (wj >= 10.0 * DBL_EPSILON) { wsum += wj; wbsum += wj * b_of(jj); }
         }
         const double bbar = cta_sum(wbsum, sh) / cta_sum(wsum, sh);
         double s = 0.0;
@@ -117,50 +129,103 @@ __global__ void __launch_bounds__(LT) loo_point_kernel(const uint32_t* __restric
         sigma = -xi / bbar;
         khat = (Mt * xi + 5.0) / (Mt + 10.0);
     }
-    const bool smooth = Mt > 4 && isfinite(khat);
-    // 6. log-ratios: the tail (ascending z = Mt - p) replaced by the GPD quantiles, then capped at 0 (the largest raw one)
-    auto lw = [&](int p) {
-        double v;
-        if (smooth && p < Mt) {
-            const double pz = (Mt - p - 0.5) / Mt;
-            const double q = khat == 0.0 ? -sigma * log1p(-pz) : sigma * expm1(-khat * log1p(-pz)) / khat;
-            v = log(q + ec);
-        } else {
-            v = rr(p);
-        }
-        return v > 0.0 ? 0.0 : v;
-    };
+    w.khat = khat;
+    w.sigma = sigma;
+    w.smooth = Mt > 4 && isfinite(khat);
+    // normalisation: lse_w = logsumexp over the draws of the capped log-ratios
     double mx = -DBL_MAX;
-    for (int p = tid; p < S; p += LT) mx = fmax(mx, lw(p));
+    for (int p = tid; p < S; p += LT) mx = fmax(mx, w.lw(p));
     mx = cta_max(mx, sh);
     double s = 0.0;
-    for (int p = tid; p < S; p += LT) s += exp(lw(p) - mx);
-    const double lse_w = mx + log(cta_sum(s, sh));
+    for (int p = tid; p < S; p += LT) s += exp(w.lw(p) - mx);
+    w.lse_w = mx + log(cta_sum(s, sh));
+    return w;
+}
+
+__device__ __forceinline__ void write_nan(double* p) { *p = __longlong_as_double(0x7ff8000000000000LL); }
+
+// One point per CTA.  keys: the slab's sorted keys, S per point.  M = ceil(min(0.2 S, 3 sqrt(S / r_eff))) (host).
+// out[row * N + i], rows: 0 elpd_loo, 1 p_loo, 2 pareto_k, 3 lppd, 4 p_waic, 5 elpd_waic; tail[i] = M'.
+// Dynamic shared memory: 30 + floor(sqrt(M)) doubles (the L_j of the fit).
+__global__ void __launch_bounds__(LT) loo_point_kernel(const uint32_t* __restrict__ keys, int S, int M, int N, int i0,
+                                                       const int* __restrict__ nonfinite, double* __restrict__ out,
+                                                       int* __restrict__ tail) {
+    extern __shared__ double sL[];
+    __shared__ double sh[LW];
+    const int j = blockIdx.x, i = i0 + j, tid = threadIdx.x;
+    const uint32_t* kp = keys + (long long)j * S;
+    if (nonfinite[i]) {
+        if (tid == 0) {
+            for (int r = 0; r < 6; ++r) write_nan(out + (long long)r * N + i);
+            tail[i] = 0;
+        }
+        return;
+    }
+    const Psis w = psis_smooth(kp, S, M, sL, sh);
+    const double lse_w = w.lse_w;
     // 7. elpd_loo = logsumexp(lw + ll), lw normalised
-    mx = -DBL_MAX;
-    for (int p = tid; p < S; p += LT) mx = fmax(mx, (lw(p) - lse_w) + llv(p));
+    double mx = -DBL_MAX;
+    for (int p = tid; p < S; p += LT) mx = fmax(mx, (w.lw(p) - lse_w) + w.llv(p));
     mx = cta_max(mx, sh);
-    s = 0.0;
-    for (int p = tid; p < S; p += LT) s += exp(((lw(p) - lse_w) + llv(p)) - mx);
+    double s = 0.0;
+    for (int p = tid; p < S; p += LT) s += exp(((w.lw(p) - lse_w) + w.llv(p)) - mx);
     const double elpd = mx + log(cta_sum(s, sh));
     // lppd = logsumexp(ll) - log S (the largest ll is the last sorted draw); p_waic = var(ll), ddof 1
-    const double llmax = llv(S - 1);
+    const double llmax = w.llv(S - 1);
     double se = 0.0, sm = 0.0;
-    for (int p = tid; p < S; p += LT) { const double v = llv(p); se += exp(v - llmax); sm += v; }
+    for (int p = tid; p < S; p += LT) { const double v = w.llv(p); se += exp(v - llmax); sm += v; }
     const double lppd = (llmax + log(cta_sum(se, sh))) - log((double)S);
     const double mean = cta_sum(sm, sh) / S;
     double sv = 0.0;
-    for (int p = tid; p < S; p += LT) { const double d = llv(p) - mean; sv += d * d; }
+    for (int p = tid; p < S; p += LT) { const double d = w.llv(p) - mean; sv += d * d; }
     const double pw = cta_sum(sv, sh) / (S - 1);
     if (tid == 0) {
         out[i] = elpd;
         out[(long long)N + i] = lppd - elpd;
-        out[2LL * N + i] = khat;
+        out[2LL * N + i] = w.khat;
         out[3LL * N + i] = lppd;
         out[4LL * N + i] = pw;
         out[5LL * N + i] = lppd - pw;
-        tail[i] = Mt;
+        tail[i] = w.Mt;
     }
+}
+
+// LOO-PIT, one point per CTA: pit[i, o] = sum_p w~_p Phi((y_io - f_{g_p, i, o}) sqrt(tau_{g_p})) over the sorted positions p
+// of the point's draws, w~_p = exp(lw(p) - lse_w) the normalised PSIS weights of psis_smooth and g_p = c n + s the flat
+// index the sort carried.  Phi(x) = erfc(-x / sqrt 2) / 2 in fp64; each output's sum is thread-strided over p, then the
+// fixed tree of cta_sum.  pareto_k[i] = k-hat.  A point with a non-finite draw: NaN pit and k-hat.
+__global__ void __launch_bounds__(LT) loo_pit_kernel(const uint32_t* __restrict__ keys, const int* __restrict__ idx,
+                                                     int S, int M, int n, int O, int i0, const float* __restrict__ f,
+                                                     long long fcs, long long fds, const float* __restrict__ y,
+                                                     const float* __restrict__ tau, long long tcs, long long tds,
+                                                     const int* __restrict__ nonfinite, double* __restrict__ pit,
+                                                     double* __restrict__ pareto_k) {
+    extern __shared__ double sL[];
+    __shared__ double sh[LW];
+    const int j = blockIdx.x, i = i0 + j, tid = threadIdx.x;
+    const uint32_t* kp = keys + (long long)j * S;
+    const int* ip = idx + (long long)j * S;
+    if (nonfinite[i]) {
+        if (tid == 0) {
+            for (int o = 0; o < O; ++o) write_nan(pit + (long long)i * O + o);
+            write_nan(pareto_k + i);
+        }
+        return;
+    }
+    const Psis w = psis_smooth(kp, S, M, sL, sh);
+    for (int o = 0; o < O; ++o) {
+        const double yo = (double)y[(long long)i * O + o];
+        double s = 0.0;
+        for (int p = tid; p < S; p += LT) {
+            const int g = ip[p], c = g / n, t = g - c * n;
+            const double fv = (double)f[(long long)c * fcs + (long long)t * fds + (long long)i * O + o];
+            const double sq = sqrt((double)tau[(long long)c * tcs + (long long)t * tds]);
+            s += exp(w.lw(p) - w.lse_w) * (0.5 * erfc(-((yo - fv) * sq) * 0.70710678118654752440));
+        }
+        s = cta_sum(s, sh);
+        if (tid == 0) pit[(long long)i * O + o] = s;
+    }
+    if (tid == 0) pareto_k[i] = w.khat;
 }
 
 }  // namespace
@@ -171,17 +236,38 @@ int loo_tail_cap(int S, double r_eff) {
 
 size_t loo_workspace_bytes(int C, int n, int k) { return rank_sort_workspace_bytes(C, n, k); }
 
+// dynamic shared memory of the PSIS kernels: the 30 + floor(sqrt(M')) <= 30 + floor(sqrt(M)) L_j of the fit
+static size_t fit_smem(int M) { return (size_t)(30 + (int)floor(sqrt((double)M))) * sizeof(double); }
+
 int loo_pass(const float* ll, long long cs, long long ds, int C, int n, int N, int i0, int k, double r_eff, double* out,
              int* tail, int* nonfinite, void* ws, cudaStream_t st) {
     const int S = C * n;
     const uint32_t* keys = nullptr;
-    int rc = rank_sort(ll, cs, ds, C, n, i0, k, nonfinite, ws, &keys, st);
+    const int* idx = nullptr;
+    int rc = rank_sort(ll, cs, ds, C, n, i0, k, nonfinite, ws, &keys, &idx, st);
     if (rc != HMCX_OK) return rc;
     const int M = loo_tail_cap(S, r_eff);
-    const size_t smem = (size_t)(30 + (int)floor(sqrt((double)M))) * sizeof(double);
+    const size_t smem = fit_smem(M);
     if (cudaFuncSetAttribute(loo_point_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
         return HMCX_ERR_CUDA;
     loo_point_kernel<<<k, LT, smem, st>>>(keys, S, M, N, i0, nonfinite, out, tail);
+    return cudaGetLastError() == cudaSuccess ? HMCX_OK : HMCX_ERR_CUDA;
+}
+
+int loo_pit_pass(const float* ll, long long cs, long long ds, const float* f, long long fcs, long long fds, int C, int n,
+                 int O, int i0, int k, double r_eff, const float* y, const float* tau, long long tcs, long long tds,
+                 double* pit, double* pareto_k, int* nonfinite, void* ws, cudaStream_t st) {
+    const int S = C * n;
+    const uint32_t* keys = nullptr;
+    const int* idx = nullptr;
+    int rc = rank_sort(ll, cs, ds, C, n, i0, k, nonfinite, ws, &keys, &idx, st);
+    if (rc != HMCX_OK) return rc;
+    const int M = loo_tail_cap(S, r_eff);
+    const size_t smem = fit_smem(M);
+    if (cudaFuncSetAttribute(loo_pit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+        return HMCX_ERR_CUDA;
+    loo_pit_kernel<<<k, LT, smem, st>>>(keys, idx, S, M, n, O, i0, f, fcs, fds, y, tau, tcs, tds, nonfinite, pit,
+                                        pareto_k);
     return cudaGetLastError() == cudaSuccess ? HMCX_OK : HMCX_ERR_CUDA;
 }
 

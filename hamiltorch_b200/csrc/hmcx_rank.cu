@@ -422,8 +422,8 @@ size_t rank_workspace_bytes(int C, int n, int k) {
     return b;
 }
 
-// The sort alone (stages 1-2) for the PSIS pass of hmcx_loo.cu: keys and indices twice plus the digit counts -- the
-// pieces 0-3 and 5 of ws_sizes, carved in that order.
+// The sort alone (stages 1-2) for the PSIS passes of hmcx_loo.cu: keys and indices twice plus the digit counts -- the
+// pieces 0-3 and 5 of ws_sizes, carved in that order.  Hands back the sorted keys and their flat draw indices c*n + s.
 size_t rank_sort_workspace_bytes(int C, int n, int k) {
     size_t sz[7];
     ws_sizes(C * n, k, sz);
@@ -431,7 +431,7 @@ size_t rank_sort_workspace_bytes(int C, int n, int k) {
 }
 
 int rank_sort(const float* x, long long cs, long long ds, int C, int n, int d0, int k, int* nonfinite, void* ws,
-              const uint32_t** sorted_keys, cudaStream_t st) {
+              const uint32_t** sorted_keys, const int** sorted_idx, cudaStream_t st) {
     const int L = C * n;
     size_t sz[7];
     ws_sizes(L, k, sz);
@@ -442,6 +442,7 @@ int rank_sort(const float* x, long long cs, long long ds, int C, int n, int d0, 
     int* ib = (int*)(p += sz[2]);
     uint32_t* cnt = (uint32_t*)(p += sz[3]);
     *sorted_keys = ka;
+    *sorted_idx = ia;
     const int rc = sort_slab(x, cs, ds, n, L, d0, k, nonfinite, ka, kb, ia, ib, cnt, st);
     if (rc != HMCX_OK) return rc;
     return cudaGetLastError() == cudaSuccess ? HMCX_OK : HMCX_ERR_CUDA;

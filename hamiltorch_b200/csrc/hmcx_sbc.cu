@@ -51,7 +51,7 @@ __global__ void __launch_bounds__(PT) sbc_prior_kernel(PriorTable tab, uint64_t 
 }
 
 // Regression: y = f + z / sqrt(tau_out), one Philox block per 4 consecutive outputs of a sim.  Binary: y = 1 when the
-// output's u01 word is below sigmoid(f) (fp64), else 0.
+// output's u01 word is below sigmoid(f) (fp64), else 0.  The element definitions are hmcx_common.cuh's sim_*.
 __global__ void __launch_bounds__(PT) sbc_simulate_elem_kernel(const float* __restrict__ f, uint64_t seed, long long m0,
                                                                long long n_out, long long total, int binary,
                                                                float noise_sd, float* __restrict__ y) {
@@ -72,18 +72,12 @@ __global__ void __launch_bounds__(PT) sbc_simulate_elem_kernel(const float* __re
             if (idx >= n_out) break;
             const long long at = m * n_out + idx;
             const float fv = f[at];
-            if (binary) {
-                const double p = 1.0 / (1.0 + exp(-(double)fv));
-                y[at] = (double)u01(w[e]) < p ? 1.0f : 0.0f;
-            } else {
-                y[at] = add(fv, mul(z[e], noise_sd));
-            }
+            y[at] = binary ? sim_bernoulli(fv, w[e]) : sim_gaussian(fv, z[e], noise_sd);
         }
     }
 }
 
-// Multi-class: one label per row from Categorical(softmax f): e_c = exp(f_c - max f) in class order (fp64), the label is
-// the first class c with u * sum_c' e_c' <= e_0 + ... + e_c (the last class if rounding leaves none).
+// Multi-class: one label per row from Categorical(softmax f) (sim_categorical), u = u01(word x of vector = row).
 __global__ void __launch_bounds__(PT) sbc_simulate_class_kernel(const float* __restrict__ f, uint64_t seed, long long m0,
                                                                 int N, int O, long long total, float* __restrict__ y) {
     for (long long i = (long long)blockIdx.x * PT + threadIdx.x; i < total; i += (long long)gridDim.x * PT) {
@@ -91,18 +85,7 @@ __global__ void __launch_bounds__(PT) sbc_simulate_class_kernel(const float* __r
         const int row = (int)(i - m * N);
         const float* fr = f + i * O;
         const uint4 r = philox_draw(seed, (uint64_t)(m0 + m), 0, (uint32_t)row, STREAM_SBC_DATA);
-        double mx = (double)fr[0];
-        for (int c = 1; c < O; ++c) mx = fmax(mx, (double)fr[c]);
-        double tot = 0.0;
-        for (int c = 0; c < O; ++c) tot += exp((double)fr[c] - mx);
-        const double t = (double)u01(r.x) * tot;
-        double cum = 0.0;
-        int label = O - 1;
-        for (int c = 0; c < O - 1; ++c) {
-            cum += exp((double)fr[c] - mx);
-            if (t <= cum) { label = c; break; }
-        }
-        y[i] = (float)label;
+        y[i] = (float)sim_categorical(fr, O, r.x);
     }
 }
 

@@ -768,6 +768,44 @@ int hmcx_sbc_simulate(const hmcx_target_t* target, const float* f, uint64_t seed
 int hmcx_sbc_rank(const float* samples, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t keep, int32_t K,
                   int32_t D, const float* truth, int64_t truth_stride, int32_t* ranks_out, void* stream);
 
+/*
+ * Posterior predictive checks of Bayesian NNs (additive v12 symbols; DESIGN §3.20, hamiltorch_b200/ppc.py).  Callers of
+ * an older v12 library check for the symbols.
+ *   hmcx_ppc_pass    for a slab of k posterior draws, draw j the pooled draw g = draws[j] (int64 device, g = c n + s) with
+ *                    network outputs f [k, num_rows, O] fp32 (hmcx_mlp_pointwise_out): one replicated data set per draw
+ *                    from Philox stream 8, counter (v, 0, 8 << 24, g lo), key (seed lo, seed hi ^ g hi), with the element
+ *                    definitions of hmcx_sbc_simulate (v the vector of 4 flattened outputs e = i O + o for regression
+ *                    and binary, v = row for multi-class; both multi-class losses draw from softmax f), written to
+ *                    y_rep [k, num_rows, y_cols] (y_cols = O, or 1 for multi-class).  Regression noise sd =
+ *                    1 / sqrt(tau), tau = tau_out[j] (fp32 device), or the target's tau_out when tau_out is NULL.
+ *                    stats [k, K] fp64, K = 4 O + 1 (regression: mean, sd (ddof 1), min, max of each output column in
+ *                    column order), O + 1 (binary: the mean of each column; multi-class: the frequency of each class);
+ *                    column K - 1 the deviance -2 sum_i ll_i(y_rep | theta_g), dev_obs [k] = -2 sum_i ll_i(y | theta_g)
+ *                    with y the target's data and ll the density of hmcx_mlp_pointwise_ll_tau evaluated in fp64 from the
+ *                    fp32 outputs.  nonfinite [k] int32: 1 where the draw has a non-finite output (its statistics and
+ *                    deviances are NaN).  One CTA per draw, fixed-order fp64 sums, no atomics: a draw's results depend on
+ *                    (seed, g, its outputs) only.  NULL pointers (tau_out excepted), a target without data, k < 1 or a
+ *                    non-positive target tau_out with tau_out NULL (regression): HMCX_ERR_INVALID_ARG; non-MLP targets:
+ *                    HMCX_ERR_UNSUPPORTED.
+ *   hmcx_loo_pit_pass  LOO-PIT of the points [i0, i0 + k) of a regression: the sort and the Pareto smoothing of
+ *                    hmcx_loo_pass on the log-likelihood block ll (the same arguments, N points), then per point i and
+ *                    output o in fp64 pit[i, o] = sum_p w_p Phi((y[i, o] - f[c_p, s_p, i, o]) sqrt(tau[c_p, s_p])) over the
+ *                    sorted draws p, w_p the normalised smoothed weights exp(lw_p) and (c_p, s_p) the draw the stable sort
+ *                    put at p; Phi(x) = erfc(-x / sqrt 2) / 2.  f at f + c*f_chain_stride + s*f_draw_stride + i*O + o, y
+ *                    [N, O] fp32, tau at tau_out + c*tau_chain_stride + s*tau_draw_stride (a stride of 0 repeats one
+ *                    value).  pit [N, O], pareto_k [N] fp64 (k-hat, the bits hmcx_loo_pass writes for the same block and
+ *                    r_eff), nonfinite [N] int32 (1: NaN pit and k-hat).  Workspace: hmcx_loo_workspace_bytes(C, n, k).
+ *                    The checks of hmcx_loo_pass, and NULL f / y / tau_out, O < 1 or negative strides:
+ *                    HMCX_ERR_INVALID_ARG.
+ */
+int hmcx_ppc_pass(const hmcx_target_t* target, const float* f, int32_t k, const int64_t* draws, uint64_t seed,
+                  const float* tau_out, float* y_rep, double* stats, double* dev_obs, int32_t* nonfinite, void* stream);
+int hmcx_loo_pit_pass(const float* ll, int64_t chain_stride, int64_t draw_stride, const float* f, int64_t f_chain_stride,
+                      int64_t f_draw_stride, int32_t C, int32_t n, int32_t O, int32_t N, int32_t i0, int32_t k,
+                      double r_eff, const float* y, const float* tau_out, int64_t tau_chain_stride,
+                      int64_t tau_draw_stride, double* pit, double* pareto_k, int32_t* nonfinite, void* workspace,
+                      size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
