@@ -3,7 +3,7 @@
 Exports the same names as the reference's ``hamiltorch/__init__.py:1-4`` plus the engine's native additions
 (``targets``, ``sample_chains``, ``diagnostics``, ``loo``, ``predictive``: held-out accuracy, NLL, Brier score,
 calibration and predictive uncertainty of Bayesian NNs; ``sbc``: simulation-based calibration of a Bayesian-NN fit;
-``ppc``: posterior predictive checks and LOO-PIT of a fitted Bayesian NN).
+``ppc``: posterior predictive checks and LOO-PIT of a fitted Bayesian NN; chain and model stacking in ``loo``).
 The CUDA library is loaded lazily by the first sampling call and that call fails loudly if libhmcx.so is missing or no GPU
 is present: there is no CPU fallback.
 """

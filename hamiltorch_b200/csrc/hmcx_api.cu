@@ -66,7 +66,7 @@ int mlp_pointwise_out(const hmcx_target_t*, const float*, long long, long long, 
 size_t pred_workspace_bytes(int, int, int, int);
 size_t pred_scan_smem(int, int);
 int pred_pass(const float*, long long, long long, int, int, int, int, const float*, const float*, long long, long long,
-              int, int, int, double*, double*, int*, double*, void*, cudaStream_t);
+              int, int, int, double*, double*, int*, double*, void*, cudaStream_t, const double*);
 int pred_totals(const double*, int, int, double*, cudaStream_t);
 int sbc_prior(const hmcx_target_t*, uint64_t, long long, int, int, int, float*, cudaStream_t);
 int sbc_simulate(const hmcx_target_t*, const float*, uint64_t, long long, int, float*, cudaStream_t);
@@ -75,6 +75,11 @@ int ppc_pass(const hmcx_target_t*, const float*, int, const long long*, uint64_t
              int*, cudaStream_t);
 int loo_pit_pass(const float*, long long, long long, const float*, long long, long long, int, int, int, int, int, double,
                  const float*, const float*, long long, long long, double*, double*, int*, void*, cudaStream_t);
+int loo_chain_pass(const float*, long long, long long, int, int, int, int, int, double, double*, int*, int*,
+                   cudaStream_t);
+size_t stack_workspace_bytes(int, int);
+int stack_eval(const double*, int, int, const double*, double*, double*, double*, void*, cudaStream_t);
+int stack_em(const double*, int, int, double, int, double*, double*, double*, double*, int*, void*, cudaStream_t);
 }  // namespace hmcx
 
 static inline bool has_mu_chain(const hmcx_nuts_t* nuts) { return nuts && nuts->enabled && nuts->mu_chain; }
@@ -483,7 +488,25 @@ int hmcx_pred_pass(const float* f, int64_t chain_stride, int64_t draw_stride, in
     if (hmcx::pred_scan_smem(pred_form(loss), O) > 227 * 1024) return HMCX_ERR_UNSUPPORTED;
     return hmcx::pred_pass(f, chain_stride, draw_stride, C, n, O, pred_form(loss), y, tau_out, tau_chain_stride,
                            tau_draw_stride, N, i0, k, pointwise, per_output, nonfinite, partials, workspace,
-                           (cudaStream_t)stream);
+                           (cudaStream_t)stream, nullptr);
+}
+
+int hmcx_pred_pass_weighted(const float* f, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t O,
+                            int32_t loss, const float* y, const float* tau_out, int64_t tau_chain_stride,
+                            int64_t tau_draw_stride, int32_t N, int32_t i0, int32_t k, double* pointwise,
+                            double* per_output, int32_t* nonfinite, double* partials, void* workspace,
+                            size_t workspace_bytes, const double* chain_weights, void* stream) {
+    if (!chain_weights) return HMCX_ERR_INVALID_ARG;
+    if (!f || !y || !pointwise || !per_output || !nonfinite || !partials || !workspace || chain_stride < 0 ||
+        draw_stride < 0 || !pred_shape_ok(C, n, k) || O < 1 || O > 0xffffff || N < 1 || i0 < 0 ||
+        (int64_t)i0 + k > N || !pred_loss_ok(loss) ||
+        (loss == HMCX_LOSS_REGRESSION && (!tau_out || tau_chain_stride < 0 || tau_draw_stride < 0)) ||
+        workspace_bytes < hmcx::pred_workspace_bytes(n, O, pred_form(loss), k))
+        return HMCX_ERR_INVALID_ARG;
+    if (hmcx::pred_scan_smem(pred_form(loss), O) > 227 * 1024) return HMCX_ERR_UNSUPPORTED;
+    return hmcx::pred_pass(f, chain_stride, draw_stride, C, n, O, pred_form(loss), y, tau_out, tau_chain_stride,
+                           tau_draw_stride, N, i0, k, pointwise, per_output, nonfinite, partials, workspace,
+                           (cudaStream_t)stream, chain_weights);
 }
 
 int hmcx_pred_totals(const double* partials, int32_t n, int32_t N, double* totals, void* stream) {
@@ -570,6 +593,44 @@ int hmcx_loo_pit_pass(const float* ll, int64_t chain_stride, int64_t draw_stride
     return hmcx::loo_pit_pass(ll, chain_stride, draw_stride, f, f_chain_stride, f_draw_stride, C, n, O, i0, k, r_eff, y,
                               tau_out, tau_chain_stride, tau_draw_stride, pit, pareto_k, nonfinite, workspace,
                               (cudaStream_t)stream);
+}
+
+int hmcx_loo_chain_pass(const float* ll, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t N,
+                        int32_t i0, int32_t k, double r_eff, double* out, int32_t* tail_size, int32_t* nonfinite,
+                        void* stream) {
+    if (!ll || !out || !tail_size || !nonfinite || chain_stride < 0 || draw_stride < 0 || C < 1 || C > 65535 ||
+        n < 2 || n > HMCX_LOO_CHAIN_MAX_DRAWS || N < 1 || i0 < 0 || !rank_slab_ok(k) || (int64_t)i0 + k > N ||
+        !(r_eff > 0.0) || !(r_eff <= DBL_MAX))
+        return HMCX_ERR_INVALID_ARG;
+    return hmcx::loo_chain_pass(ll, chain_stride, draw_stride, C, n, N, i0, k, r_eff, out, tail_size, nonfinite,
+                                (cudaStream_t)stream);
+}
+
+static inline bool stack_shape_ok(int32_t K, int32_t N) {
+    return K >= 1 && K <= 65535 && N >= 1 && (int64_t)K * N <= 0x7fffffffLL;
+}
+
+size_t hmcx_stack_workspace_bytes(int32_t K, int32_t N) {
+    if (!stack_shape_ok(K, N)) return 0;
+    return hmcx::stack_workspace_bytes(K, N);
+}
+
+int hmcx_stack_eval(const double* E, int32_t K, int32_t N, const double* w, double* objective, double* grad,
+                    double* pointwise, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!E || !w || !objective || !grad || !pointwise || !workspace || !stack_shape_ok(K, N) ||
+        workspace_bytes < hmcx::stack_workspace_bytes(K, N))
+        return HMCX_ERR_INVALID_ARG;
+    return hmcx::stack_eval(E, K, N, w, objective, grad, pointwise, workspace, (cudaStream_t)stream);
+}
+
+int hmcx_stack_em(const double* E, int32_t K, int32_t N, double tol, int32_t iterations, double* w, double* objective,
+                  double* grad, double* pointwise, int32_t* state, void* workspace, size_t workspace_bytes,
+                  void* stream) {
+    if (!E || !w || !objective || !grad || !pointwise || !state || !workspace || !stack_shape_ok(K, N) ||
+        iterations < 1 || !(tol >= 0.0) || !(tol <= DBL_MAX) || workspace_bytes < hmcx::stack_workspace_bytes(K, N))
+        return HMCX_ERR_INVALID_ARG;
+    return hmcx::stack_em(E, K, N, tol, iterations, w, objective, grad, pointwise, state, workspace,
+                          (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -49,6 +49,7 @@ struct PredArgs {
     int* nonfinite;       // [N]
     double* terms;        // [2n + PRED_TOTAL_ROWS, k]
     double* rec;          // [n, pred_rec_rows, k]: the sums over the C draws of each step
+    const double* cw;     // [C] chain weights (pred_step_kernel<LOSS, true> only)
 };
 
 __host__ __device__ __forceinline__ int pred_rec_rows(int loss, int O) {
@@ -68,7 +69,10 @@ constexpr int OC = 16;                    // outputs per register chunk of pred_
 //   binary       0..O-1 sum_c sigmoid, O..2O-1 / 2O..3O-1 logsumexp of log p_c(y_o), 3O sum of entropies, 3O+1 non-finite
 //   regression   0..O-1 sum_c e, O..2O-1 sum_c e^2 (e = f - f of draw (0, 1)), 2O..3O-1 sum_c Phi, 3O / 3O+1 logsumexp
 //                of ll_c, 3O+2 sum_c 1/tau, 3O+3 non-finite
-template <int LOSS>
+// WEIGHTED: chain c's terms are scaled by C w_c (its log-densities shifted by log(C w_c)) and chains with w_c = 0 are
+// skipped, so the sums are C times the w-weighted mixture of the chains' draws t, and pred_scan_kernel's divisions by
+// S_t = C t turn them into the mixture of the first t draws of every chain, chain c weighted w_c.
+template <int LOSS, bool WEIGHTED = false>
 __global__ void __launch_bounds__(256) pred_step_kernel(const PredArgs a) {
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= (long long)a.n * a.k) return;
@@ -85,6 +89,14 @@ __global__ void __launch_bounds__(256) pred_step_kernel(const PredArgs a) {
 #pragma unroll
         for (int j = 0; j < OC; ++j) { P[j] = 0.0; Q[j] = LOSS == HMCX_LOSS_BINARY ? -INFINITY : 0.0; R[j] = 0.0; }
         for (int c = 0; c < C; ++c) {
+            double wc = 1.0, lwc = 0.0;
+            if (WEIGHTED) {
+                wc = (double)C * a.cw[c];
+                if (wc == 0.0) continue;
+                lwc = log(wc);
+            }
+            auto sc = [&](double v) { return WEIGHTED ? wc * v : v; };      // a scaled sum term
+            auto sl = [&](double v) { return WEIGHTED ? v + lwc : v; };     // a shifted log term
             const float* z = base + (long long)c * a.cs;
             if (LOSS == HMCX_LOSS_MULTICLASS) {
                 double mx = -INFINITY;
@@ -100,12 +112,12 @@ __global__ void __launch_bounds__(256) pred_step_kernel(const PredArgs a) {
                         const double lp = ((double)v - mx) - ls;
                         h -= xlogx(exp(lp), lp);
                     }
-                    H += h;
-                    lse_add(m, s, ((double)z[(int)yi[0]] - mx) - ls);
+                    H += sc(h);
+                    lse_add(m, s, sl(((double)z[(int)yi[0]] - mx) - ls));
                 }
 #pragma unroll
                 for (int j = 0; j < OC; ++j)
-                    if (o0 + j < O) P[j] += exp(((double)z[o0 + j] - mx) - ls);
+                    if (o0 + j < O) P[j] += sc(exp(((double)z[o0 + j] - mx) - ls));
             } else if (LOSS == HMCX_LOSS_BINARY) {
 #pragma unroll
                 for (int j = 0; j < OC; ++j) {
@@ -116,9 +128,9 @@ __global__ void __launch_bounds__(256) pred_step_kernel(const PredArgs a) {
                     const double l1p = log1p(exp(-fabs(v)));
                     const double ls1 = -(fmax(-v, 0.0) + l1p), ls0 = -(fmax(v, 0.0) + l1p);   // log sigmoid(+-v)
                     const double p = exp(ls1), q = exp(ls0);
-                    P[j] += p;
-                    H -= xlogx(p, ls1) + xlogx(q, ls0);
-                    lse_add(Q[j], R[j], yv * ls1 + (1.0 - yv) * ls0);
+                    P[j] += sc(p);
+                    H -= sc(xlogx(p, ls1) + xlogx(q, ls0));
+                    lse_add(Q[j], R[j], sl(yv * ls1 + (1.0 - yv) * ls0));
                 }
             } else {
                 const double tau = (double)a.tau[(long long)c * a.tcs + (long long)t * a.tds];
@@ -130,17 +142,17 @@ __global__ void __launch_bounds__(256) pred_step_kernel(const PredArgs a) {
                         const double d = (double)v - (double)yi[o];
                         ll -= 0.5 * tau * d * d;
                     }
-                    lse_add(m, s, ll + 0.5 * O * (log(tau) - LOG_2PI));
-                    alea += 1.0 / tau;
+                    lse_add(m, s, sl(ll + 0.5 * O * (log(tau) - LOG_2PI)));
+                    alea += sc(1.0 / tau);
                 }
                 const double sq = sqrt(tau);
 #pragma unroll
                 for (int j = 0; j < OC; ++j) {
                     if (o0 + j >= O) continue;
                     const double v = (double)z[o0 + j], e = v - (double)a.f[(long long)i * O + o0 + j];
-                    P[j] += e;
-                    Q[j] += e * e;
-                    R[j] += normcdf(((double)yi[o0 + j] - v) * sq);
+                    P[j] += sc(e);
+                    Q[j] += sc(e * e);
+                    R[j] += sc(normcdf(((double)yi[o0 + j] - v) * sq));
                 }
             }
         }
@@ -329,10 +341,10 @@ size_t pred_scan_smem(int loss, int O) { return (size_t)pred_sums(loss) * O * PR
 
 int pred_pass(const float* f, long long cs, long long ds, int C, int n, int O, int loss, const float* y, const float* tau,
               long long tcs, long long tds, int N, int i0, int k, double* pointwise, double* per_output, int* nonfinite,
-              double* partials, void* ws, cudaStream_t st) {
+              double* partials, void* ws, cudaStream_t st, const double* cw) {
     const size_t nterms = (2 * (size_t)n + PRED_TOTAL_ROWS) * (size_t)k;
     PredArgs a = {f, cs, ds, C, n, O, N, i0, k, y, tau, tcs, tds, pointwise, per_output, nonfinite, (double*)ws,
-                  (double*)ws + nterms};
+                  (double*)ws + nterms, cw};
     const size_t smem = pred_scan_smem(loss, O);
     if (smem > 227 * 1024) return HMCX_ERR_UNSUPPORTED;
     void (*kern)(PredArgs) = loss == HMCX_LOSS_REGRESSION ? pred_scan_kernel<HMCX_LOSS_REGRESSION>
@@ -343,7 +355,12 @@ int pred_pass(const float* f, long long cs, long long ds, int C, int n, int O, i
         return HMCX_ERR_UNSUPPORTED;
     }
     const long long steps = (long long)n * k;
-    if (loss == HMCX_LOSS_REGRESSION) pred_step_kernel<HMCX_LOSS_REGRESSION><<<(unsigned)((steps + 255) / 256), 256, 0, st>>>(a);
+    const unsigned sb = (unsigned)((steps + 255) / 256);
+    if (cw) {
+        if (loss == HMCX_LOSS_REGRESSION) pred_step_kernel<HMCX_LOSS_REGRESSION, true><<<sb, 256, 0, st>>>(a);
+        else if (loss == HMCX_LOSS_BINARY) pred_step_kernel<HMCX_LOSS_BINARY, true><<<sb, 256, 0, st>>>(a);
+        else pred_step_kernel<HMCX_LOSS_MULTICLASS, true><<<sb, 256, 0, st>>>(a);
+    } else if (loss == HMCX_LOSS_REGRESSION) pred_step_kernel<HMCX_LOSS_REGRESSION><<<(unsigned)((steps + 255) / 256), 256, 0, st>>>(a);
     else if (loss == HMCX_LOSS_BINARY) pred_step_kernel<HMCX_LOSS_BINARY><<<(unsigned)((steps + 255) / 256), 256, 0, st>>>(a);
     else pred_step_kernel<HMCX_LOSS_MULTICLASS><<<(unsigned)((steps + 255) / 256), 256, 0, st>>>(a);
     const int g0 = i0 / PRED_GROUP, ng = (i0 + k - 1) / PRED_GROUP - g0 + 1;

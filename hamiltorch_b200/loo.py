@@ -9,6 +9,8 @@ ArviZ's ``az.loo`` / ``az.waic`` and PyMC report, restated in numpy fp64 by test
     lo = hamiltorch_b200.loo.reloo(lo, target, params_init, num_samples=..., ...)   # exact refits where k-hat is high
     f = hamiltorch_b200.loo.kfold_split(N, K)                   # K-fold CV: one launch fits every fold
     kf = hamiltorch_b200.loo.kfold(sample_chains(target, params_init, folds=f, ...), target)
+    st = hamiltorch_b200.loo.chain_stacking(res, target)        # chain weights of a non-mixing run (psis_loo_chains)
+    hamiltorch_b200.loo.stacking_weights(lo_a, lo_b)            # model stacking weights
 
 ``target`` is the ``MLPTarget`` of ``define_model_log_prob`` or the list ``define_split_model_log_prob`` returns (data
 points in split order).  Two CUDA passes:
@@ -484,3 +486,218 @@ def reloo(lo, target, params_init, **sample_kwargs):
     out.num_bad_k = int((out.pareto_k > out.k_threshold).sum())
     return out
 
+
+
+# ------------------------------------------------------------------------------------------------------------------
+# Per-chain PSIS-LOO and stacking (Yao, Vehtari, Simpson & Gelman 2018; Yao, Vehtari & Gelman 2022)
+# ------------------------------------------------------------------------------------------------------------------
+class ChainLooResult:
+    """``psis_loo_chains``: per chain and point (C, N) fp64 on the block's device -- ``pointwise`` (elpd_loo_ci of chain
+    c's draws alone), ``lppd``, ``pareto_k``, ``tail_size`` (int32, M'); per chain (C,) fp64 ``elpd_loo`` and ``se`` =
+    sqrt(N) sd(pointwise[c]) (ddof 1), ``num_bad_k`` (C,) int64 (points with pareto_k above ``k_threshold`` = min(1 -
+    1/log10 n, 0.7)); ``num_nonfinite`` ((chain, point) pairs with a non-finite draw: NaN outputs), ``num_chains``,
+    ``num_draws`` (n, per chain), ``num_points``, ``r_eff``."""
+
+    kind = 'loo_chains'
+
+    def __repr__(self):
+        return ('ChainLooResult(C=%d, n=%d, N=%d, elpd_loo per chain in [%.3f, %.3f], bad k-hat=%d, nonfinite=%d)'
+                % (self.num_chains, self.num_draws, self.num_points, float(self.elpd_loo.min()),
+                   float(self.elpd_loo.max()), int(self.num_bad_k.sum()), self.num_nonfinite))
+
+
+class StackingResult:
+    """``stacking_weights`` / ``chain_stacking``: ``weights`` (K,) fp64 on the simplex (input order: models, or chains);
+    ``pointwise`` (N,) = log sum_k w_k exp(E_ki), ``elpd`` = its sum and ``se`` = sqrt(N) sd(pointwise) (ddof 1).
+    ``elpd`` is optimistic: the weights were fitted to the same leave-one-out densities they are scored on, so it is not
+    an estimate of the stacked predictive's out-of-sample elpd (score held-out data with ``predictive.evaluate(...,
+    chain_weights=weights)`` for that).  ``objective`` = elpd as fitted, ``kkt_gap`` = max_k g_k / N - 1 (>= 0; the
+    stopping rule bounds the shortfall from the optimum by N kkt_gap), ``iterations`` (EM updates), ``converged``
+    (kkt_gap <= tol), ``num_rows`` (K), ``num_points`` (N), and for ``chain_stacking`` ``chain_loo`` (the
+    ``ChainLooResult``; None for models)."""
+
+    def __repr__(self):
+        return ('StackingResult(K=%d, N=%d, elpd=%.3f (optimistic), se=%.3f, kkt_gap=%.2e, iterations=%d, converged=%s)'
+                % (self.num_rows, self.num_points, self.elpd, self.se, self.kkt_gap, self.iterations, self.converged))
+
+
+def _draws_per_chain(x):
+    """n of what ``diagnostics.as_block`` reads, without touching the device (None when it cannot tell)."""
+    from .engine import HMCResult
+    if isinstance(x, HMCResult):
+        x = x.samples_padded
+    if isinstance(x, (list, tuple)):
+        return len(x)
+    if torch.is_tensor(x):
+        return int(x.shape[1]) if x.dim() == 3 else int(x.shape[0]) if x.dim() == 2 else None
+    return None
+
+
+def _chain_slab_points(Np, S, per_point):
+    """Points per slab of the per-chain pass: from samples, the slab's fp32 likelihood block within the budget."""
+    if _slab_points_override is not None:
+        return max(1, min(Np, N.RANK_MAX_SLAB, int(_slab_points_override)))
+    k = max(1, min(Np, N.RANK_MAX_SLAB, _diag.RANK_WORKSPACE_BUDGET // max(1, per_point)))
+    if per_point and _ROW_TILE <= k < Np:
+        k -= k % _ROW_TILE
+    return k
+
+
+def psis_loo_chains(x, target=None, r_eff=1.0, tau_out=None):
+    """PSIS-LOO of every chain on its own: for each chain c and point i, the PSIS-LOO of ``psis_loo`` over chain c's n
+    draws only (tail M = ceil(min(0.2 n, 3 sqrt(n / r_eff)))).  Column c is bit for bit ``psis_loo(ll[c:c+1])``.  These
+    are the rows ``chain_stacking`` weighs: chains that sit in different modes of a multimodal posterior give different
+    leave-one-out predictives, and stacking them uses draws that pooled estimators weigh equally.
+
+    ``x`` / ``target`` / ``r_eff`` / ``tau_out`` as ``psis_loo`` (a tempered run's result brings its cold rows).  Each
+    chain's draws are sorted in one CTA's shared memory, so n <= 8192 draws per chain (``thin`` a longer run).  K-fold
+    runs are refused: their chains are fits of different data.  Returns a ``ChainLooResult``."""
+    if getattr(x, 'folds', None) is not None:
+        raise TypeError('psis_loo_chains: this is a K-fold run (sample_chains(..., folds=...)): its chains are fits of '
+                        'different data, so their leave-one-out densities are not comparable; use kfold')
+    n = _draws_per_chain(x)
+    if n is not None and n > N.LOO_CHAIN_MAX_DRAWS:
+        raise RuntimeError('psis_loo_chains: %d draws per chain exceed the %d a chain\'s shared-memory sort holds; thin '
+                           'the run (sample_chains(..., thin=...), or x[:, ::t])' % (n, N.LOO_CHAIN_MAX_DRAWS))
+    blk, r_eff, tau = _prepare(x, target, r_eff, tau_out)
+    C_, n = int(blk.shape[0]), int(blk.shape[1])
+    if C_ > 65535:
+        raise RuntimeError('psis_loo_chains: at most 65535 chains, got %d' % C_)
+    N.require_cuda()
+    lib = N.load_library()
+    dev = blk.device
+    if target is None:
+        Np = int(blk.shape[2])
+        k = _chain_slab_points(Np, C_ * n, 0)
+        nt = None
+    else:
+        nt = _native_target(target, dev)
+        Np = int(nt.mlp_struct.num_rows)
+        k = _chain_slab_points(Np, C_ * n, 4 * C_ * n)
+    out = torch.empty((3, C_, Np), dtype=torch.float64, device=dev)
+    tail = torch.empty((C_, Np), dtype=torch.int32, device=dev)
+    flag = torch.empty((C_, Np), dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        st = N.stream_ptr(dev)
+        lb = None if nt is None else torch.empty((C_, n, k), dtype=torch.float32, device=dev)
+        for i0 in range(0, Np, k):
+            kk = min(k, Np - i0)
+            if nt is None:
+                src, base = blk, N.ptr(blk)
+            else:
+                _ll_rows(lib, nt, blk, i0, i0 + kk, lb, tau)
+                src, base = lb, C.c_void_p(lb.data_ptr() - 4 * i0)   # point i at column i - i0 of the slab's block
+            rc = lib.hmcx_loo_chain_pass(base, src.stride(0), src.stride(1), C_, n, Np, i0, kk, float(r_eff),
+                                         N.ptr(out), N.ptr(tail), N.ptr(flag), st)
+            N.check(rc, 'hmcx_loo_chain_pass')
+    r = ChainLooResult()
+    r.pointwise, r.lppd, r.pareto_k, r.tail_size = out[0], out[1], out[2], tail
+    r.elpd_loo = out[0].sum(1)
+    r.se = math.sqrt(Np) * out[0].std(1, unbiased=True) if Np > 1 else torch.full_like(r.elpd_loo, float('nan'))
+    r.k_threshold = min(1.0 - 1.0 / math.log10(n), 0.7)
+    r.num_bad_k = (out[2] > r.k_threshold).sum(1)
+    r.num_nonfinite = int((flag != 0).sum())
+    r.num_chains, r.num_draws, r.num_points, r.r_eff = C_, n, Np, r_eff
+    return r
+
+
+def _stack_args(tol, max_iter, prefix):
+    t = float(tol)
+    if not (t > 0.0 and math.isfinite(t)):
+        raise ValueError('%s: tol must be a finite positive number, got %r' % (prefix, tol))
+    if isinstance(max_iter, bool) or int(max_iter) != max_iter or int(max_iter) < 1:
+        raise ValueError('%s: max_iter must be a positive integer, got %r' % (prefix, max_iter))
+    return t, int(max_iter)
+
+
+def _stack(E, tol, max_iter, prefix):
+    """Stacking weights of the rows of E (K, N) fp64 CUDA: the EM update on the device from uniform weights, the
+    converged flag read back once per batch of iterations (batches of 16, doubling up to 1024)."""
+    K, Np = int(E.shape[0]), int(E.shape[1])
+    bad = int((~torch.isfinite(E)).sum())
+    if bad:
+        raise ValueError('%s: %d of the %d x %d pointwise log densities are not finite; every point must be scored by '
+                         'every row (a non-finite draw makes its point NaN)' % (prefix, bad, K, Np))
+    N.require_cuda()
+    lib = N.load_library()
+    dev = E.device
+    E = E.contiguous()
+    w = torch.full((K,), 1.0 / K, dtype=torch.float64, device=dev)
+    obj = torch.empty(1, dtype=torch.float64, device=dev)
+    grad = torch.empty(K, dtype=torch.float64, device=dev)
+    pw = torch.empty(Np, dtype=torch.float64, device=dev)
+    state = torch.zeros(2, dtype=torch.int32, device=dev)
+    ws_bytes = lib.hmcx_stack_workspace_bytes(K, Np)
+    if ws_bytes == 0:
+        raise RuntimeError('%s: %d rows x %d points are beyond the stacking pass' % (prefix, K, Np))
+    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    with torch.cuda.device(dev):
+        st = N.stream_ptr(dev)
+        done, batch = 0, 16
+        while done < max_iter:
+            it = min(batch, max_iter - done)
+            rc = lib.hmcx_stack_em(N.ptr(E), K, Np, tol, it, N.ptr(w), N.ptr(obj), N.ptr(grad), N.ptr(pw),
+                                   N.ptr(state), N.ptr(ws), ws_bytes, st)
+            N.check(rc, 'hmcx_stack_em')
+            done += it
+            batch = min(2 * batch, 1024)
+            if int(state[0]):
+                break
+        # the evaluation at the returned weights (after max_iter updates the last one has not been evaluated yet)
+        rc = lib.hmcx_stack_eval(N.ptr(E), K, Np, N.ptr(w), N.ptr(obj), N.ptr(grad), N.ptr(pw), N.ptr(ws), ws_bytes, st)
+        N.check(rc, 'hmcx_stack_eval')
+    s = state.cpu()
+    r = StackingResult()
+    r.weights, r.pointwise = w, pw
+    r.objective = float(obj)
+    r.elpd, r.se = _total(pw)
+    r.kkt_gap = float(grad.max()) / Np - 1.0
+    r.iterations = int(s[1])
+    r.converged = bool(s[0]) or r.kkt_gap <= tol
+    r.num_rows, r.num_points, r.tol = K, Np, tol
+    r.chain_loo = None
+    return r
+
+
+def stacking_weights(*results, tol=1e-6, max_iter=20000):
+    """Model stacking weights (Yao, Vehtari, Simpson & Gelman 2018; ArviZ ``compare``'s default, Stan's
+    ``loo_model_weights``): the weights w on the simplex that maximise sum_i log sum_k w_k exp(elpd_ki) over the
+    models' pointwise leave-one-out densities -- ``psis_loo`` (``reloo`` included), ``waic`` or ``kfold`` results of one
+    kind on the same N points, refused otherwise as ``compare`` refuses them.  The multiplicative (EM) update runs on the
+    GPU in fp64 from uniform weights until max_k g_k <= N (1 + tol), g the gradient, or ``max_iter`` updates; the
+    objective is then within N tol of its maximum.  A model whose predictive is dominated by the others' mixture gets
+    weight ~0; duplicates share their weight.  A non-finite pointwise value is refused.  Returns a ``StackingResult``
+    (``elpd`` is optimistic: the weights were fitted to the same densities)."""
+    tol, max_iter = _stack_args(tol, max_iter, 'stacking_weights')
+    if len(results) == 1 and isinstance(results[0], (list, tuple)):
+        results = tuple(results[0])
+    if len(results) < 2:
+        raise ValueError('stacking_weights: need at least two results')
+    kinds = {getattr(r, 'kind', None) for r in results}
+    if len(kinds) != 1 or kinds.pop() not in _ELPD:
+        raise TypeError('stacking_weights: pass psis_loo results only, waic results only or kfold results only')
+    n0 = results[0].num_points
+    if any(r.num_points != n0 for r in results):
+        raise RuntimeError('stacking_weights: the results score different numbers of data points (%s); models are '
+                           'compared on the same data' % ', '.join(str(r.num_points) for r in results))
+    dev = results[0].pointwise.device
+    E = torch.stack([r.pointwise.to(device=dev, dtype=torch.float64) for r in results])
+    if not E.is_cuda:
+        raise RuntimeError('stacking_weights: the pointwise values are %s tensors; stacking runs on a CUDA device'
+                           % E.device.type)
+    return _stack(E, tol, max_iter, 'stacking_weights')
+
+
+def chain_stacking(x, target=None, r_eff=1.0, tau_out=None, tol=1e-6, max_iter=20000):
+    """Stacking of the chains of one run (Yao, Vehtari & Gelman 2022, *Stacking for non-mixing Bayesian computations*):
+    ``psis_loo_chains`` gives every chain's own leave-one-out predictive, and the chain weights maximise the leave-one-out
+    log score of their mixture, as ``stacking_weights`` does for models.  A run where some chains are stuck in a poor mode
+    is reweighted towards the chains that predict well, with no new sampling; score the stacked predictive on held-out
+    data with ``predictive.evaluate(..., chain_weights=result.weights)``.  Arguments as ``psis_loo_chains`` and
+    ``stacking_weights``.  Returns a ``StackingResult`` with ``chain_loo``; its ``elpd`` is optimistic (the weights were
+    fitted to the same leave-one-out densities)."""
+    tol, max_iter = _stack_args(tol, max_iter, 'chain_stacking')
+    cl = psis_loo_chains(x, target, r_eff, tau_out)
+    r = _stack(cl.pointwise, tol, max_iter, 'chain_stacking')
+    r.chain_loo = cl
+    return r

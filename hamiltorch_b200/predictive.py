@@ -56,7 +56,8 @@ class PredictiveResult:
     ``*_se`` (sd / sqrt N, ddof 1, of the per-point values), ``ece`` and ``reliability`` (15, 3) = count, mean confidence,
     accuracy per bin (NaN for an empty bin); regression ``rmse`` and ``coverage`` {level: fraction}.  Curves (n,) fp64:
     ``nll_curve`` and ``accuracy_curve`` or ``rmse_curve``.  ``num_nonfinite`` counts points with a non-finite output
-    (NaN outputs, NaN totals); ``num_points``, ``num_draws``, ``model_loss``."""
+    (NaN outputs, NaN totals); ``num_points``, ``num_draws``, ``model_loss``; ``chain_weights`` ((C,) fp64 CPU, the
+    normalised weights of a weighted evaluation, or None for the pooled draws)."""
 
     def __repr__(self):
         if self.model_loss == 'regression':
@@ -149,8 +150,30 @@ def _slab_points(lib, C_, n, O_, loss, Np, block_per_point):
     return k
 
 
-def _run(lib, dev, C_, n, O_, Np, loss, y, tau, fill):
-    """Drive hmcx_pred_pass over the slabs; ``fill(i0, kk)`` returns (base pointer of point 0, chain / draw strides)."""
+def _chain_weights(w):
+    """``chain_weights`` as a 1-D fp64 CPU tensor, normalised; refused unless finite, non-negative and summing to 1
+    within 1e-6."""
+    if w is None:
+        return None
+    t = torch.as_tensor(w).detach().to(device='cpu', dtype=torch.float64)
+    if t.dim() != 1 or t.numel() < 1:
+        raise ValueError('predictive: chain_weights must be a (C,) vector, got shape %s' % (tuple(t.shape),))
+    if not bool(torch.isfinite(t).all()) or bool((t < 0).any()):
+        raise ValueError('predictive: chain_weights must be finite and non-negative')
+    total = float(t.sum())
+    if abs(total - 1.0) > 1e-6:
+        raise ValueError('predictive: chain_weights must sum to 1 (within 1e-6), got %.9g' % total)
+    return t / total
+
+
+def _check_chain_weights(w, C_):
+    if w is not None and w.numel() != C_:
+        raise ValueError('predictive: chain_weights holds %d weights, the draws come from %d chains' % (w.numel(), C_))
+
+
+def _run(lib, dev, C_, n, O_, Np, loss, y, tau, fill, cw=None):
+    """Drive hmcx_pred_pass (hmcx_pred_pass_weighted with chain weights ``cw``) over the slabs; ``fill(i0, kk)`` returns
+    (base pointer of point 0, chain / draw strides)."""
     G = (Np + _GROUP - 1) // _GROUP
     rows = 2 * n + _TOTAL_ROWS
     pw = torch.empty((7, Np), dtype=torch.float64, device=dev)
@@ -162,15 +185,21 @@ def _run(lib, dev, C_, n, O_, Np, loss, y, tau, fill):
     k = fill.k
     ws_bytes = lib.hmcx_pred_workspace_bytes(C_, n, O_, loss, k)
     ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev)
+    cwd = None if cw is None else cw.to(dev)
     with torch.cuda.device(dev):
         st = N.stream_ptr(dev)
         for i0 in range(0, Np, k):
             kk = min(k, Np - i0)
             base, cs, ds = fill(i0, kk)
-            rc = lib.hmcx_pred_pass(base, cs, ds, C_, n, O_, loss, N.ptr(yd), N.ptr(tau),
-                                    0 if tau is None else tau.stride(0), 0 if tau is None else tau.stride(1), Np, i0, kk,
-                                    N.ptr(pw), N.ptr(po), N.ptr(flag), N.ptr(partials), N.ptr(ws), ws_bytes, st)
-            N.check(rc, 'hmcx_pred_pass')
+            args = (base, cs, ds, C_, n, O_, loss, N.ptr(yd), N.ptr(tau), 0 if tau is None else tau.stride(0),
+                    0 if tau is None else tau.stride(1), Np, i0, kk, N.ptr(pw), N.ptr(po), N.ptr(flag), N.ptr(partials),
+                    N.ptr(ws), ws_bytes)
+            if cwd is None:
+                rc = lib.hmcx_pred_pass(*args, st)
+                N.check(rc, 'hmcx_pred_pass')
+            else:
+                rc = lib.hmcx_pred_pass_weighted(*args, N.ptr(cwd), st)
+                N.check(rc, 'hmcx_pred_pass_weighted')
         N.check(lib.hmcx_pred_totals(N.ptr(partials), n, Np, N.ptr(totals), st), 'hmcx_pred_totals')
     return pw, po, flag, totals
 
@@ -225,7 +254,7 @@ def _sd_se(v):
     return float(v.std(unbiased=True) / math.sqrt(n)) if n > 1 else float('nan')
 
 
-def evaluate(x, target=None, *, y=None, model_loss=None, tau_out=None):
+def evaluate(x, target=None, *, y=None, model_loss=None, tau_out=None, chain_weights=None):
     """Score the posterior predictive of a Bayesian NN on held-out data, on the GPU.
 
     Two routes:
@@ -237,7 +266,12 @@ def evaluate(x, target=None, *, y=None, model_loss=None, tau_out=None):
     ``tau_out`` (regression only): a number, or one noise precision per draw, (C, n) (or (n,) for one chain); an
     ``HMCResult`` of a run with a tau_out hyperprior brings its ``tau_out_trace``; otherwise the target's value.  An
     outputs block of a regression without a target needs it.  See the module docstring for the definitions.
-    Returns a ``PredictiveResult``."""
+    ``chain_weights``: (C,) non-negative weights summing to 1 (normalised; refused if off by more than 1e-6), e.g.
+    ``loo.chain_stacking(...).weights``.  The predictive is then the mixture sum_c w_c (chain c's draws, equally
+    weighted) instead of the pooled draws, and every curve entry t the same mixture of the first t draws of every chain;
+    chains with weight 0 are not read.  None: the pooled predictive.
+    Returns a ``PredictiveResult`` (its ``chain_weights``: the normalised weights, or None)."""
+    cw = _chain_weights(chain_weights)
     if target is not None and not (torch.is_tensor(x) and x.dim() == 4):
         loss, O_, yv, tau_t = _target_data(target)
         if y is not None or model_loss is not None:
@@ -246,6 +280,7 @@ def evaluate(x, target=None, *, y=None, model_loss=None, tau_out=None):
         yv = _check_y(yv, loss, O_, Np)
         blk = _loo._samples_block(x, target)
         C_, n = int(blk.shape[0]), int(blk.shape[1])
+        _check_chain_weights(cw, C_)
         tau = _tau(tau_out, x, C_, n, blk.device) if loss == T.LOSS_REGRESSION else None
         if loss == T.LOSS_REGRESSION and tau is None:
             tau = _tau(tau_t, None, C_, n, blk.device)
@@ -265,6 +300,7 @@ def evaluate(x, target=None, *, y=None, model_loss=None, tau_out=None):
             loss, yv, tau_t, O_ = _loss_id(model_loss), y, None, None
         f = _outputs_block(x)
         C_, n, Np = int(f.shape[0]), int(f.shape[1]), int(f.shape[2])
+        _check_chain_weights(cw, C_)
         if O_ is not None and int(f.shape[3]) != O_:
             raise RuntimeError('predictive: the block has %d outputs per point, the target %d' % (f.shape[3], O_))
         O_ = int(f.shape[3])
@@ -280,8 +316,10 @@ def evaluate(x, target=None, *, y=None, model_loss=None, tau_out=None):
         N.require_cuda()
         lib = N.load_library()
         fill = _FromBlock(f, _slab_points(lib, C_, n, O_, loss, Np, 0))
-    pw, po, flag, tot = _run(lib, fill.device, C_, n, O_, Np, loss, yv, tau, fill)
-    return _result(pw, po, flag, tot, loss, C_, n, O_, Np)
+    pw, po, flag, tot = _run(lib, fill.device, C_, n, O_, Np, loss, yv, tau, fill, cw)
+    r = _result(pw, po, flag, tot, loss, C_, n, O_, Np)
+    r.chain_weights = cw
+    return r
 
 
 def _result(pw, po, flag, tot, loss, C_, n, O_, Np):

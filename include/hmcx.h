@@ -806,6 +806,52 @@ int hmcx_loo_pit_pass(const float* ll, int64_t chain_stride, int64_t draw_stride
                       int64_t tau_draw_stride, double* pit, double* pareto_k, int32_t* nonfinite, void* workspace,
                       size_t workspace_bytes, void* stream);
 
+/*
+ * Stacking of chains and models (additive v12 symbols; DESIGN §3.21, hamiltorch_b200/loo.py).  Callers of an older v12
+ * library check for the symbols.
+ *   hmcx_loo_chain_pass  per-chain PSIS-LOO of the points [i0, i0 + k) of the block ll (the strides of hmcx_loo_pass, N
+ *                    points): for every chain c the PSIS-LOO of hmcx_loo_pass over that chain's n draws alone, M =
+ *                    ceil(min(0.2 n, 3 sqrt(n / r_eff))).  One CTA per (point, chain) sorts the chain's n keys in shared
+ *                    memory, so n <= HMCX_LOO_CHAIN_MAX_DRAWS; no workspace.  out [3, C, N] fp64, rows: 0 elpd_loo,
+ *                    1 lppd, 2 pareto_k -- column c the bits hmcx_loo_pass writes (rows 0, 3, 2) for the one-chain block
+ *                    of chain c; tail_size [C, N] int32 (M'); nonfinite [C, N] int32 (1: the chain has a non-finite draw
+ *                    at the point, its three outputs NaN).  NULL pointers, C < 1 or > 65535, n < 2 or >
+ *                    HMCX_LOO_CHAIN_MAX_DRAWS, negative strides, a slab outside [0, N), k > HMCX_RANK_MAX_SLAB or r_eff
+ *                    not in (0, inf): HMCX_ERR_INVALID_ARG.
+ *   hmcx_stack_workspace_bytes  workspace of hmcx_stack_eval / hmcx_stack_em: 8 (K N + (K + 1) ceil(N / 128)) bytes (0 for
+ *                    K < 1, K > 65535, N < 1 or K N > INT32_MAX).
+ *   hmcx_stack_eval  for E [K, N] fp64 and weights w [K] fp64 (device): pointwise [N] = m_i + log sum_k w_k exp(E_ki - m_i),
+ *                    m_i = max_k E_ki (rows with w_k = 0 add nothing); objective [1] = sum_i pointwise_i; grad [K] =
+ *                    sum_i exp(E_ki - m_i) / s_i, s_i the inner sum.  Sums over points in 128-point groups in point
+ *                    order, then the groups in order; no atomics, so the same inputs give the same bits.
+ *   hmcx_stack_em    `iterations` rounds of: hmcx_stack_eval at w, then, unless max_k grad_k <= N (1 + tol) (state[0] :=
+ *                    1, and every later round of this and later calls does nothing), w_k := w_k grad_k / N and state[1]
+ *                    += 1.  state [2] int32 device (0, 0 to start).  Once converged, objective / grad / pointwise hold
+ *                    the evaluation at the returned w.
+ *                    NULL pointers, bad shapes, iterations < 1, tol not in [0, inf) or a workspace smaller than
+ *                    hmcx_stack_workspace_bytes(K, N): HMCX_ERR_INVALID_ARG.
+ *   hmcx_pred_pass_weighted  hmcx_pred_pass over the mixture sum_c w_c (chain c's draws, equally weighted), chain_weights
+ *                    [C] fp64 device, non-negative and summing to 1: every per-step sum takes chain c's terms scaled by
+ *                    C w_c and its log-densities shifted by log(C w_c); chains with w_c = 0 are not read (but the first
+ *                    draw of chain 0 is the regression moments' shift).  Curves: the mixture of the first t draws of every
+ *                    chain.  The checks of hmcx_pred_pass, and NULL chain_weights: HMCX_ERR_INVALID_ARG.
+ */
+#define HMCX_LOO_CHAIN_MAX_DRAWS 8192          /* 2 n uint32 keys of a chain in 64 KB of shared memory */
+int hmcx_loo_chain_pass(const float* ll, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t N,
+                        int32_t i0, int32_t k, double r_eff, double* out, int32_t* tail_size, int32_t* nonfinite,
+                        void* stream);
+size_t hmcx_stack_workspace_bytes(int32_t K, int32_t N);
+int hmcx_stack_eval(const double* E, int32_t K, int32_t N, const double* w, double* objective, double* grad,
+                    double* pointwise, void* workspace, size_t workspace_bytes, void* stream);
+int hmcx_stack_em(const double* E, int32_t K, int32_t N, double tol, int32_t iterations, double* w, double* objective,
+                  double* grad, double* pointwise, int32_t* state, void* workspace, size_t workspace_bytes,
+                  void* stream);
+int hmcx_pred_pass_weighted(const float* f, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t O,
+                            int32_t loss, const float* y, const float* tau_out, int64_t tau_chain_stride,
+                            int64_t tau_draw_stride, int32_t N, int32_t i0, int32_t k, double* pointwise,
+                            double* per_output, int32_t* nonfinite, double* partials, void* workspace,
+                            size_t workspace_bytes, const double* chain_weights, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
