@@ -1,7 +1,9 @@
-"""fp64 per-iteration replay of the dense (chains x D).(D x D) and the coupled sampling paths.
+"""fp64 per-iteration replay of the dense (chains x D).(D x D), the coupled and the element-wise sampling paths.
 
 A plain batched torch restatement, in fp64 and vectorised over chains, of what hmcx_tc.cu computes for
-GaussianIso / GaussianDiag / GaussianFull targets, and hmc_small_kernel / hmcx_coupled.cu for those and Neal's funnel:
+GaussianIso / GaussianDiag / GaussianFull targets, hmc_small_kernel / hmcx_coupled.cu for those and Neal's funnel, and
+the element-wise persistent loop of hmcx_hmc.cu (hmc_run_kernel, hmc_run_big_kernel) for GaussianIso / GaussianDiag
+with inv_mass None or (D,):
 HMC and HMC_NUTS with inv_mass None, 1-D or 2-D (the reference's
 gibbs samplers.py:185-202, leapfrog :267-304, hamiltonian :779-815 and rho = min(0, H_old - H_new) :626), and
 constant-metric RMHMC (explicit A-B-C-B-A :389-462 with the sequential C rotation, implicit :305-387, whose fixed
@@ -12,6 +14,9 @@ Per-iteration replay, not a free-running chain: iteration n >= burn + 2 restarts
 n - 1 - burn; iterations up to burn + 1 (whose states are not retained) start from the replay's own proposals, chosen
 by the kernel's decisions.  So no error accumulates along the chain, a decision flip does not end the comparison, and
 every iteration of every chain is checked (``check``).
+
+The element-wise kernels keep the reference's fp32 operation order, so their retained rows are also held bit for bit to
+an fp32 replay of the same kind (``replay_rows32``).
 """
 import math
 
@@ -277,3 +282,53 @@ def dual_averaging(ham, burn, step_size, desired_accept_rate=0.8, diverged=None)
             out[:, n] = torch.exp(x_new)
     out[:, burn] = eps_bar
     return out
+
+
+def replay_rows32(tag, target, inv_mass, params_init, accepted, samples, normals, eps, L, burn, mass_factor=None):
+    """fp32 per-iteration replay of an element-wise run (GaussianIso / GaussianDiag, inv_mass None or (D,)): every
+    accepted retained row must equal, bit for bit, the trajectory of oracle/hmc_oracle.leapfrog_hmc restated batched
+    over chains in its fp32 operation order (p + (0.5 eps) g, q + (eps inv_mass) p, g = -x or -(inv_var (x - mean)), the
+    gradient autograd gives for targets.py).  It restarts from the kernel's own row like ``replay``; the warm-up states
+    (not retained) are its own, chosen by the kernel's decisions.  The momentum is z times the mass factor
+    ``mass_factor`` (default (1 / inv_mass) ** 0.5, the operand engine.NativeMass passes).  Runs on the device of
+    ``samples``; returns the number of rows compared."""
+    f32 = torch.float32
+    C, D = params_init.shape
+    S = accepted.shape[1]
+    dev = samples.device
+    diag = isinstance(target, T.GaussianDiag)
+    mean = target.mean.to(dev, f32) if diag else None
+    iv = target.inv_var.to(dev, f32) if diag else None
+    im = None if inv_mass is None else inv_mass.to(dev, f32)
+    if im is not None and mass_factor is None:
+        mass_factor = (1 / inv_mass.detach().to(f32)) ** 0.5
+    sd = None if im is None else mass_factor.to(dev, f32)
+
+    def grad(q):
+        return -q if iv is None else -(iv * (q - mean))
+
+    acc = accepted.to(dev).bool()
+    rows = samples[..., :D].to(dev, f32)
+    eps = eps.to(dev, f32)
+    start = params_init.to(dev, f32)
+    compared = 0
+    for n in range(S):
+        if n >= burn + 2:
+            start = rows[:, n - 1 - burn]
+        z = normals[n][..., :D].to(dev, f32)
+        p = z if sd is None else z * sd
+        e = (eps[n] if eps.dim() == 2 else eps)[:, None]
+        p = p + (0.5 * e) * grad(start)                                         # :281
+        q = start
+        for _ in range(L):
+            q = q + e * p if im is None else q + e * im * p                     # :284 / :296
+            p = p + e * grad(q)
+        if n > burn:
+            take = acc[:, n]
+            bad = (rows[:, n - burn].view(torch.int32) != q.view(torch.int32)).any(1) & take
+            assert not bool(bad.any()), '%s: %d accepted rows of iteration %d differ bit-wise from the fp32 replay ' \
+                '(first chain %d)' % (tag, int(bad.sum()), n, int(torch.nonzero(bad)[0]))
+            compared += int(take.sum())
+        else:
+            start = torch.where(acc[:, n, None], q, start)
+    return compared

@@ -3,13 +3,16 @@
 
 * It accepts the unmodified reference's chains (the committed fixtures) as if they were kernel output: identical
   decisions, states and Hamiltonians within FIXTURE_BOUND (funnel11_nuts, whose LogProbError iterations go through
-  check(diverged=) and dual_averaging(diverged=), within FUNNEL_NUTS_BOUND).
+  check(diverged=) and dual_averaging(diverged=), within FUNNEL_NUTS_BOUND).  The element-wise fixtures' accepted rows
+  also equal the fp32 replay (replay_rows32) bit for bit.
 * It accepts the fp32 oracle's chains at D = 250 (a full target with a full and with a diagonal mass) within
   ORACLE_BOUND.
 * It rejects the same oracle runs made with one 64-column block of the precision or of inv_mass off by a relative 1e-4
   (of the order of one missing lo term of a 3xTF32 product, an estimate): the harness catches a one-tile error.
 * It accepts the fp32 oracle's funnel chains at D = 16 and rejects them when the oracle's exp(v) sum(x^2) term is
   scaled by 1 + 1e-4.
+* It accepts the fp32 oracle's element-wise chains at D = 250 (GaussianDiag, diagonal mass) and rejects them when one
+  inv_var element is one ulp off, or the mass factor of a 64-column block is.
 """
 import copy
 import os
@@ -47,9 +50,13 @@ def _run(model, init, acc, samples, z, logu, ham, eps, L, burn, tag, bound):
     return dense_ref.check(tag, rep, init, samples, acc, ham, logu, burn, ceiling=bound)
 
 
+# the element-wise fixtures (GaussianIso / GaussianDiag, inv_mass None or (D,)): the kernels of hmcx_hmc.cu
+ELEMENTWISE = ['cfg1_gauss3', 'iso256', 'diag48_mass', 'diag16_rejects', 'nuts_iso128']
+
+
 @pytest.mark.parametrize('name', ['full48_dense', 'full40_fullmass', 'iso40_fullmass_nuts', 'iso40_blockmass',
                                   'cfg1_corr_gauss3', 'diag5_fullmass', 'diag6_blockmass', 'funnel11_hmc',
-                                  'funnel11_nuts'])
+                                  'funnel11_nuts'] + ELEMENTWISE)
 def test_replay_accepts_the_reference_hmc_chains(name):
     case = K.plain_cases()[name]
     kw = case['kw']
@@ -72,6 +79,10 @@ def test_replay_accepts_the_reference_hmc_chains(name):
                             ceiling=FUNNEL_NUTS_BOUND if name == 'funnel11_nuts' else FIXTURE_BOUND, diverged=diverged)
     assert flips == 0
     assert bool(diverged.any()) == (name == 'funnel11_nuts')
+    if name in ELEMENTWISE:                                  # and every accepted retained row, bit for bit
+        n = dense_ref.replay_rows32('cpu_replay/' + name, case['target'], kw.get('inv_mass'), init, t('accepted'),
+                                    t('samples'), z, eps, L, burn)
+        assert n == int(t('accepted')[:, burn + 1:].sum()) > 0
 
 
 @pytest.mark.parametrize('name', ['rmhmc_exp_hess_full24', 'rmhmc_imp_softabs_diag20'])
@@ -189,3 +200,54 @@ def test_replay_checks_the_funnel(rel):
             _run(*args)
     else:
         assert _run(*args) == 0
+
+
+# ---- element-wise chains: the fp32 oracle at D = 250, with one inv_var element or a block of the mass factor one ulp off --
+def _elem_problem():
+    g = torch.Generator().manual_seed(11)
+    tgt = T.GaussianDiag(torch.linspace(-1, 1, D250), 0.5 + torch.rand(D250, generator=g))
+    return tgt, 0.5 + torch.rand(D250, generator=g)
+
+
+def _elem_oracle(tgt, im):
+    outs, inits, zs, lus = [], [], [], []
+    for c in range(C3):
+        init, z, logu, _ = O.reference_stream(500 + c, D250, S6, prior=lambda: tgt.mean + torch.randn(D250))
+        outs.append(O.sample_hmc(tgt, init, num_samples=S6, num_steps_per_sample=L5, step_size=float(EPS3[c]),
+                                 burn=1, inv_mass=im, normals=z, log_uniforms=logu))
+        inits.append(init), zs.append(z), lus.append(logu)
+    acc = torch.tensor([o['accepted'] for o in outs])
+    samples = torch.stack([torch.stack(o['samples']) for o in outs])
+    ham = torch.tensor([[o['ham_old'], o['ham_new']] for o in outs], dtype=torch.float64).transpose(1, 2)
+    return torch.stack(inits), acc, samples, torch.stack(zs, 1), torch.stack(lus, 1), ham
+
+
+def _up_one_ulp(x):
+    return torch.nextafter(x, torch.full_like(x, float('inf')))
+
+
+@pytest.mark.parametrize('fault', [None, 'inv_var', 'mass_factor'])
+def test_elementwise_row_replay_is_bit_exact(fault, monkeypatch):
+    """replay + check + replay_rows32 accept the oracle's GaussianDiag chains with a diagonal mass; one inv_var element
+    one ulp off, or the mass factor of columns 64..127 one ulp off, makes some accepted row differ bit-wise."""
+    tgt, im = _elem_problem()
+    run_tgt = tgt
+    if fault == 'inv_var':
+        run_tgt = copy.copy(tgt)
+        run_tgt.inv_var = tgt.inv_var.clone()
+        run_tgt.inv_var[100] = _up_one_ulp(tgt.inv_var[100])
+    elif fault == 'mass_factor':
+        factor = (1 / im) ** 0.5
+        factor[64:128] = _up_one_ulp(factor[64:128])
+        monkeypatch.setattr(O, 'momentum_from_normals', lambda z, mass, scale_tril=None: z * factor)
+    init, acc, samples, z, logu, ham = _elem_oracle(run_tgt, im)
+    assert 0 < int(acc[:, 2:].sum()) < acc[:, 2:].numel()
+    flips = _run(dense_ref.HMC(tgt, im), init, acc, samples, z, logu, ham, EPS3, L5, 1, 'cpu_replay/elem250',
+                 ORACLE_BOUND)
+    assert flips == 0
+    rows = lambda: dense_ref.replay_rows32('cpu_replay/elem250', tgt, im, init, acc, samples, z, EPS3, L5, 1)
+    if fault:
+        with pytest.raises(AssertionError, match='bit-wise'):
+            rows()
+    else:
+        assert rows() == int(acc[:, 2:].sum())

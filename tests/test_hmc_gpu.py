@@ -10,7 +10,7 @@ import torch
 import hamiltorch_b200 as hb
 from hamiltorch_b200 import engine, targets as T
 from oracle import cases, hmc_oracle as O
-from tests import parity
+from tests import dense_ref, parity
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden')
@@ -150,6 +150,19 @@ def test_hamiltonian_vs_oracle_and_nonfinite_flag():
         for c in range(C):
             ref = float(O.hamiltonian_hmc(tgt, q[c], p[c], mass))
             assert abs(float(H[c]) - ref) <= 50 * parity.H_TOL_REL * (abs(ref) + 1)
+    # against fp64 at the widths where hamiltonian_kernel's block (ld / 4 threads, rounded up to a warp, at most 256)
+    # changes: one warp at D = 1 and 3, 256 threads with one float4 each at D = 1000, several per thread at 4099, 9001
+    for Dw in (1, 3, 1000, 4099, 9001):
+        g = torch.Generator().manual_seed(Dw)
+        for tgt_w in (T.GaussianIso(Dw), T.GaussianDiag(torch.randn(Dw, generator=g), 0.3 + torch.rand(Dw, generator=g))):
+            qw, pw = torch.randn(C, Dw, generator=g), torch.randn(C, Dw, generator=g)
+            for mass in (None, 0.5 + torch.rand(Dw, generator=g)):
+                H, flags = engine.hamiltonian(tgt_w, qw, pw, inv_mass=mass)
+                assert int(flags.sum()) == 0
+                want = dense_ref.HMC(tgt_w, mass).hamiltonian(qw.double(), pw.double())
+                parity.assert_close('elem_ref/hamiltonian_%s_%s_d%d' % (type(tgt_w).__name__, 'none' if mass is None
+                                                                        else 'diag', Dw),
+                                    H.double().cpu().numpy(), want.numpy(), 2e-4)
     h1 = hb.hamiltonian(q[0], p[0], tgt)
     assert h1.dim() == 0
     q[2, 5] = float('inf')

@@ -9,12 +9,11 @@ the injected-stream twin.
 elem_hmc_run takes the producer form for at most 2 chains per SM and the plain paired form (PW = 0) above that, so the
 chain counts derive from the device's SM count (256 / 255 on a 132-SM H100), and the plain paired form is pinned the
 same way at 2 x SM count + 1 chains."""
-import time
-
 import pytest
 import torch
 
 from hamiltorch_b200 import engine, targets as T, _native as N
+from tests.launched import ran as _ran
 from tests.test_philox_stream_gpu import OFFSETS, SEEDS, _elem, _init, _philox_vs_injected
 
 pytestmark = pytest.mark.gpu
@@ -34,25 +33,6 @@ def _sms():
 def _producer_chains():
     """the largest chain count (at most 256) that runs the producer form"""
     return min(256, 2 * _sms())
-
-
-def _ran(kernel, fn, attempts=3):
-    """fn() under the profiler; asserts that it launched hmc_run_kernel<...kernel>.  Late in a long GPU session the
-    profiler has come back with no hmc_run_kernel record at all for a run that did launch one (it keeps only the device
-    records it can place inside its host-side window).  So the window is padded on both sides, and a trace holding no
-    hmc_run_kernel record is taken again (fn is deterministic); a trace that records another form fails at once."""
-    for _ in range(attempts):
-        torch.cuda.synchronize()
-        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA], acc_events=True) as prof:
-            time.sleep(0.05)
-            res = fn()
-            torch.cuda.synchronize()
-            time.sleep(0.05)
-        names = sorted({e.name for e in prof.events() if 'hmc_run_kernel<' in e.name})
-        if names:
-            break
-    assert any(kernel in n for n in names), ('expected hmc_run_kernel<...%s' % kernel, names)
-    return res
 
 
 def _run_both(tgt, init, S, L, eps, kernel=PRODUCER_KERNEL, **kw):
