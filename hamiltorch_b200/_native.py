@@ -218,12 +218,23 @@ _PROTOS = {
                                           C.c_int32, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int32,
                                           C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                           C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    'hmcx_mlp_log_prior': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
+                                     C.POINTER(C.c_int32), C.POINTER(C.c_double), C.c_void_p, C.c_void_p]),
+    'hmcx_psens_ll_totals': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                       C.c_void_p, C.c_void_p, C.c_void_p]),
+    'hmcx_psens_workspace_bytes': (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
+    'hmcx_psens_weights': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_double,
+                                     C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                     C.c_void_p]),
+    'hmcx_psens_pass': (C.c_int, [C.c_void_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                  C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
 }
 
 DIAG_LAG_BLOCK = 32                     # HMCX_DIAG_LAG_BLOCK: lags per hmcx_diag_acov pass
 RANK_MAX_DRAWS = 2147418112             # HMCX_RANK_MAX_DRAWS: largest C*n hmcx_rank_pass takes
 RANK_MAX_SLAB = 65535                   # HMCX_RANK_MAX_SLAB: most dimensions per hmcx_rank_pass
 LOO_CHAIN_MAX_DRAWS = 8192              # HMCX_LOO_CHAIN_MAX_DRAWS: most draws per chain hmcx_loo_chain_pass sorts
+PSENS_SETS, PSENS_ROWS = 4, 14          # HMCX_PSENS_SETS / HMCX_PSENS_ROWS: weight sets and output rows of hmcx_psens_pass
 
 EXPORTED_SYMBOLS = tuple(_PROTOS)
 

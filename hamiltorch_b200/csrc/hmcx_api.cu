@@ -80,6 +80,13 @@ int loo_chain_pass(const float*, long long, long long, int, int, int, int, int, 
 size_t stack_workspace_bytes(int, int);
 int stack_eval(const double*, int, int, const double*, double*, double*, double*, void*, cudaStream_t);
 int stack_em(const double*, int, int, double, int, double*, double*, double*, double*, int*, void*, cudaStream_t);
+int mlp_log_prior(const float*, long long, long long, int, int, int, const int*, const double*, double*, cudaStream_t);
+int psens_ll_totals(const float*, long long, long long, int, int, int, int, const double*, double*, cudaStream_t);
+size_t psens_workspace_bytes(int, int, int);
+int psens_weights(const float*, long long, long long, int, int, int, double, double*, double*, int*, int*, void*,
+                  cudaStream_t);
+int psens_pass(const float*, long long, long long, int, int, int, int, int, const double*, double*, int*, void*,
+               cudaStream_t);
 }  // namespace hmcx
 
 static inline bool has_mu_chain(const hmcx_nuts_t* nuts) { return nuts && nuts->enabled && nuts->mu_chain; }
@@ -631,6 +638,56 @@ int hmcx_stack_em(const double* E, int32_t K, int32_t N, double tol, int32_t ite
         return HMCX_ERR_INVALID_ARG;
     return hmcx::stack_em(E, K, N, tol, iterations, w, objective, grad, pointwise, state, workspace,
                           (cudaStream_t)stream);
+}
+
+int hmcx_mlp_log_prior(const float* samples, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n,
+                       int32_t num_tensors, const int32_t* sizes, const double* tau, double* out, void* stream) {
+    if (!samples || !sizes || !tau || !out || chain_stride < 0 || draw_stride < 0 || C < 1 || n < 1 ||
+        (int64_t)C * n > 0x7fffffffLL || num_tensors < 1 || num_tensors > 2 * HMCX_MLP_MAX_LAYERS)
+        return HMCX_ERR_INVALID_ARG;
+    int64_t total = 0;
+    for (int t = 0; t < num_tensors; ++t) {
+        if (sizes[t] < 1 || !(tau[t] >= 0.0) || !(tau[t] <= DBL_MAX)) return HMCX_ERR_INVALID_ARG;
+        total += sizes[t];
+    }
+    if (total > 0x7fffffffLL) return HMCX_ERR_INVALID_ARG;
+    return hmcx::mlp_log_prior(samples, chain_stride, draw_stride, C, n, num_tensors, sizes, tau, out,
+                               (cudaStream_t)stream);
+}
+
+int hmcx_psens_ll_totals(const float* ll, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t r0,
+                         int32_t k, const double* coef, double* totals, void* stream) {
+    if (!ll || !totals || chain_stride < 0 || draw_stride < 0 || !loo_shape_ok(C, n) || r0 < 0 || r0 % 128 || k < 1 ||
+        (int64_t)r0 + k > 0x7fffffffLL)
+        return HMCX_ERR_INVALID_ARG;
+    return hmcx::psens_ll_totals(ll, chain_stride, draw_stride, C, n, r0, k, coef, totals, (cudaStream_t)stream);
+}
+
+size_t hmcx_psens_workspace_bytes(int32_t C, int32_t n, int32_t k) {
+    if (!loo_shape_ok(C, n) || !rank_slab_ok(k)) return 0;
+    return hmcx::psens_workspace_bytes(C, n, k);
+}
+
+int hmcx_psens_weights(const float* neg_log_ratio, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n,
+                       int32_t K, double r_eff, double* weights, double* pareto_k, int32_t* tail_size,
+                       int32_t* nonfinite, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!neg_log_ratio || !weights || !pareto_k || !tail_size || !nonfinite || !workspace || chain_stride < 0 ||
+        draw_stride < 0 || !loo_shape_ok(C, n) || !rank_slab_ok(K) || !(r_eff > 0.0) || !(r_eff <= DBL_MAX) ||
+        workspace_bytes < hmcx::psens_workspace_bytes(C, n, K))
+        return HMCX_ERR_INVALID_ARG;
+    return hmcx::psens_weights(neg_log_ratio, chain_stride, draw_stride, C, n, K, r_eff, weights, pareto_k, tail_size,
+                               nonfinite, workspace, (cudaStream_t)stream);
+}
+
+int hmcx_psens_pass(const float* x, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t D,
+                    int32_t d0, int32_t k, const double* weights, double* out, int32_t* nonfinite, void* workspace,
+                    size_t workspace_bytes, void* stream) {
+    if (!x || !weights || !out || !nonfinite || !workspace || chain_stride < 0 || draw_stride < 0 ||
+        !loo_shape_ok(C, n) || D < 1 || d0 < 0 || !rank_slab_ok(k) || (int64_t)d0 + k > D ||
+        workspace_bytes < hmcx::psens_workspace_bytes(C, n, k))
+        return HMCX_ERR_INVALID_ARG;
+    return hmcx::psens_pass(x, chain_stride, draw_stride, C, n, D, d0, k, weights, out, nonfinite, workspace,
+                            (cudaStream_t)stream);
 }
 
 }  // extern "C"

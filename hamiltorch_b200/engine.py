@@ -515,8 +515,8 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
     the parameter tensors in tau_list order, then tau_out -- each None (fixed) or (a, b) (shape, rate), Gibbs-updated
     inside the kernel after every MH step (include/hmcx.h hmcx_hyper_t, DESIGN §3.15).  Injected mode takes ``gammas``
     (S, C, 2L + 1) fp64 standard-gamma draws.  The result gains ``tau_list_trace`` (C, keep, 2L), ``tau_out_trace``
-    (C, keep) -- on the device whatever ``host_samples`` says -- and the final state ``tau_list_final`` (C, 2L),
-    ``tau_out_final`` (C,).
+    (C, keep) -- on the device whatever ``host_samples`` says -- the final state ``tau_list_final`` (C, 2L),
+    ``tau_out_final`` (C,), and ``hyper`` (the list as given, which ``sensitivity.log_components`` reads).
     ``temper`` (Bayesian-NN targets with a ``scheme``): replica exchange, a dict with ``betas`` (T Python floats, 1.0 first,
     strictly decreasing), ``swap_every`` and ``swap_log_uniforms`` ((rounds, R, T - 1) fp64 or None: Philox).  The C = R T
     rows are R ladders, row r T + t at beta_t (include/hmcx.h hmcx_temper_t, DESIGN §3.17): the run goes in windows of
@@ -772,6 +772,7 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
     if hyper_s is not None:
         res.tau_list_trace, res.tau_out_trace = tau_trace, tau_out_trace
         res.tau_list_final, res.tau_out_final = tau, tau_out
+        res.hyper = list(hyper)
     if folds is not None:
         res.folds, res.num_folds = folds, num_folds
     if temper_out is not None:

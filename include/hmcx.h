@@ -852,6 +852,48 @@ int hmcx_pred_pass_weighted(const float* f, int64_t chain_stride, int64_t draw_s
                             double* per_output, int32_t* nonfinite, double* partials, void* workspace,
                             size_t workspace_bytes, const double* chain_weights, void* stream);
 
+/*
+ * Power-scaling prior and likelihood sensitivity (additive v12 symbols; DESIGN §3.22, hamiltorch_b200/sensitivity.py).
+ * Callers of an older v12 library check for the symbols.  Draws are pooled as g = c n + s, S = C n.
+ *   hmcx_mlp_log_prior  out [S] fp64 (device) = sum over the parameter tensors t with tau[t] > 0 of the Normal(0,
+ *                    tau_t^-1/2) log density of the tensor's entries, -tau_t / 2 sum_i w_i^2 + n_t / 2 (log tau_t - log
+ *                    2 pi), in fp64.  The tensors are consecutive in the draw, sizes [num_tensors] and tau [num_tensors]
+ *                    are host arrays (tau 0: the tensor is left out).  One CTA per draw reads the draw once; the sums
+ *                    are in a fixed order.  NULL pointers, a bad shape, num_tensors not in [1, 2 HMCX_MLP_MAX_LAYERS],
+ *                    a size < 1 or a tau that is negative or not finite: HMCX_ERR_INVALID_ARG.
+ *   hmcx_psens_ll_totals  totals [S] fp64 (device) += sum_i coef[r0 + i] ll[c, s, i] over the slab's rows i in [0, k)
+ *                    (ll[c, s, i] at ll + c chain_stride + s draw_stride + i; coef NULL: 1), in 128-row groups in row
+ *                    order, each group a fixed-order sum.  With r0 a multiple of 128 and totals zeroed before the first
+ *                    slab, the totals are the same bits for every split of the rows into slabs.  r0 not a multiple of
+ *                    128 or the checks below: HMCX_ERR_INVALID_ARG.
+ *   hmcx_psens_workspace_bytes  workspace of hmcx_psens_weights (k = K) and hmcx_psens_pass for a slab of k columns.
+ *   hmcx_psens_weights  the Pareto-smoothed importance weights of K log-ratio columns: neg_log_ratio [C, n, K] fp32 holds
+ *                    -r (unit stride along K), each column smoothed as hmcx_loo_pass smooths a point's ll (M =
+ *                    ceil(min(0.2 S, 3 sqrt(S / r_eff)))).  weights [K, S] fp64 the normalised weights in flat-draw
+ *                    order, pareto_k [K], tail_size [K] (M'), nonfinite [K] (1: a non-finite -r, NaN weights and k-hat).
+ *   hmcx_psens_pass  for the columns [d0, d0 + k) of x (the strides of hmcx_rank_pass, D columns) and the weights
+ *                    [HMCX_PSENS_SETS, S] of hmcx_psens_weights: out [HMCX_PSENS_ROWS, D] fp64, rows 0..3 the cumulative
+ *                    Jensen-Shannon distance max(cjs+, cjs-) of each weight set against equal weights, 4 the mean, 5..8
+ *                    the weighted means, 9 the sd, 10..13 the weighted sds; nonfinite [D] (1: a non-finite draw, NaN in
+ *                    every row).  Fixed-order sums, no atomics: the outputs depend on the inputs alone.
+ *   For the three workspace users: NULL pointers, negative strides, C n < 2 or > HMCX_RANK_MAX_DRAWS, n < 1, a slab
+ *   outside [0, D), k (or K) not in [1, HMCX_RANK_MAX_SLAB], r_eff not in (0, inf) or a workspace smaller than
+ *   hmcx_psens_workspace_bytes: HMCX_ERR_INVALID_ARG.
+ */
+#define HMCX_PSENS_SETS 4
+#define HMCX_PSENS_ROWS 14
+int hmcx_mlp_log_prior(const float* samples, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n,
+                       int32_t num_tensors, const int32_t* sizes, const double* tau, double* out, void* stream);
+int hmcx_psens_ll_totals(const float* ll, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t r0,
+                         int32_t k, const double* coef, double* totals, void* stream);
+size_t hmcx_psens_workspace_bytes(int32_t C, int32_t n, int32_t k);
+int hmcx_psens_weights(const float* neg_log_ratio, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n,
+                       int32_t K, double r_eff, double* weights, double* pareto_k, int32_t* tail_size,
+                       int32_t* nonfinite, void* workspace, size_t workspace_bytes, void* stream);
+int hmcx_psens_pass(const float* x, int64_t chain_stride, int64_t draw_stride, int32_t C, int32_t n, int32_t D,
+                    int32_t d0, int32_t k, const double* weights, double* out, int32_t* nonfinite, void* workspace,
+                    size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif
