@@ -482,6 +482,86 @@ class HMCResult:
         return 1.0 - self.num_rejected.double() / self.num_samples
 
 
+def _run_device(params_init, device):
+    """The device of an hmc_run / rmhmc_run call: ``device``, else params_init's CUDA device, else the current one.
+    Refuses first when there is no CUDA device or no native library."""
+    N.require_cuda()
+    N.load_library()
+    if device is None:
+        device = params_init.device if params_init.is_cuda else torch.device('cuda', torch.cuda.current_device())
+    return torch.device(device)
+
+
+class _Run:
+    """What one hmc_run / rmhmc_run call builds once and each of its launches reads: the device and its current stream,
+    the native target, the (C, ld) rows of the initial and current state, the per-chain step sizes, the per-iteration
+    outputs and ``keep_alive``, everything an asynchronous launch may still read when the call returns.  The caller then
+    sets the sample block and the random-stream struct; hmc_run also the NUTS struct and its dual-averaging state, the
+    integrator ``scheme``, ``tuning``, the element-wise workspace ``ws`` and ``num_folds``."""
+
+    def __init__(self, nt, params_init, num_samples, num_steps_per_sample, step_size, burn, record_ham, device):
+        self.lib = N.load_library()
+        self.device, self.stream = device, N.stream_ptr(device)
+        self.nt, self.D, self.ld = nt, nt.dim, N.padded_ld(nt.dim)
+        self.S, self.L, self.burn = int(num_samples), int(num_steps_per_sample), int(burn)
+        self.q_init = _as_rows(params_init, self.ld, device)
+        self.Cn = Cn = self.q_init.shape[0]
+        self.q_cur = self.q_init.clone()
+        self.eps = _eps_vector(step_size, Cn, device)
+        self.accepted = torch.empty((Cn, self.S), dtype=torch.uint8, device=device)
+        self.diverged = torch.empty((Cn, self.S), dtype=torch.uint8, device=device)
+        self.ham = torch.empty((Cn, self.S, 2), dtype=torch.float32, device=device) if record_ham else None
+        self.num_rejected = torch.zeros(Cn, dtype=torch.int32, device=device)
+        self.samples = self.rng = self.nuts = self.h_bar = self.eps_bar = self.scheme = self.ws = None
+        self.tuning = self.num_folds = 0
+        self.keep_alive = []
+
+    def args(self, it0, it1):
+        """The arguments every run entry takes from q_init to num_rejected, for iterations [it0, it1)."""
+        return (N.ptr(self.q_init), N.ptr(self.q_cur), N.ptr(self.eps), self.Cn, self.ld, self.L, self.S, self.burn, it0,
+                it1, N.ptr(self.samples), N.ptr(self.accepted), N.ptr(self.diverged), N.ptr(self.ham),
+                N.ptr(self.num_rejected))
+
+
+def _rng_struct(run, seed, chain_offset, normals, log_uniforms, perms=None, uniforms=None, jitter=False):
+    """The random-stream struct of a run: Philox keyed by (seed, chain_offset + c, iteration), or -- when ``normals``
+    (S, C, D) is given -- the injected stream: ``log_uniforms`` (S, C), SPLITTING_RAND's ``perms`` (S, C, M) if given and,
+    for RMHMC with ``jitter``, the metric-jitter ``uniforms`` (S, C, J, D).  The device copies join run.keep_alive."""
+    rng = N.RngStruct()
+    if normals is None:
+        rng.mode, rng.seed, rng.chain_offset = N.RNG_PHILOX, int(seed), int(chain_offset)
+        return rng
+    S, Cn, D, ld, device = run.S, run.Cn, run.D, run.ld, run.device
+    z = normals.detach().to(device=device, dtype=torch.float32)
+    if z.dim() == 2:
+        z = z.unsqueeze(1)
+    if tuple(z.shape) != (S, Cn, D):
+        raise RuntimeError('normals must be (S, C, D) = (%d, %d, %d), got %s' % (S, Cn, D, tuple(z.shape)))
+    z = N.pad_rows(z.contiguous(), ld)
+    lu = log_uniforms.detach().to(device=device, dtype=torch.float32).reshape(S, Cn).contiguous()
+    rng.mode, rng.normals, rng.log_uniforms = N.RNG_INJECTED, z.data_ptr(), lu.data_ptr()
+    run.keep_alive += [z, lu]
+    if perms is not None:
+        if perms.dim() != 3 or tuple(perms.shape[:2]) != (S, Cn) or perms.shape[2] != run.nt.num_splits:
+            raise RuntimeError('perms must be (S, C, M) = (%d, %d, %d), got %s'
+                               % (S, Cn, run.nt.num_splits, tuple(perms.shape)))
+        pm = perms.detach().to(device=device, dtype=torch.int32).contiguous()
+        rng.perms = pm.data_ptr()
+        run.keep_alive.append(pm)
+    if jitter:
+        if uniforms is None:
+            raise RuntimeError('injected RMHMC with jitter needs the uniforms stream')
+        u = uniforms.detach().to(device=device, dtype=torch.float32)
+        if u.dim() == 3:
+            u = u.unsqueeze(1)
+        if u.dim() != 4 or tuple(u.shape[:2]) != (S, Cn) or u.shape[3] != D:
+            raise RuntimeError('uniforms must be (S, C, J, D) = (%d, %d, J, %d), got %s' % (S, Cn, D, tuple(u.shape)))
+        u = N.pad_rows(u.contiguous(), ld)
+        rng.uniforms, rng.uniforms_per_iter = u.data_ptr(), u.shape[2]
+        run.keep_alive.append(u)
+    return rng
+
+
 def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, burn=0, inv_mass=None,
             nuts=False, desired_accept_rate=0.8, seed=0, chain_offset=0, normals=None, log_uniforms=None,
             record_ham=False, out=None, device=None, tuning=0, eps_schedule=None, record_eps=False, scheme=None,
@@ -531,11 +611,7 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
     prior and settings -- the fold path with the training sets given directly (sbc.fit passes K copies of one target, each
     holding its own simulated y).  Chain g = chain_offset + c samples fits[g mod K].
     """
-    N.require_cuda()
-    lib = N.load_library()
-    if device is None:
-        device = params_init.device if params_init.is_cuda else torch.device('cuda', torch.cuda.current_device())
-    device = torch.device(device)
+    device = _run_device(params_init, device)
     num_folds = 0
     if folds is not None or fits is not None:
         if scheme != N.SCHEME_PLAIN or temper is not None or hyper is not None or adapt_mass:
@@ -547,15 +623,11 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
         target = fits
         num_folds = len(fits)
     nt = native_target(target, device)
-    D, ld = nt.dim, N.padded_ld(nt.dim)
-    nm = native_mass(inv_mass, D, device)
-    S, L, burn = int(num_samples), int(num_steps_per_sample), int(burn)
-    q_init = _as_rows(params_init, ld, device)
-    if q_init.shape[1] != ld or params_init.shape[-1] != D:
+    nm = native_mass(inv_mass, nt.dim, device)
+    run = _Run(nt, params_init, num_samples, num_steps_per_sample, step_size, burn, record_ham, device)
+    D, ld, Cn, S, burn = run.D, run.ld, run.Cn, run.S, run.burn
+    if run.q_init.shape[1] != ld or params_init.shape[-1] != D:
         raise RuntimeError('params_init last dimension must be %d' % D)
-    Cn = q_init.shape[0]
-    q_cur = q_init.clone()
-    eps = _eps_vector(step_size, Cn, device)
     thin = int(thin)
     if thin < 1:
         raise RuntimeError('thin must be >= 1')
@@ -596,51 +668,26 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
         samples = out
         if tuple(samples.shape) != (Cs, keep, ld) or samples.dtype != torch.float32 or not samples.is_contiguous():
             raise RuntimeError('out must be a contiguous fp32 (%s, S-burn, ld) tensor' % ('C' if temper is None else 'R'))
-    accepted = torch.empty((Cn, S), dtype=torch.uint8, device=device)
-    diverged = torch.empty((Cn, S), dtype=torch.uint8, device=device)
-    ham = torch.empty((Cn, S, 2), dtype=torch.float32, device=device) if record_ham else None
-    num_rejected = torch.zeros(Cn, dtype=torch.int32, device=device)
+    run.samples = samples
+    run.rng = _rng_struct(run, seed, chain_offset, normals, log_uniforms, perms=perms)
 
-    rng = N.RngStruct()
-    keep_alive = []
-    if normals is not None:
-        z = normals.detach().to(device=device, dtype=torch.float32)
-        if z.dim() == 2:
-            z = z.unsqueeze(1)
-        if tuple(z.shape[:2]) != (S, Cn) or z.shape[2] != D:
-            raise RuntimeError('normals must be (S, C, D)')
-        z = N.pad_rows(z.contiguous(), ld)
-        lu = log_uniforms.detach().to(device=device, dtype=torch.float32).reshape(S, Cn).contiguous()
-        rng.mode = N.RNG_INJECTED
-        rng.normals, rng.log_uniforms = z.data_ptr(), lu.data_ptr()
-        keep_alive += [z, lu]
-        if perms is not None:
-            if perms.dim() != 3 or tuple(perms.shape[:2]) != (S, Cn) or perms.shape[2] != nt.num_splits:
-                raise RuntimeError('perms must be (S, C, M) = (%d, %d, %d), got %s'
-                                   % (S, Cn, nt.num_splits, tuple(perms.shape)))
-            pm = perms.detach().to(device=device, dtype=torch.int32).contiguous()
-            rng.perms = pm.data_ptr()
-            keep_alive.append(pm)
-    else:
-        rng.mode, rng.seed, rng.chain_offset = N.RNG_PHILOX, int(seed), int(chain_offset)
-
-    nuts_s = N.NutsStruct()
+    nuts_s = run.nuts = N.NutsStruct()
     eps_trace = None
     if not torch.is_tensor(step_size):
         nuts_s.step_size_init = float(step_size)           # the double the reference divides in its split drifts
     if nuts:
         table = nuts_table_restarted_device(burn, device) if adapt_mass else nuts_table_device(burn, device)
-        h_bar = torch.zeros(Cn, dtype=torch.float64, device=device)
-        eps_bar = torch.ones(Cn, dtype=torch.float64, device=device)
+        run.h_bar = torch.zeros(Cn, dtype=torch.float64, device=device)
+        run.eps_bar = torch.ones(Cn, dtype=torch.float64, device=device)
         nuts_s.enabled = 1
         nuts_s.desired_accept_rate = float(desired_accept_rate)
         nuts_s.mu = nuts_mu(step_size if not torch.is_tensor(step_size) else float(step_size.reshape(-1)[0]))
-        nuts_s.table, nuts_s.h_bar, nuts_s.eps_bar = table.data_ptr(), h_bar.data_ptr(), eps_bar.data_ptr()
-        keep_alive += [table, h_bar, eps_bar]
+        nuts_s.table, nuts_s.h_bar, nuts_s.eps_bar = table.data_ptr(), run.h_bar.data_ptr(), run.eps_bar.data_ptr()
+        run.keep_alive += [table, run.h_bar, run.eps_bar]
         if eps_schedule is not None:
             sched = eps_schedule.detach().to(device=device, dtype=torch.float32).reshape(S, Cn).contiguous()
             nuts_s.eps_schedule = sched.data_ptr()
-            keep_alive.append(sched)
+            run.keep_alive.append(sched)
         if record_eps:
             eps_trace = torch.zeros((Cn, S), dtype=torch.float32, device=device)
             nuts_s.eps_trace = eps_trace.data_ptr()
@@ -673,99 +720,64 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
         tau_out_trace = torch.zeros((Cn, keep), dtype=torch.float32, device=device)
         hyper_s.tau, hyper_s.tau_out = tau.data_ptr(), tau_out.data_ptr()
         hyper_s.tau_trace, hyper_s.tau_out_trace = tau_trace.data_ptr(), tau_out_trace.data_ptr()
-        keep_alive += [tau, tau_out, tau_trace, tau_out_trace]
-        if rng.mode == N.RNG_INJECTED:
+        run.keep_alive += [tau, tau_out, tau_trace, tau_out_trace]
+        if run.rng.mode == N.RNG_INJECTED:
             if gammas is None or tuple(gammas.shape) != (S, Cn, K + 1):
                 raise RuntimeError('injected hyperpriors need gammas (S, C, 2L + 1) = (%d, %d, %d)' % (S, Cn, K + 1))
             gm = gammas.detach().to(device=device, dtype=torch.float64).contiguous()
             hyper_s.gammas = gm.data_ptr()
-            keep_alive.append(gm)
+            run.keep_alive.append(gm)
+    run.scheme, run.tuning, run.num_folds = scheme, int(tuning), num_folds
     mass_out = None
     temper_out = None
     with torch.cuda.device(device):
+        if scheme is None:
+            ws_bytes = run.lib.hmcx_hmc_workspace_bytes(nt.ref(), nm.ref(), Cn, ld)
+            run.ws = torch.empty(ws_bytes // 4, dtype=torch.float32, device=device) if ws_bytes else None
         if temper is not None:
-            temper_out = _tempered_launches(lib, nt, nm, rng, nuts_s, scheme, q_init, q_cur, eps, Cn, ld, L, S, burn,
-                                            samples, accepted, diverged, ham, num_rejected, sink, temper, device,
-                                            keep_alive)
+            temper_out = _tempered_launches(run, nm, sink, temper)
         elif adapt_mass:
             if sink is None:
                 sink = N.SinkStruct()
                 sink.thin = 1
-            mass_out = _adapted_launches(lib, nt, nm, rng, nuts_s, scheme, q_init, q_cur, eps, Cn, D, ld, L, S, burn,
-                                         samples, accepted, diverged, ham, num_rejected, int(tuning), sink, h_bar,
-                                         eps_bar, mass_pool, device, keep_alive, hyper_s)
-        elif num_folds:
-            rc = lib.hmcx_split_run_folds(nt.ref(), nm.ref(), C.byref(rng), C.byref(nuts_s), int(scheme), N.ptr(q_init),
-                                          N.ptr(q_cur), N.ptr(eps), Cn, ld, L, S, burn, 0, S, N.ptr(samples),
-                                          N.ptr(accepted), N.ptr(diverged), N.ptr(ham), N.ptr(num_rejected),
-                                          None if sink is None else C.byref(sink), num_folds, N.stream_ptr(device))
-            N.check(rc, 'hmcx_split_run_folds')
-        elif scheme is None:
-            ws_bytes = lib.hmcx_hmc_workspace_bytes(nt.ref(), nm.ref(), Cn, ld)
-            ws = torch.empty(ws_bytes // 4, dtype=torch.float32, device=device) if ws_bytes else None
-            if use_sink:
-                rc = lib.hmcx_hmc_run_sink(nt.ref(), nm.ref(), C.byref(rng), C.byref(nuts_s), N.ptr(q_init),
-                                           N.ptr(q_cur), N.ptr(eps), Cn, ld, L, S, burn, 0, S, N.ptr(samples),
-                                           N.ptr(accepted), N.ptr(diverged), N.ptr(ham), N.ptr(num_rejected),
-                                           int(tuning), N.ptr(ws), C.byref(sink), N.stream_ptr(device))
-                N.check(rc, 'hmcx_hmc_run_sink')
-            elif host_out is not None:
-                if tuple(host_out.shape) != (Cn, keep, ld) or host_out.dtype != torch.float32 or not host_out.is_contiguous():
-                    raise RuntimeError('out must be a contiguous fp32 (C, S-burn, ld) tensor')
-                W = min(int(host_windows), S)
-                main = torch.cuda.current_stream(device)
-                side = _side_stream(device)
-                pitch, slot_bytes = keep * ld * 4, ld * 4
-                for w in range(W):
-                    a, b = (S * w) // W, (S * (w + 1)) // W
-                    rc = lib.hmcx_hmc_run(nt.ref(), nm.ref(), C.byref(rng), C.byref(nuts_s), N.ptr(q_init), N.ptr(q_cur),
-                                          N.ptr(eps), Cn, ld, L, S, burn, a, b, N.ptr(samples), N.ptr(accepted),
-                                          N.ptr(diverged), N.ptr(ham), N.ptr(num_rejected), int(tuning), N.ptr(ws),
-                                          C.c_void_p(main.cuda_stream))
-                    N.check(rc, 'hmcx_hmc_run')
-                    lo = 0 if a == 0 else max(a - burn, 1)               # slots this window wrote: 0 = params_init (:959),
-                    hi = max(b - burn, 1 if a == 0 else lo)              # n - burn for every iteration n > burn
-                    if hi > lo:
-                        ev = torch.cuda.Event()
-                        ev.record(main)
-                        side.wait_event(ev)
-                        rc = lib.hmcx_copy_rows_async(C.c_void_p(host_out.data_ptr() + lo * slot_bytes), pitch,
+            mass_out = _adapted_launches(run, nm, sink, hyper_s, mass_pool)
+        elif host_out is not None and sink is None:
+            if tuple(host_out.shape) != (Cn, keep, ld) or host_out.dtype != torch.float32 or not host_out.is_contiguous():
+                raise RuntimeError('out must be a contiguous fp32 (C, S-burn, ld) tensor')
+            W = min(int(host_windows), S)
+            main = torch.cuda.current_stream(device)
+            side = _side_stream(device)
+            pitch, slot_bytes = keep * ld * 4, ld * 4
+            for w in range(W):
+                a, b = (S * w) // W, (S * (w + 1)) // W
+                _launch(run, a, b, nm.ref(), None)
+                lo = 0 if a == 0 else max(a - burn, 1)               # slots this window wrote: 0 = params_init (:959),
+                hi = max(b - burn, 1 if a == 0 else lo)              # n - burn for every iteration n > burn
+                if hi > lo:
+                    ev = torch.cuda.Event()
+                    ev.record(main)
+                    side.wait_event(ev)
+                    rc = run.lib.hmcx_copy_rows_async(C.c_void_p(host_out.data_ptr() + lo * slot_bytes), pitch,
                                                       C.c_void_p(samples.data_ptr() + lo * slot_bytes), pitch,
                                                       (hi - lo) * slot_bytes, Cn, C.c_void_p(side.cuda_stream))
-                        N.check(rc, 'hmcx_copy_rows_async')
-                done = torch.cuda.Event()
-                done.record(side)
-                main.wait_event(done)                       # the caller's stream sees the delivered block
-                keep_alive.append(samples)
-                samples = host_out
-            else:
-                rc = lib.hmcx_hmc_run(nt.ref(), nm.ref(), C.byref(rng), C.byref(nuts_s), N.ptr(q_init), N.ptr(q_cur),
-                                      N.ptr(eps), Cn, ld, L, S, burn, 0, S, N.ptr(samples), N.ptr(accepted),
-                                      N.ptr(diverged), N.ptr(ham), N.ptr(num_rejected), int(tuning), N.ptr(ws),
-                                      N.stream_ptr(device))
-                N.check(rc, 'hmcx_hmc_run')
-        elif hyper_s is not None:
-            rc = lib.hmcx_split_run_hyper(nt.ref(), nm.ref(), C.byref(rng), C.byref(nuts_s), int(scheme), N.ptr(q_init),
-                                          N.ptr(q_cur), N.ptr(eps), Cn, ld, L, S, burn, 0, S, N.ptr(samples),
-                                          N.ptr(accepted), N.ptr(diverged), N.ptr(ham), N.ptr(num_rejected),
-                                          None if sink is None else C.byref(sink), C.byref(hyper_s), N.stream_ptr(device))
-            N.check(rc, 'hmcx_split_run_hyper')
+                    N.check(rc, 'hmcx_copy_rows_async')
+            done = torch.cuda.Event()
+            done.record(side)
+            main.wait_event(done)                       # the caller's stream sees the delivered block
+            run.keep_alive.append(samples)
+            samples = host_out
         else:
-            rc = lib.hmcx_split_run_sink(nt.ref(), nm.ref(), C.byref(rng), C.byref(nuts_s), int(scheme), N.ptr(q_init),
-                                         N.ptr(q_cur), N.ptr(eps), Cn, ld, L, S, burn, 0, S, N.ptr(samples),
-                                         N.ptr(accepted), N.ptr(diverged), N.ptr(ham), N.ptr(num_rejected),
-                                         None if sink is None else C.byref(sink), N.stream_ptr(device))
-            N.check(rc, 'hmcx_split_run_sink')
-    res = HMCResult(samples, accepted, diverged, ham, eps, num_rejected, D, S)
+            _launch(run, 0, S, nm.ref(), sink, hyper_s)
+    res = HMCResult(samples, run.accepted, run.diverged, run.ham, run.eps, run.num_rejected, D, S)
     res.eps_trace = eps_trace
     res.thin = thin
     # compensated running sums: hi + lo combined in fp64 (relative error ~2^-46 whatever the run length)
     res.moment_sum = None if msum is None else (msum.double() + msum_lo.double())[:, :D]
     res.moment_sumsq = None if msq is None else (msq.double() + msq_lo.double())[:, :D]
     res.moment_count = S - burn - 1
-    res.final_state = q_cur[:, :D]
+    res.final_state = run.q_cur[:, :D]
     if nuts:
-        res.eps_bar, res.h_bar = eps_bar, h_bar
+        res.eps_bar, res.h_bar = run.eps_bar, run.h_bar
     if mass_out is not None:
         res.inv_mass_trace, res.mass_windows = mass_out
         res.inv_mass = res.inv_mass_trace[-1]
@@ -780,7 +792,7 @@ def hmc_run(target, params_init, num_samples, num_steps_per_sample, step_size, b
         a = res.swap_accepted
         tried = (a >= 0).sum(dim=(0, 1))
         res.swap_rate = (a == 1).sum(dim=(0, 1)).double() / tried.clamp_min(1).double()
-    res._keep_alive = keep_alive          # buffers the asynchronous kernel still reads
+    res._keep_alive = run.keep_alive      # buffers the asynchronous kernel still reads
     return res
 
 
@@ -789,16 +801,15 @@ def swap_rounds(num_samples, swap_every):
     return max(0, -(-int(num_samples) // int(swap_every)) - 1)
 
 
-def _tempered_launches(lib, nt, nm, rng, nuts_s, scheme, q_init, q_cur, eps, Cn, ld, L, S, burn, samples, accepted,
-                       diverged, ham, num_rejected, sink, temper, device, keep_alive):
+def _tempered_launches(run, nm, sink, temper):
     """hmc_run with replica exchange: the windows [k E, min(S, (k + 1) E)) of E = swap_every iterations, each a tempered
     sink launch (hmcx_split_run_temper) that leaves the untempered log-likelihood of every row in swap_ll[k], followed by
     swap round k (hmcx_temper_swap) when iterations remain.  All on the current stream, no host synchronisation.  Returns
     (betas (T,) fp64, swap_accepted (rounds, R, T - 1) int8, swap_ll (rounds, C) fp64)."""
     betas = [float(b) for b in temper['betas']]
     T, E = len(betas), int(temper['swap_every'])
-    R, rounds = Cn // T, swap_rounds(S, E)
-    tau0 = nt.mlp_desc.tau_out
+    R, rounds = run.Cn // T, swap_rounds(run.S, E)
+    tau0 = run.nt.mlp_desc.tau_out
     ts = N.TemperStruct()
     ts.num_temps = T
     for t, b in enumerate(betas):
@@ -807,33 +818,26 @@ def _tempered_launches(lib, nt, nm, rng, nuts_s, scheme, q_init, q_cur, eps, Cn,
     if sink_s is None:
         sink_s = N.SinkStruct()
         sink_s.thin = 1
-    swap_acc = torch.empty((rounds, R, T - 1), dtype=torch.int8, device=device)
-    swap_ll = torch.empty((rounds, Cn), dtype=torch.float64, device=device)
+    swap_acc = torch.empty((rounds, R, T - 1), dtype=torch.int8, device=run.device)
+    swap_ll = torch.empty((rounds, run.Cn), dtype=torch.float64, device=run.device)
     lu = temper.get('swap_log_uniforms')
     if lu is not None:
         if tuple(lu.shape) != (rounds, R, T - 1):
             raise ValueError('swap_log_uniforms must be (rounds, R, T - 1) = (%d, %d, %d), got %s'
                              % (rounds, R, T - 1, tuple(lu.shape)))
-        lu = lu.detach().to(device=device, dtype=torch.float64).contiguous()
+        lu = lu.detach().to(device=run.device, dtype=torch.float64).contiguous()
     srng = N.RngStruct()
     srng.mode = N.RNG_INJECTED if lu is not None else N.RNG_PHILOX
-    srng.seed, srng.chain_offset = rng.seed, rng.chain_offset
+    srng.seed, srng.chain_offset = run.rng.seed, run.rng.chain_offset
     cb = (C.c_double * T)(*betas)
-    keep_alive += [swap_acc, swap_ll, lu, ts, sink_s, srng, cb]
-    stream = N.stream_ptr(device)
+    run.keep_alive += [swap_acc, swap_ll, lu, ts, sink_s, srng, cb]
     for k in range(rounds + 1):
-        it0, it1 = k * E, min(S, (k + 1) * E)
-        r = _window_rng(rng, it0, Cn, ld, nt.num_splits)
-        keep_alive.append(r)
         ts.ll_out = swap_ll[k].data_ptr() if k < rounds else None
-        rc = lib.hmcx_split_run_temper(nt.ref(), nm.ref(), C.byref(r), C.byref(nuts_s), int(scheme), N.ptr(q_init),
-                                       N.ptr(q_cur), N.ptr(eps), Cn, ld, L, S, burn, it0, it1, N.ptr(samples),
-                                       N.ptr(accepted), N.ptr(diverged), N.ptr(ham), N.ptr(num_rejected),
-                                       C.byref(sink_s), C.byref(ts), stream)
-        N.check(rc, 'hmcx_split_run_temper')
+        _launch(run, k * E, min(run.S, (k + 1) * E), nm.ref(), sink_s, temper=ts)
         if k < rounds and T > 1:
-            rc = lib.hmcx_temper_swap(N.ptr(q_cur), Cn, ld, T, cb, N.ptr(swap_ll[k]), k, C.byref(srng),
-                                      None if lu is None else C.c_void_p(lu[k].data_ptr()), N.ptr(swap_acc[k]), stream)
+            rc = run.lib.hmcx_temper_swap(N.ptr(run.q_cur), run.Cn, run.ld, T, cb, N.ptr(swap_ll[k]), k, C.byref(srng),
+                                          None if lu is None else C.c_void_p(lu[k].data_ptr()), N.ptr(swap_acc[k]),
+                                          run.stream)
             N.check(rc, 'hmcx_temper_swap')
     return torch.tensor(betas, dtype=torch.float64), swap_acc, swap_ll
 
@@ -861,15 +865,42 @@ def _window_rng(rng, it0, Cn, ld, num_splits):
     return r
 
 
-def _adapted_launches(lib, nt, nm, rng, nuts_s, scheme, q_init, q_cur, eps, Cn, D, ld, L, S, burn, samples, accepted,
-                      diverged, ham, num_rejected, tuning, sink, h_bar, eps_bar, mass_pool, device, keep_alive,
-                      hyper_s=None):
+def _launch(run, it0, it1, mass_ref, sink, hyper=None, temper=None):
+    """Iterations [it0, it1) of ``run`` as one launch on the run's stream: the only call of a libhmcx run entry.  The
+    injected streams (and injected gamma draws) move to row it0; the per-launch struct copies join run.keep_alive.
+    Descriptor targets (``run.scheme`` None): hmcx_hmc_run_sink, ``sink`` None for a plain run.
+    Bayesian-NN targets: hmcx_split_run_folds for K-fold runs, hmcx_split_run_temper with ``temper``, else
+    hmcx_split_run_hyper (``sink`` and ``hyper`` may be None)."""
+    rng = _window_rng(run.rng, it0, run.Cn, run.ld, run.nt.num_splits)
+    h = None if hyper is None else _window_hyper(hyper, it0, run.Cn, 2 * run.nt.mlp_desc.num_layers + 1)
+    run.keep_alive += [rng, h]
+    head = (run.nt.ref(), mass_ref, C.byref(rng), C.byref(run.nuts))
+    sink = None if sink is None else C.byref(sink)
+    lib = run.lib
+    if run.scheme is None:
+        name = 'hmcx_hmc_run_sink'
+        rc = lib.hmcx_hmc_run_sink(*head, *run.args(it0, it1), run.tuning, N.ptr(run.ws), sink, run.stream)
+    elif run.num_folds:
+        name = 'hmcx_split_run_folds'
+        rc = lib.hmcx_split_run_folds(*head, int(run.scheme), *run.args(it0, it1), sink, run.num_folds, run.stream)
+    elif temper is not None:
+        name = 'hmcx_split_run_temper'
+        rc = lib.hmcx_split_run_temper(*head, int(run.scheme), *run.args(it0, it1), sink, C.byref(temper), run.stream)
+    else:
+        name = 'hmcx_split_run_hyper'
+        rc = lib.hmcx_split_run_hyper(*head, int(run.scheme), *run.args(it0, it1), sink, None if h is None else C.byref(h),
+                                      run.stream)
+    N.check(rc, name)
+
+
+def _adapted_launches(run, nm, sink, hyper_s, mass_pool):
     """hmc_run with adapt_mass: [0, a_1) and every window [a_k, b_k) of mass_windows(burn), each window followed by
     hmcx_adapt_diag_mass, then [b_K, S) with the caller's sink (and the hyperprior state ``hyper_s``, if any).  Every launch is a sink launch (mu_chain and moments_all
     are read by the sink forms only); the launches chain through q_cur, eps, the dual-averaging state and, for element-wise
     targets, the log p workspace.  Returns (inv_mass_trace (K, D), windows)."""
-    windows = mass_windows(burn)
+    windows = mass_windows(run.burn)
     K = len(windows)
+    Cn, ld, device = run.Cn, run.ld, run.device
     trace = torch.zeros((K, ld), dtype=torch.float32, device=device)          # row k: inv_mass after window k
     factor = torch.zeros((K, ld), dtype=torch.float32, device=device)         # row k: its sqrt(1 / inv_mass)
     acc = [torch.zeros((Cn, ld), dtype=torch.float32, device=device) for _ in range(4)]
@@ -883,32 +914,13 @@ def _adapted_launches(lib, nt, nm, rng, nuts_s, scheme, q_init, q_cur, eps, Cn, 
         m = N.MassStruct()
         m.kind, m.inv_mass, m.mass_factor = N.MASS_DIAG, trace[k].data_ptr(), factor[k].data_ptr()
         masses.append(m)
-    keep_alive += [trace, factor, mu_chain, wsink, masses] + acc
-    ws = None
-    if scheme is None:
-        ws_bytes = lib.hmcx_hmc_workspace_bytes(nt.ref(), nm.ref(), Cn, ld)
-        ws = torch.empty(ws_bytes // 4, dtype=torch.float32, device=device) if ws_bytes else None
-        keep_alive.append(ws)
-    stream = N.stream_ptr(device)
+    run.keep_alive += [trace, factor, mu_chain, wsink, masses] + acc
+    if run.scheme is None:
+        run.keep_alive.append(run.ws)
 
     def launch(it0, it1, mass_ref, sink_s, per_chain_mu):
-        nuts_s.mu_chain = mu_chain.data_ptr() if per_chain_mu else None
-        r = _window_rng(rng, it0, Cn, ld, nt.num_splits)
-        keep_alive.append(r)
-        if scheme is None:
-            rc = lib.hmcx_hmc_run_sink(nt.ref(), mass_ref, C.byref(r), C.byref(nuts_s), N.ptr(q_init), N.ptr(q_cur),
-                                       N.ptr(eps), Cn, ld, L, S, burn, it0, it1, N.ptr(samples), N.ptr(accepted),
-                                       N.ptr(diverged), N.ptr(ham), N.ptr(num_rejected), tuning, N.ptr(ws),
-                                       C.byref(sink_s), stream)
-            N.check(rc, 'hmcx_hmc_run_sink')
-        else:
-            h = _window_hyper(hyper_s, it0, Cn, 2 * nt.mlp_desc.num_layers + 1)
-            keep_alive.append(h)
-            rc = lib.hmcx_split_run_hyper(nt.ref(), mass_ref, C.byref(r), C.byref(nuts_s), int(scheme), N.ptr(q_init),
-                                          N.ptr(q_cur), N.ptr(eps), Cn, ld, L, S, burn, it0, it1, N.ptr(samples),
-                                          N.ptr(accepted), N.ptr(diverged), N.ptr(ham), N.ptr(num_rejected),
-                                          C.byref(sink_s), None if h is None else C.byref(h), stream)
-            N.check(rc, 'hmcx_split_run_hyper')
+        run.nuts.mu_chain = mu_chain.data_ptr() if per_chain_mu else None
+        _launch(run, it0, it1, mass_ref, sink_s, hyper_s)
 
     mass_ref = nm.ref()
     launch(0, windows[0][0], mass_ref, sink, False)
@@ -916,17 +928,17 @@ def _adapted_launches(lib, nt, nm, rng, nuts_s, scheme, q_init, q_cur, eps, Cn, 
         launch(a, b, mass_ref, wsink, k > 0)
         sums = acc if mass_pool is None else [mass_pool(t).contiguous() for t in acc]
         if mass_pool is not None:
-            keep_alive.extend(sums)
-        rc = lib.hmcx_adapt_diag_mass(*(N.ptr(t) for t in sums), sums[0].shape[0], ld, D, b - a, N.ptr(eps), Cn,
-                                      N.ptr(trace[k]), N.ptr(factor[k]), N.ptr(mu_chain), N.ptr(h_bar), N.ptr(eps_bar),
-                                      stream)
+            run.keep_alive.extend(sums)
+        rc = run.lib.hmcx_adapt_diag_mass(*(N.ptr(t) for t in sums), sums[0].shape[0], ld, run.D, b - a, N.ptr(run.eps),
+                                          Cn, N.ptr(trace[k]), N.ptr(factor[k]), N.ptr(mu_chain), N.ptr(run.h_bar),
+                                          N.ptr(run.eps_bar), run.stream)
         N.check(rc, 'hmcx_adapt_diag_mass')
         if mass_pool is not None:                  # the kernel zeroed the gathered copies; the next window starts from zero
             for t in acc:
                 t.zero_()
         mass_ref = C.byref(masses[k])
-    launch(windows[-1][1], S, mass_ref, sink, True)
-    return trace[:, :D], windows
+    launch(windows[-1][1], run.S, mass_ref, sink, True)
+    return trace[:, :run.D], windows
 
 
 def hyper_gamma_draws(seed, num_chains, iter_begin, iter_end, shapes, chain_offset=0, device='cuda'):
@@ -1051,81 +1063,40 @@ def rmhmc_run(target, params_init, num_samples, num_steps_per_sample, step_size,
     Injected (parity) mode: ``normals`` (S, C, D), ``log_uniforms`` (S, C) and -- when ``jitter`` is not None --
     ``uniforms`` (S, C, J, D): the ``torch.rand(D)`` jitter draws of every ``fisher`` call of iteration n in the
     reference's order (J = 8*L+3 for the explicit integrator)."""
-    N.require_cuda()
-    lib = N.load_library()
-    if device is None:
-        device = params_init.device if params_init.is_cuda else torch.device('cuda', torch.cuda.current_device())
-    device = torch.device(device)
+    device = _run_device(params_init, device)
     nt = native_target(target, device)
-    D, ld = nt.dim, N.padded_ld(nt.dim)
-    S, L, burn = int(num_samples), int(num_steps_per_sample), int(burn)
-    q_init = _as_rows(params_init, ld, device)
-    Cn = q_init.shape[0]
-    q_cur = q_init.clone()
     if explicit and torch.is_tensor(step_size) and step_size.numel() > 1:
         s = step_size.detach().reshape(-1)
         if not bool((s == s[0]).all()):
             # every kernel applies ONE binding rotation c, s = cos/sin(2 * omega * step_size) (:435-436) to all chains
             raise NotImplementedError('the explicit RMHMC integrator takes one step size for all chains')
-    eps = _eps_vector(step_size, Cn, device)
-    samples = torch.empty((Cn, S - burn, ld), dtype=torch.float32, device=device)
-    accepted = torch.empty((Cn, S), dtype=torch.uint8, device=device)
-    diverged = torch.empty((Cn, S), dtype=torch.uint8, device=device)
-    ham = torch.empty((Cn, S, 2), dtype=torch.float32, device=device) if record_ham else None
-    num_rejected = torch.zeros(Cn, dtype=torch.int32, device=device)
+    run = _Run(nt, params_init, num_samples, num_steps_per_sample, step_size, burn, record_ham, device)
+    D, ld, Cn, S, burn = run.D, run.ld, run.Cn, run.S, run.burn
+    run.samples = torch.empty((Cn, S - burn, ld), dtype=torch.float32, device=device)
     if softabs and softabs_const is None:
         raise RuntimeError('Metric.SOFTABS needs softabs_const')
 
     cfg = _rmhmc_cfg(D, step_size, jitter, softabs_const, explicit_binding_const, fixed_point_threshold,
                      fixed_point_max_iterations, jitter_max_tries, explicit, softabs, jacdiag)
-
-    rng = N.RngStruct()
-    keep_alive = []
-    if normals is not None:
-        z = normals.detach().to(device=device, dtype=torch.float32)
-        if z.dim() == 2:
-            z = z.unsqueeze(1)
-        if tuple(z.shape) != (S, Cn, D):
-            raise RuntimeError('normals must be (S, C, D) = (%d, %d, %d), got %s' % (S, Cn, D, tuple(z.shape)))
-        z = N.pad_rows(z.contiguous(), ld)
-        lu = log_uniforms.detach().to(device=device, dtype=torch.float32).reshape(S, Cn).contiguous()
-        rng.mode, rng.normals, rng.log_uniforms = N.RNG_INJECTED, z.data_ptr(), lu.data_ptr()
-        keep_alive += [z, lu]
-        if jitter is not None:
-            if uniforms is None:
-                raise RuntimeError('injected RMHMC with jitter needs the uniforms stream')
-            u = uniforms.detach().to(device=device, dtype=torch.float32)
-            if u.dim() == 3:
-                u = u.unsqueeze(1)
-            if u.dim() != 4 or tuple(u.shape[:2]) != (S, Cn) or u.shape[3] != D:
-                raise RuntimeError('uniforms must be (S, C, J, D) = (%d, %d, J, %d), got %s'
-                                   % (S, Cn, D, tuple(u.shape)))
-            u = N.pad_rows(u.contiguous(), ld)
-            rng.uniforms, rng.uniforms_per_iter = u.data_ptr(), u.shape[2]
-            keep_alive.append(u)
-    else:
-        rng.mode, rng.seed, rng.chain_offset = N.RNG_PHILOX, int(seed), int(chain_offset)
+    rng = run.rng = _rng_struct(run, seed, chain_offset, normals, log_uniforms, uniforms=uniforms,
+                                jitter=jitter is not None)
     with torch.cuda.device(device):
         if _rmhmc_is_dense(nt.target, jitter, jacdiag):
             ginv_d, lower_d, log_det = const_metric_device(nt.target, softabs, softabs_const, device)
             gm = N.ConstMetricStruct()
             gm.metric_inv, gm.metric_chol, gm.log_det = ginv_d.data_ptr(), lower_d.data_ptr(), log_det
-            ws = torch.empty(lib.hmcx_rmhmc_dense_workspace_bytes(Cn, D) // 4, dtype=torch.float32, device=device)
-            keep_alive += [ginv_d, lower_d, ws]
-            rc = lib.hmcx_rmhmc_dense_run(nt.ref(), C.byref(cfg), C.byref(gm), C.byref(rng), N.ptr(q_init),
-                                          N.ptr(q_cur), N.ptr(eps), Cn, ld, L, S, burn, 0, S, N.ptr(samples),
-                                          N.ptr(accepted), N.ptr(diverged), N.ptr(ham), N.ptr(num_rejected),
-                                          N.ptr(ws), N.stream_ptr(device))
+            ws = torch.empty(run.lib.hmcx_rmhmc_dense_workspace_bytes(Cn, D) // 4, dtype=torch.float32, device=device)
+            run.keep_alive += [ginv_d, lower_d, ws]
+            rc = run.lib.hmcx_rmhmc_dense_run(nt.ref(), C.byref(cfg), C.byref(gm), C.byref(rng), *run.args(0, S),
+                                              N.ptr(ws), run.stream)
             N.check(rc, 'hmcx_rmhmc_dense_run')
         else:
-            rc = lib.hmcx_rmhmc_run(nt.ref(), C.byref(cfg), C.byref(rng), N.ptr(q_init), N.ptr(q_cur), N.ptr(eps), Cn,
-                                    ld, L, S, burn, 0, S, N.ptr(samples), N.ptr(accepted), N.ptr(diverged), N.ptr(ham),
-                                    N.ptr(num_rejected), N.stream_ptr(device))
+            rc = run.lib.hmcx_rmhmc_run(nt.ref(), C.byref(cfg), C.byref(rng), *run.args(0, S), run.stream)
             N.check(rc, 'hmcx_rmhmc_run')
-    res = HMCResult(samples, accepted, diverged, ham, eps, num_rejected, D, S)
+    res = HMCResult(run.samples, run.accepted, run.diverged, run.ham, run.eps, run.num_rejected, D, S)
     res.eps_trace = None
-    res.final_state = q_cur[:, :D]
-    res._keep_alive = keep_alive
+    res.final_state = run.q_cur[:, :D]
+    res._keep_alive = run.keep_alive
     return res
 
 

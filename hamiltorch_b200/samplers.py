@@ -275,6 +275,50 @@ def _draw_reference_stream(dim, num_samples, device, num_perm=0, blocks=None, ga
     return out + ((gam,) if gam is not None else ())
 
 
+def _draw_rmhmc_reference_stream(dim, num_samples, L, jitter, explicit, device):
+    """``_draw_reference_stream`` for sampler=RMHMC, as engine.rmhmc_run's ``normals`` / ``log_uniforms`` / ``uniforms``:
+    with ``jitter``, the J = 8 L + 3 ``torch.rand(D)`` draws of the explicit integrator's ``fisher`` calls interleave
+    with each iteration's momentum normals."""
+    if jitter is not None and not explicit:
+        raise NotImplementedError(
+            "implicit RMHMC with jitter draws a data-dependent number of uniforms per iteration; its "
+            "reference stream cannot be pre-drawn -- use rng='philox'")
+    J = (8 * L + 3) if jitter is not None else 0
+    z = torch.empty((num_samples, dim), dtype=torch.float32, device=device)
+    logu = torch.empty(num_samples, dtype=torch.float32)
+    uni = torch.zeros((num_samples, max(J, 1), dim), dtype=torch.float32)
+    for n in range(num_samples):                     # fisher's rand(D) (:115) is always CPU, gibbs first (:184)
+        if J:
+            uni[n, 0] = torch.rand(dim)
+        z[n] = torch.randn(dim, dtype=torch.float32, device=device)
+        for j in range(1, J):
+            uni[n, j] = torch.rand(dim)
+        logu[n] = torch.log(torch.rand(1))[0]
+    return dict(normals=z.unsqueeze(1), log_uniforms=logu.unsqueeze(1), uniforms=uni.unsqueeze(1) if J else None)
+
+
+def _stream_args(rng, q0, seed, normals, log_uniforms, injected, draw_reference):
+    """The random stream of a run as engine.hmc_run / rmhmc_run keyword arguments.  rng='reference': one chain replaying
+    torch's global generators, pre-drawn by ``draw_reference()``; 'injected': ``normals`` and ``log_uniforms`` (both
+    required) with the sampler family's other streams ``injected``; 'philox': the in-kernel stream keyed by ``seed``
+    (None: drawn from torch's RNG)."""
+    if rng == 'reference':
+        if q0.shape[0] != 1:
+            raise RuntimeError("rng='reference' replays torch's global stream and is defined for one chain")
+        stream = draw_reference()
+    elif rng == 'injected':
+        if normals is None or log_uniforms is None:
+            raise RuntimeError("rng='injected' needs normals and log_uniforms")
+        stream = dict(injected, normals=normals, log_uniforms=log_uniforms)
+    elif rng == 'philox':
+        if seed is None:
+            seed = int(torch.randint(0, 2 ** 62, (1,)))
+        stream = dict(normals=None, log_uniforms=None)
+    else:
+        raise ValueError('unknown rng mode %r' % (rng,))
+    return dict(stream, seed=seed or 0)
+
+
 def sample(log_prob_func, params_init, num_samples=10, num_steps_per_sample=10, step_size=0.1, burn=0, jitter=None,
            inv_mass=None, normalizing_const=1., softabs_const=None, explicit_binding_const=100,
            fixed_point_threshold=1e-5, fixed_point_max_iterations=1000, jitter_max_tries=10, sampler=Sampler.HMC,
@@ -613,37 +657,12 @@ def _run_chains(log_prob_func, q0, num_samples, L, step_size, burn, jitter, inv_
     if sampler == Sampler.HMC and integrator not in _SPLIT_INTEGRATORS:
         if isinstance(log_prob_func, list):
             raise NotImplementedError('a list log_prob_func needs a SPLITTING integrator')
+        scheme = N.SCHEME_PLAIN if isinstance(log_prob_func, T.MLPRegression) else None
         D = log_prob_func.dim
-        if q0.shape[1] != D:
-            raise RuntimeError('params_init has %d entries, the target has %d' % (q0.shape[1], D))
-        if rng == 'reference':
-            if q0.shape[0] != 1:
-                raise RuntimeError("rng='reference' replays torch's global stream and is defined for one chain")
-            drawn = _draw_reference_stream(D, num_samples, q0.device, gamma_shapes=gshapes,
-                                           blocks=[b.shape[0] for b in inv_mass] if isinstance(inv_mass, list) else None)
-            z, logu = drawn[0], drawn[1]
-            normals, log_uniforms = z.unsqueeze(1), logu.unsqueeze(1)
-            if hyper is not None:
-                gammas = drawn[-1].unsqueeze(1)
-        elif rng == 'injected':
-            if normals is None or log_uniforms is None:
-                raise RuntimeError("rng='injected' needs normals and log_uniforms")
-        elif rng == 'philox':
-            normals = log_uniforms = None
-            if seed is None:
-                seed = int(torch.randint(0, 2 ** 62, (1,)))
-        else:
-            raise ValueError('unknown rng mode %r' % (rng,))
-        return engine.hmc_run(log_prob_func, q0, num_samples, L, step_size, burn=burn, inv_mass=inv_mass, nuts=nuts,
-                              desired_accept_rate=desired_accept_rate, seed=seed or 0, chain_offset=chain_offset,
-                              normals=normals, log_uniforms=log_uniforms, record_ham=record_ham, out=out,
-                              scheme=N.SCHEME_PLAIN if isinstance(log_prob_func, T.MLPRegression) else None,
-                              gammas=gammas, **hyper_kw, **sink)
-    if sampler == Sampler.HMC:
+    elif sampler == Sampler.HMC:
         if type(log_prob_func) is not list:
             raise RuntimeError('For splitting log_prob_func must be list of functions')            # :466-467
-        M = len(log_prob_func)
-        if M == 1 and integrator in (Integrator.SPLITTING, Integrator.SPLITTING_KMID):
+        if len(log_prob_func) == 1 and integrator in (Integrator.SPLITTING, Integrator.SPLITTING_KMID):
             raise RuntimeError('For symmetric splitting log_prob_func must be list of functions greater than '
                                'length 1')                                                          # :497-498, :577-578
         if isinstance(inv_mass, list):
@@ -652,95 +671,55 @@ def _run_chains(log_prob_func, q0, num_samples, L, step_size, burn, jitter, inv_
         scheme = {Integrator.SPLITTING: N.SCHEME_SPLIT_SYM, Integrator.SPLITTING_RAND: N.SCHEME_SPLIT_RAND,
                   Integrator.SPLITTING_KMID: N.SCHEME_SPLIT_KMID}[integrator]
         D = log_prob_func[0].dim
-        if q0.shape[1] != D:
-            raise RuntimeError('params_init has %d entries, the target has %d' % (q0.shape[1], D))
-        perms = None
-        if rng == 'reference':
-            if q0.shape[0] != 1:
-                raise RuntimeError("rng='reference' replays torch's global stream and is defined for one chain")
-            rand_perm = integrator == Integrator.SPLITTING_RAND
-            drawn = _draw_reference_stream(D, num_samples, q0.device, M if rand_perm else 0, gamma_shapes=gshapes)
-            z, logu, pm = drawn[0], drawn[1], (drawn[2] if rand_perm else None)
-            if hyper is not None:
-                gammas = drawn[-1].unsqueeze(1)
-            normals, log_uniforms = z.unsqueeze(1), logu.unsqueeze(1)
-            perms = None if pm is None else pm.unsqueeze(1)
-        elif rng == 'injected':
-            if normals is None or log_uniforms is None:
-                raise RuntimeError("rng='injected' needs normals and log_uniforms")
-            perms = injected_perms
-        elif rng == 'philox':
-            normals = log_uniforms = None
-            if seed is None:
-                seed = int(torch.randint(0, 2 ** 62, (1,)))
-        else:
-            raise ValueError('unknown rng mode %r' % (rng,))
-        return engine.hmc_run(log_prob_func, q0, num_samples, L, step_size, burn=burn, inv_mass=inv_mass, nuts=nuts,
-                              desired_accept_rate=desired_accept_rate, seed=seed or 0, chain_offset=chain_offset,
-                              normals=normals, log_uniforms=log_uniforms, record_ham=record_ham, out=out,
-                              scheme=scheme, perms=perms, gammas=gammas, **hyper_kw, **sink)
-    if hyper is not None:
-        raise NotImplementedError('hyperpriors on tau_list / tau_out: sampler HMC or HMC_NUTS')
-    if sampler == Sampler.RMHMC and integrator in (Integrator.EXPLICIT, Integrator.IMPLICIT):
+    else:
+        if hyper is not None:
+            raise NotImplementedError('hyperpriors on tau_list / tau_out: sampler HMC or HMC_NUTS')
+        if sampler != Sampler.RMHMC or integrator not in (Integrator.EXPLICIT, Integrator.IMPLICIT):
+            raise NotImplementedError()                                                             # :606, :844
         if isinstance(log_prob_func, list) or not isinstance(log_prob_func, (T.Funnel, T.GaussianIso, T.GaussianDiag,
                                                                              T.GaussianFull)):
             raise NotImplementedError('RMHMC needs closed-form third derivatives: Funnel / Gaussian descriptors')
         jacdiag = metric == Metric.JACOBIAN_DIAG
         if metric not in (Metric.HESSIAN, Metric.SOFTABS, Metric.JACOBIAN_DIAG):
             raise NotImplementedError()
-        Dd = log_prob_func.dim
+        D = log_prob_func.dim
         const_metric = jitter is None and not jacdiag and isinstance(log_prob_func, (T.GaussianIso, T.GaussianDiag,
                                                                                      T.GaussianFull))
-        if Dd > 64 and not const_metric:
+        if D > 64 and not const_metric:
             raise NotImplementedError('RMHMC with a position-dependent or jittered metric: D <= 64 (metric, eigenvectors '
                                       'and one work matrix in shared memory); Gaussian targets with jitter=None run on '
                                       'the constant-metric tensor-core path at any D')
         if inv_mass is not None:
             pass                                            # the reference ignores inv_mass for RMHMC (:989 comment)
-        D = log_prob_func.dim
-        if q0.shape[1] != D:
-            raise RuntimeError('params_init has %d entries, the target has %d' % (q0.shape[1], D))
+    if q0.shape[1] != D:
+        raise RuntimeError('params_init has %d entries, the target has %d' % (q0.shape[1], D))
+    if sampler == Sampler.RMHMC:
         explicit = integrator == Integrator.EXPLICIT
-        uniforms = None
-        if rng == 'reference':
-            if q0.shape[0] != 1:
-                raise RuntimeError("rng='reference' replays torch's global stream and is defined for one chain")
-            if jitter is not None and not explicit:
-                raise NotImplementedError(
-                    "implicit RMHMC with jitter draws a data-dependent number of uniforms per iteration; its "
-                    "reference stream cannot be pre-drawn -- use rng='philox'")
-            J = (8 * L + 3) if jitter is not None else 0
-            z = torch.empty((num_samples, D), dtype=torch.float32, device=q0.device)
-            logu = torch.empty(num_samples, dtype=torch.float32)
-            uni = torch.zeros((num_samples, max(J, 1), D), dtype=torch.float32)
-            for n in range(num_samples):                     # fisher's rand(D) (:115) is always CPU, gibbs first (:184)
-                if J:
-                    uni[n, 0] = torch.rand(D)
-                z[n] = torch.randn(D, dtype=torch.float32, device=q0.device)
-                for j in range(1, J):
-                    uni[n, j] = torch.rand(D)
-                logu[n] = torch.log(torch.rand(1))[0]
-            normals, log_uniforms = z.unsqueeze(1), logu.unsqueeze(1)
-            uniforms = uni.unsqueeze(1) if J else None
-        elif rng == 'injected':
-            if normals is None or log_uniforms is None:
-                raise RuntimeError("rng='injected' needs normals and log_uniforms")
-            uniforms = injected_uniforms
-        elif rng == 'philox':
-            normals = log_uniforms = None
-            if seed is None:
-                seed = int(torch.randint(0, 2 ** 62, (1,)))
-        else:
-            raise ValueError('unknown rng mode %r' % (rng,))
+        stream = _stream_args(rng, q0, seed, normals, log_uniforms, dict(uniforms=injected_uniforms),
+                              lambda: _draw_rmhmc_reference_stream(D, num_samples, L, jitter, explicit, q0.device))
         return engine.rmhmc_run(log_prob_func, q0, num_samples, L, step_size, burn=burn, jitter=jitter,
                                 softabs_const=softabs_const, explicit_binding_const=explicit_binding_const,
                                 fixed_point_threshold=fixed_point_threshold,
                                 fixed_point_max_iterations=fixed_point_max_iterations,
                                 jitter_max_tries=jitter_max_tries, explicit=explicit,
-                                softabs=(metric == Metric.SOFTABS), jacdiag=jacdiag, seed=seed or 0,
-                                chain_offset=chain_offset,
-                                normals=normals, log_uniforms=log_uniforms, uniforms=uniforms, record_ham=record_ham)
-    raise NotImplementedError()                                                                     # :606, :844
+                                softabs=(metric == Metric.SOFTABS), jacdiag=jacdiag, chain_offset=chain_offset,
+                                record_ham=record_ham, **stream)
+
+    num_perm = len(log_prob_func) if integrator == Integrator.SPLITTING_RAND else 0
+
+    def draw_reference():
+        drawn = _draw_reference_stream(D, num_samples, q0.device, num_perm, gamma_shapes=gshapes,
+                                       blocks=[b.shape[0] for b in inv_mass] if isinstance(inv_mass, list) else None)
+        return dict(normals=drawn[0].unsqueeze(1), log_uniforms=drawn[1].unsqueeze(1),
+                    perms=drawn[2].unsqueeze(1) if num_perm else None,
+                    gammas=drawn[-1].unsqueeze(1) if hyper is not None else None)
+
+    stream = _stream_args(rng, q0, seed, normals, log_uniforms,
+                          dict(perms=injected_perms if integrator in _SPLIT_INTEGRATORS else None, gammas=gammas),
+                          draw_reference)
+    return engine.hmc_run(log_prob_func, q0, num_samples, L, step_size, burn=burn, inv_mass=inv_mass, nuts=nuts,
+                          desired_accept_rate=desired_accept_rate, chain_offset=chain_offset, record_ham=record_ham,
+                          out=out, scheme=scheme, **stream, **hyper_kw, **sink)
 
 
 # ----------------------------------------------------------------------------------------------------------
